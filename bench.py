@@ -5,6 +5,7 @@ shapes (BASELINE.json).  One JSON line on stdout (rank 0).
     python bench.py --gpus 1 --steps 10 --warmup 3                       # ogbn-products-shaped, bf16, full batch (config 3)
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...   # rank-local graph partitions + grad allreduce
     python bench.py --impl reference                                     # the reference's CPU path (oracle port) on host cores
+    python bench.py --steps 10 --warmup 3 --dump-outputs DIR             # + DIR/*.npy: what the last timed step computed
 
 Timed region: device-timed with CUDA events on the launching stream, barrier + synchronize on both sides, max over
 ranks.  `value` has the inputs resident in HBM; `e2e` copies the step's inputs from pinned host memory every step
@@ -61,7 +62,19 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
+
+
+def gpu_info(index):
+    """Name and power limit of the measuring GPU: a time means little without them (a card may be capped below 700 W)."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return info
 
 
 class ClockSampler:
@@ -105,6 +118,29 @@ class ClockSampler:
         if not sm:
             return None
         return {"sm_mhz": statistics.median(sm), "sm_max_mhz": max(mx), "reasons": sorted(reasons), "samples": len(sm)}
+
+
+DUMP_ROWS = 65536      # logits rows sampled into --dump-outputs (fixed seed): 65536 x 172 classes x 4 B = 45 MB at most
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(path, out, loss, model):
+    """Write what the timed step computed in its last call, as DIR/<name>.npy (float32; row indices float64): the loss, the
+    logits of a fixed seeded sample of rows (all rows when there are fewer) and every parameter after the optimizer step."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    n = out.shape[0]
+    rows = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:DUMP_ROWS].sort().values
+    arrays = {"loss": loss.detach().float().reshape(1).cpu().numpy(),
+              "logits_sample": out.detach()[rows.to(out.device)].float().cpu().numpy(),
+              "logits_sample_rows": rows.numpy().astype(np.float64)}
+    for name, prm in model.named_parameters():
+        arrays["param." + name] = prm.detach().float().cpu().numpy()
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_MAX_BYTES:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed {DUMP_MAX_BYTES}")
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def spmm_algorithmic_bytes(n, nnz, h, b):
@@ -261,9 +297,10 @@ def _optimizer(model, graph_capturable=True):
 
 
 def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_roofline=False, use_graph=True, rmat=False,
-                   solo=False, sample_clocks=False):
+                   solo=False, sample_clocks=False, dump_dir=None):
     """One full-batch measurement.  parallel: 'single' | 'dp' | 'rows'.  solo=True: rank 0 alone (a single-GPU baseline taken
-    inside a multi-rank job; the other ranks return None and wait at the caller's barrier)."""
+    inside a multi-rank job; the other ranks return None and wait at the caller's barrier).  dump_dir: rank 0 writes the
+    outputs of the last timed step there (dump_outputs)."""
     from sgformer_b200 import kernels as K
     from sgformer_b200 import large as L
     from sgformer_b200.graph import clear_cache, get_graph
@@ -317,6 +354,8 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
                 p.grad.copy_(flat[o:o + k].view_as(p.grad))
                 o += k
 
+    last = {}      # logits and loss of the latest step (inside a captured graph: the graph's output buffers)
+
     def step(xd, eid, yd):
         opt.zero_grad(set_to_none=True)
         out = model(xd, eid)
@@ -324,6 +363,7 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
         loss.backward()
         allreduce_grads()
         opt.step()
+        last.update(out=out.detach(), loss=loss.detach())     # detached: must not keep the step's autograd graph alive
         return loss
 
     for _ in range(warmup):
@@ -345,6 +385,7 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
             cg = torch.cuda.CUDAGraph()
             with torch.cuda.graph(cg):
                 step(x, ei, y)
+            captured = dict(last)
         except Exception as exc:  # pragma: no cover
             print(f"[bench] CUDA graph capture failed ({type(exc).__name__}: {exc}); running eagerly", file=sys.stderr)
             cg = None
@@ -369,6 +410,8 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
         step(x, ei, y)
         per_step = K.launch_count() - l0
         ms_step = ctx.timed(run_step, steps, world)
+        if dump_dir and rank == 0:
+            dump_outputs(dump_dir, captured["out"], captured["loss"], model)
         launches = per_step * steps
         if want_roofline:
             # SpMM launch durations for the roofline: a few eager steps with CUDA events around each SpMM launch
@@ -378,6 +421,8 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
     else:
         K.spmm_events = [] if want_roofline else None
         ms_step = ctx.timed(run_step, steps, world)
+        if dump_dir and rank == 0:
+            dump_outputs(dump_dir, last["out"], last["loss"], model)
         launches = K.launch_count() - l0
         ev, K.spmm_events = (K.spmm_events or []), None
     clocks = sampler.stop() if sampler else None
@@ -418,10 +463,10 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
         timed_steps = 2 if used_graph else steps
         res["roofline"] = {"kernel": "spmm_rows_kernel (CSR SpMM fwd + transposed bwd)", "bound": "hbm", "achieved": achieved,
                            "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                           # dram__bytes of this exact launch are only known from an ncu capture (profiles/): not measured live
+                           # dram__bytes of this exact launch are only known from a profiler capture: not measured live
                            "traffic": None, "peak_source": peak_src, "algorithmic_bytes_per_launch": alg,
                            "avg_launch_ms": avg_ms, "launches_timed": len(spmm_ms),
-                           "share_of_step": avg_ms * (len(spmm_ms) / timed_steps) / ms_step, "frac_of_nominal_8TBs": achieved / 8000.0}
+                           "share_of_step": avg_ms * (len(spmm_ms) / timed_steps) / ms_step}
     del model, opt, x, y, ei, graph, params
     clear_cache()
     gc.collect()
@@ -429,7 +474,7 @@ def run_full_batch(ctx, wname, w, parallel, steps, warmup, want_e2e=False, want_
     return res
 
 
-def run_minibatch(ctx, w, steps, warmup, solo=False):
+def run_minibatch(ctx, w, steps, warmup, solo=False, dump_dir=None):
     """papers100M-shaped random-partition mini-batches (large/main-batch.py:130-151) kept on the device: CSR built once, per step a
     random batch -> Graph.subset (K9 on the CSR) -> feature gather -> fwd/bwd -> (grad all-reduce) -> Adam."""
     from sgformer_b200 import kernels as K
@@ -461,6 +506,7 @@ def run_minibatch(ctx, w, steps, warmup, solo=False):
     cap = int(bsz * (2.0 * w["e"] / n * bsz / n + 1.0) * 1.5) + 1024     # induced nnz bound: no per-batch device sync
     sampler = RandomPartitionSampler(full, x, y, bsz, capacity=cap, generator=torch.Generator(device=dev).manual_seed(11 + sr))
     batches = iter(())
+    last = {}
 
     def mb_step():
         nonlocal batches
@@ -469,7 +515,8 @@ def run_minibatch(ctx, w, steps, warmup, solo=False):
             batches = iter(sampler)
             mb = next(batches)
         opt.zero_grad(set_to_none=True)
-        loss = nll_loss_from_logits(model(mb), mb.labels, None, float(bsz))
+        out = model(mb)
+        loss = nll_loss_from_logits(out, mb.labels, None, float(bsz))
         loss.backward()
         if world > 1:
             flat = torch.cat([p.grad.reshape(-1) for p in params if p.grad is not None])
@@ -482,12 +529,15 @@ def run_minibatch(ctx, w, steps, warmup, solo=False):
                     p.grad.copy_(flat[o:o + k].view_as(p.grad))
                     o += k
         opt.step()
+        last.update(out=out.detach(), loss=loss.detach())     # detached: must not keep the step's autograd graph alive
         return loss
 
     for _ in range(warmup):
         mb_step()
     l0 = K.launch_count()
     ms_step = ctx.timed(mb_step, steps, world)
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, last["out"], last["loss"], model)
     launches = K.launch_count() - l0
     sampler.check()         # a batch whose induced subgraph exceeded `cap` would have been truncated: fail loudly
     res = dict(ms_per_step=ms_step, value=bsz * world / (ms_step * 1e-3), launches=launches, nnz=full.nnz, world=world, n=n, batch=bsz)
@@ -624,6 +674,9 @@ def main():
     ap.add_argument("--extras-child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--rmat", action="store_true", help="power-law R-MAT edges instead of uniform (secondary, not graded)")
     ap.add_argument("--no-graph", action="store_true", help="do not capture the training step in a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what the last one computed (loss, sampled logits, updated parameters) "
+                         "as DIR/<name>.npy")
     ap.add_argument("--parallel", default="dp", choices=["dp", "rows"],
                     help="N>1: 'dp' = rank-local graph partitions + gradient all-reduce (weak scaling); 'rows' = ONE graph, "
                          "nodes row-sharded, K^T V / BN all-reduces + SpMM operand all-gather (strong scaling)")
@@ -647,7 +700,7 @@ def main():
         return
 
     if "batch" in w:
-        r = run_minibatch(ctx, w, args.steps, args.warmup)
+        r = run_minibatch(ctx, w, args.steps, args.warmup, dump_dir=args.dump_outputs)
         if rank == 0:
             line = {"metric": "nodes/sec fwd+bwd", "value": r["value"], "unit": "nodes/s", "n_gpus": world,
                     "steps": args.steps, "warmup": args.warmup, "ms_per_step": r["ms_per_step"], "higher_is_better": True,
@@ -659,7 +712,8 @@ def main():
                                f"dp{world}: rank-local node shards, replicated model, NCCL grad allreduce",
                                "step": "sample batch + Graph.subset (K9 on CSR) + feature gather + fwd + fused loss + bwd + Adam",
                                "cuda_graph": False},
-                    "e2e": None, "gpu_launches": r["launches"], "clocks": None, "roofline": None, "cpu_baseline": None}
+                    "e2e": None, "gpu_launches": r["launches"], "clocks": None, "roofline": None, "cpu_baseline": None,
+                    "gpu": gpu_info(ctx.local)}
             print(json.dumps(line), flush=True)
         if world > 1:
             ctx.dist.destroy_process_group()
@@ -667,7 +721,7 @@ def main():
 
     par = "single" if world == 1 else args.parallel
     r = run_full_batch(ctx, args.workload, w, par, args.steps, args.warmup, want_e2e=not args.no_e2e, want_roofline=True,
-                       use_graph=not args.no_graph, rmat=args.rmat, sample_clocks=True)
+                       use_graph=not args.no_graph, rmat=args.rmat, sample_clocks=True, dump_dir=args.dump_outputs)
     ctx.barrier()
     extra = None
     if not args.no_extra and args.workload == "products" and not args.rmat:
@@ -702,8 +756,9 @@ def main():
                                "(sgf_adam_step)",
                        "cuda_graph": r["used_graph"],
                        "edges": "rmat(.57,.19,.19)" if args.rmat else "uniform",
-                       "l2": "inputs (>= 1 GB of activations per pass) exceed the 126 MB L2; no explicit flush"},
+                       "l2": "inputs (>= 1 GB of activations per pass) exceed the 50 MB L2; no explicit flush"},
             "e2e": r["e2e"], "gpu_launches": r["launches"], "clocks": r["clocks"], "roofline": r["roofline"], "cpu_baseline": cpu,
+            "gpu": gpu_info(ctx.local),
             "extra": extra}
     print(json.dumps(line), flush=True)
     if world > 1:

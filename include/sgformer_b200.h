@@ -1,4 +1,4 @@
-/* sgformer_b200 — C-ABI of the B200 (sm_100a) SGFormer encoder hot path.
+/* sgformer_b200 — C-ABI of the H100 (sm_90a) SGFormer encoder hot path.
  *
  * The reference (qitianwu/SGFormer) has no FFI: its hot path is `ours.py` calling torch / torch_sparse /
  * torch_geometric ops.  Each entry point below replaces one of those call sites (cited per function,
@@ -6,6 +6,12 @@
  *   - plain pointers + sizes, no torch types; every pointer is DEVICE memory unless marked host;
  *   - `stream` is a cudaStream_t passed as void*; launchers never synchronise and never allocate
  *     (workspaces are passed in; *_ws_bytes tells the size);
+ *   - sums across thread blocks are deterministic (fixed order, no float atomics): a result is bit-identical
+ *     from run to run.  The launchers that sum columns or a loss across blocks (sgf_colstats, sgf_ln_bwd,
+ *     sgf_ln_bwd_attn, sgf_bn_bwd_reduce, sgf_bn_bwd_apply, sgf_pack_operand with colsum, sgf_softmax_nll)
+ *     take a device workspace `ws` of at least sgf_reduce_ws_bytes(width) bytes (16-byte aligned; width = h,
+ *     cols, or 1 for the loss) that holds the blocks' partials and arrival counters; the launcher resets the
+ *     counters on `stream`.  Calls whose kernels may run at the same time need distinct workspaces;
  *   - return 0 on success, a positive cudaError_t, or a negative SGF_ERR_* argument error;
  *   - dtype codes: SGF_F32 = 0 (float), SGF_BF16 = 1 (__nv_bfloat16); matrices are row-major with an
  *     explicit leading dimension in ELEMENTS; feature rows must be 16-byte aligned and have a
@@ -31,7 +37,7 @@ extern "C" {
 #define SGF_ERR_UNSUPPORTED (-2)
 #define SGF_ERR_DRIVER (-3)
 
-/* library / build info: "sgformer_b200 <version> sm_100a" (host string, static storage) */
+/* library / build info: "sgformer_b200 <version> sm_90a" (host string, static storage) */
 const char* sgf_version(void);
 /* number of kernels this library has launched since load (host counter; bench.py's gpu_launches) */
 int64_t sgf_launch_count(void);
@@ -162,7 +168,7 @@ int sgf_memcpy_async(void* dst, const void* src, size_t bytes, void* stream);
 int sgf_wait_flags(const uint32_t* flags, int n, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Dense contractions on tcgen05 tensor cores (bf16 operands staged by TMA, fp32 accumulation in TMEM).
+ * Dense contractions on Hopper tensor cores (wgmma; bf16 operands staged by TMA, fp32 accumulation in registers).
  * Replace nn.Linear / torch.einsum call sites (medium/ours.py:21-22,27-28,76-85; large/ours.py:38-40,
  * 123-128,136-143,199,275).
  * ------------------------------------------------------------------------------------------------ */
@@ -242,10 +248,13 @@ int sgf_gemm_tn(const sgf_gemm_tn_args* args /* host */, void* stream);
  * All take dtype in {SGF_F32, SGF_BF16} for the [rows,h] activations; statistics/parameters are fp32.
  * ------------------------------------------------------------------------------------------------ */
 
+/* Workspace bytes of a reducing launcher (see the conventions above) for rows of `width` floats reduced
+ * across thread blocks (h; cols of sgf_pack_operand; 1 for sgf_softmax_nll). */
+int sgf_reduce_ws_bytes(int32_t width, size_t* bytes /* host out */);
 /* column statistics: sum[c] += w[r]*x[r,c], sumsq[c] += x[r,c]^2 (outputs must be zeroed by the caller;
  * sum, sumsq, w nullable).  Gives K^T 1, ||Q||^2, ||K||^2, q^T gden, BatchNorm batch statistics. */
 int sgf_colstats(const void* x, int64_t ldx, int64_t rows, int h, int dtype, const float* w,
-                 float* sum, float* sumsq, void* stream);
+                 float* sum, float* sumsq, void* ws, size_t ws_bytes, void* stream);
 
 /* y = dropout( relu?( LN?( a*x + b*r ) ) ), r nullable.  stats: fp32 [rows,2] (mean, rstd) or NULL.
  * (TransConv.forward, large/ours.py:199-216).  p = dropout prob, seed identifies the mask. */
@@ -257,7 +266,7 @@ int sgf_ln_fwd(const void* x, const void* r, int64_t ld, int64_t rows, int h, in
 int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t ld, int64_t rows, int h, int dtype,
                float a, float b, const float* gamma, const float* beta, const float* stats, int use_ln,
                int use_relu, float p, uint64_t seed, float gscale, void* dx, void* dr, float* dgamma, float* dbeta,
-               void* stream);
+               void* ws, size_t ws_bytes, void* stream);
 
 /* BatchNorm1d (+bias +ReLU +dropout +residual +branch mix) — GraphConv.forward large/ours.py:78-93, GCN.forward
  * medium/models.py:49-63, SGFormer.forward large/ours.py:270.
@@ -281,13 +290,14 @@ int sgf_bn_fwd(const void* z, const void* res, const void* mix, int64_t ld, int6
 int sgf_bn_bwd_reduce(const void* dy, const void* dy2, const float* row_scale2, const void* z, int64_t ld,
                       int64_t rows, int h, int dtype, const float* mean, const float* rstd, const float* gamma,
                       const float* beta, const float* zbias, int use_bn, int use_relu, float p, uint64_t seed,
-                      float gscale, float* sums, void* stream);
+                      float gscale, float* sums, void* ws, size_t ws_bytes, void* stream);
 int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* row_scale2, const void* z, int64_t ld,
                      int64_t rows, int h, int dtype, const float* mean, const float* rstd, const float* gamma,
                      const float* beta, const float* zbias, int use_bn, int use_relu, int training, float p,
                      uint64_t seed, float gscale, int64_t stat_rows /* rows the batch statistics span; 0 = rows (the
                      global node count when row-sharded and `sums` was all-reduced) */, const float* sums, void* dz,
-                     void* dres, int dres_accumulate, float* dz_colsum, const float* out_row_scale, void* stream);
+                     void* dres, int dres_accumulate, float* dz_colsum, const float* out_row_scale, void* ws,
+                     size_t ws_bytes, void* stream);
 
 /* out = (a*x + b*y) * row_scale[r]  (y, row_scale nullable; y has x's dtype); in/out dtypes may differ (casts). */
 int sgf_axpby(const void* x, int64_t ldx, int x_dtype, const void* y, int64_t ldy, int y_dtype, float a, float b,
@@ -299,7 +309,8 @@ int sgf_axpby(const void* x, int64_t ldx, int x_dtype, const void* y, int64_t ld
 int sgf_pack_operand(const float* src, int64_t ld_src, int64_t rows, int cols, int transpose, void* dst,
                      int64_t ld_dst, int kp, int64_t plane_ld, float* colsum,
                      const int64_t* row_index /* nullable: dst row r = src row row_index[r] (mini-batch feature gather,
-                     large/main-batch.py:138 x[idx_i]); rows = number of gathered rows; not with transpose */, void* stream);
+                     large/main-batch.py:138 x[idx_i]); rows = number of gathered rows; not with transpose */, void* ws, size_t ws_bytes,
+                     void* stream);
 /* mean over heads: out[r,c] = (1/heads) * sum_h x[r, h*d + c]  (TransConvLayer, medium/ours.py:95) */
 int sgf_head_mean(const void* x, int64_t ldx, int64_t rows, int heads, int d, int dtype, void* out, int64_t ldo,
                   void* stream);
@@ -310,7 +321,8 @@ int sgf_head_mean(const void* x, int64_t ldx, int64_t rows, int heads, int d, in
  *   dlogits[r,:] = scale * (softmax(logits[r]) - onehot(labels[r])) for selected rows, 0 otherwise (dlogits nullable).
  * mask: uint8 [rows] or NULL (all rows). */
 int sgf_softmax_nll(const float* logits, int64_t ld, const int64_t* labels, const uint8_t* mask, int64_t rows, int c,
-                    float scale, float* loss, float* dlogits, int64_t ld_d, void* stream);
+                    float scale, float* loss, float* dlogits, int64_t ld_d, void* ws, size_t ws_bytes,
+                    void* stream);
 
 /* K11 - evaluation on the device (SURVEY.md §8f-3): number of rows r = idx[i], i < m (all rows when idx is NULL, then m = rows)
  * with argmax_j logits[r, j] == labels[r] (first maximum on ties), and optionally the sum of -log_softmax(logits[r])[labels[r]].
@@ -363,7 +375,7 @@ int sgf_attn_prepare_bwd(const float* s_raw, const float* z_raw, const float* ds
  * ------------------------------------------------------------------------------------------------ */
 /* Pass 1: G[h,h] = X^T X (fp32, both triangles, pitch ldg) and s[h] = X^T 1 of a bf16 tensor-core operand X [rows, h <= 256]
  * (planes = 1: one bf16 plane; planes = 3: bf16x3 planes side by side, plane_ld elements apart, the six partial products are
- * accumulated).  tcgen05 kernel that loads every tile once for both MMA operands and accumulates only the upper block
+ * accumulated).  wgmma kernel that loads every tile once for both MMA operands and accumulates only the upper block
  * triangle; deterministic two-stage reduction through ws (sgf_gram_ws_bytes). */
 int sgf_gram_ws_bytes(int32_t h, int32_t planes, int64_t rows, size_t* bytes);
 int sgf_gram(const void* x, int64_t ldx, int64_t rows, int32_t h, int32_t planes, int64_t plane_ld, float* G, int64_t ldg,
@@ -412,7 +424,8 @@ int sgf_advance_dropout_epoch(uint64_t* epoch_dev, void* stream);   /* *epoch_de
 int sgf_ln_bwd_attn(const void* dy, const void* o, const void* r, const void* xa, int64_t ld, int64_t rows, int h, int dtype,
                     float a, float b, const float* gamma, const float* beta, const float* stats, int use_ln, int use_relu,
                     float p, uint64_t seed, float gscale, const float* den, void* gnum, float* gden, void* dr, float* dgamma,
-                    float* dbeta, float* cs, float* pg, float* sg, void* stream);
+                    float* dbeta, float* cs, float* pg, float* sg, void* ws,
+                    size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused two-group Adam (SURVEY.md §8f-3; replaces torch.optim.Adam([{params1, trans_weight_decay}, {params2,

@@ -1,6 +1,6 @@
 /* Plain-C restatement of the integer part of GraphConvLayer.forward — TEST INFRASTRUCTURE ONLY.
  *
- * Follows /root/reference/large/ours.py:26-33: in-degree over `col` (PyG degree == scatter_add of
+ * Follows the reference's large/ours.py:26-33: in-degree over `col` (PyG degree == scatter_add of
  * ones, :28) and the CSR that torch_sparse.SparseTensor(row=col, col=row, ...) builds (:33): entries
  * ordered by key target*N+source, duplicates kept, rowptr = exclusive scan of the target counts.
  * Built by __graft_entry__.build() into oracle/_build/libcsr_ref.so; only tests/ may load it.

@@ -9,7 +9,7 @@ so the same weights can be loaded into the reference, the oracle and the CUDA bu
 
 Pinning: the reference has no tests or golden vectors of its own (SURVEY.md §4, §8c), so the oracle is
 pinned against *outputs of the reference itself*: `tests/make_golden.py` imports the unmodified
-`/root/reference/{medium,large,100M}/ours.py` (through `tests/ref_shims/`), runs seeded inputs and
+the reference's `{medium,large,100M}/ours.py` (through `tests/ref_shims/`), runs seeded inputs and
 commits inputs/outputs/gradients under `tests/golden/`; `tests/test_oracle_golden.py` checks this file
 against those fixtures (and, in the build container, `tests/test_oracle_vs_reference.py` checks it
 against the live reference).  The third-party ops the reference reaches through `torch_sparse` /
@@ -17,7 +17,7 @@ against the live reference).  The third-party ops the reference reaches through 
 `large/requirements.txt:8-10`); their published semantics are restated here and cross-checked
 against scipy / fp64 einsum in `oracle/np_ref.py`.
 
-All citations are into /root/reference/.
+All citations are paths in the reference repository.
 """
 from __future__ import annotations
 

@@ -21,7 +21,7 @@ def main():
     ap.add_argument("--rows", type=int, default=2449029)
     ap.add_argument("--schedules", default="1,2")
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--peak", type=float, default=6581.6, help="HBM GB/s (MEASURED_PEAKS.json)")
+    ap.add_argument("--peak", type=float, default=3350.0, help="HBM GB/s (default: H100 SXM data sheet)")
     ap.add_argument("--lib", default=None, help="alternative build of libsgformer_b200.so to time (A/B of kernel versions)")
     args = ap.parse_args()
     if args.lib:

@@ -18,7 +18,7 @@ def main():
     ap.add_argument("--workload", default="products")
     ap.add_argument("--lib", default=None)
     ap.add_argument("--reps", type=int, default=6)
-    ap.add_argument("--peak", type=float, default=6581.6)
+    ap.add_argument("--peak", type=float, default=3350.0, help="HBM GB/s (default: H100 SXM data sheet)")
     ap.add_argument("--check", action="store_true", help="compare with the main build's result (bitwise)")
     args = ap.parse_args()
     if args.lib:

@@ -1,6 +1,6 @@
-"""In-tree build of the CUDA library: nvcc -> sgformer_b200/lib/libsgformer_b200.so (sm_100a only).
+"""In-tree build of the CUDA library: nvcc -> sgformer_b200/lib/libsgformer_b200.so (sm_90a only).
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot; nothing is JIT-compiled at run time."""
+The .so is git-ignored and built by `__graft_entry__.build()`; nothing is JIT-compiled at run time."""
 import os
 import subprocess
 import sys
@@ -12,7 +12,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 OBJ_DIR = os.path.join(HERE, "build", "obj")
 LIB_PATH = os.path.join(LIB_DIR, "libsgformer_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
           "--expt-relaxed-constexpr"]
 

@@ -112,13 +112,14 @@ _SIGS = {
     "sgf_gemm_nt": (C.c_int, [C.POINTER(GemmNtArgs), _vp]),
     "sgf_gemm_tn_ws_bytes": (C.c_int, [_i32, _i32, _i64, C.POINTER(_sz)]),
     "sgf_gemm_tn": (C.c_int, [C.POINTER(GemmTnArgs), _vp]),
-    "sgf_colstats": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
+    "sgf_reduce_ws_bytes": (C.c_int, [_i32, C.POINTER(_sz)]),
+    "sgf_colstats": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sgf_ln_fwd": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, C.c_int, _f32, _f32, _vp, _vp, C.c_int, C.c_int, _f32,
                              _u64, _vp, _vp, _vp]),
     "sgf_ln_bwd": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _f32, _f32, _vp, _vp, _vp, C.c_int, C.c_int,
-                             _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp]),
+                             _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sgf_ln_bwd_attn": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _f32, _f32, _vp, _vp, _vp, C.c_int, C.c_int,
-                                  _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+                                  _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sgf_gram_ws_bytes": (C.c_int, [_i32, _i32, _i64, C.POINTER(_sz)]),
     "sgf_gram": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i64, _vp, _i64, _vp, _vp, _sz, _vp]),
     "sgf_attn_gram_ws_floats": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(_i64)]),
@@ -129,16 +130,16 @@ _SIGS = {
     "sgf_bn_fwd": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int,
                              _f32, _u64, _f32, _vp, _vp, _vp, _vp]),
     "sgf_bn_bwd_reduce": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int,
-                                    C.c_int, _f32, _u64, _f32, _vp, _vp]),
+                                    C.c_int, _f32, _u64, _f32, _vp, _vp, _sz, _vp]),
     "sgf_bn_bwd_apply": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int,
-                                   C.c_int, C.c_int, _f32, _u64, _f32, _i64, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp]),
+                                   C.c_int, C.c_int, _f32, _u64, _f32, _i64, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _sz, _vp]),
     "sgf_axpby": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _f32, _f32, _vp, _vp, _i64, C.c_int, _i64, C.c_int,
                             _vp]),
-    "sgf_pack_operand": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _i64, C.c_int, _i64, _vp, _vp, _vp]),
+    "sgf_pack_operand": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _i64, C.c_int, _i64, _vp, _vp, _vp, _sz, _vp]),
     "sgf_csr_subset_ws_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
     "sgf_csr_subset": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "sgf_eval_acc": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, C.c_int, _vp, _vp, _vp]),
-    "sgf_softmax_nll": (C.c_int, [_vp, _i64, _vp, _vp, _i64, C.c_int, _f32, _vp, _vp, _i64, _vp]),
+    "sgf_softmax_nll": (C.c_int, [_vp, _i64, _vp, _vp, _i64, C.c_int, _f32, _vp, _vp, _i64, _vp, _sz, _vp]),
     "sgf_head_mean": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, C.c_int, _vp, _i64, _vp]),
     "sgf_attn_prepare_fwd": (C.c_int, [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _i64, _vp, _i64,
                                        _i64, _vp, _vp]),

@@ -7,7 +7,7 @@ namespace sgf {
 std::atomic<int64_t> g_launches{0};
 }
 
-extern "C" const char* sgf_version(void) { return "sgformer_b200 0.1.0 sm_100a"; }
+extern "C" const char* sgf_version(void) { return "sgformer_b200 0.1.0 sm_90a"; }
 extern "C" int64_t sgf_launch_count(void) { return sgf::g_launches.load(std::memory_order_relaxed); }
 
 // This library links its own (static) CUDA runtime; the host framework selects the device on its runtime, so the

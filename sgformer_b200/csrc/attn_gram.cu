@@ -8,7 +8,7 @@
 // so with alpha = 1/(||q|| ||k||), beta = alpha/N the whole layer is   out = (x Bt^T + bt) / (x ct + dt),
 //     Bt = beta S^T Wq + Wv [d,h],  bt = beta S^T bq + bv,  ct = beta Wq^T z1,  dt = beta bq.z1 + 1
 // (numerator and denominator of medium/ours.py:21-31 divided by N).  sgf_attn_gram_prepare_fwd evaluates this from G, s and the
-// weights; the node passes themselves are tcgen05 GEMMs (sgf_gemm_tn x^T x, sgf_gemm_nt with SGF_EPI_ATTN_GRAM).
+// weights; the node passes themselves are wgmma GEMMs (sgf_gemm_tn x^T x, sgf_gemm_nt with SGF_EPI_ATTN_GRAM).
 // Backward (SURVEY.md Appendix A.1 pushed through the projections): with gnum' = g/den~, gden' = -(g.o)/den~ (sgf_ln_bwd_attn),
 // P = x^T gnum', pg = x^T gden', cs = 1^T gnum', sg = 1^T gden':
 //     dS = Wq P + bq cs^T,  dz = Wq pg + bq sg,  c = beta(<dS,S> + <dz,z1>),  cq = -c/||q||^2,  ck = -c/||k||^2

@@ -1,6 +1,6 @@
-// Common device helpers for the sgformer_b200 kernels (sm_100a only).
-// Thin inline-PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
-// UMMA shared-memory + instruction descriptors, cache-hinted 128-bit global loads/stores.
+// Common device helpers for the sgformer_b200 kernels (sm_90a).
+// Thin inline-PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), wgmma and its shared-memory descriptors,
+// cache-hinted 128-bit global loads/stores.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -26,7 +26,7 @@
 
 namespace sgf {
 
-constexpr int kNumSMsDefault = 148;
+constexpr int kNumSMsDefault = 132;
 
 __host__ inline int num_sms() {
     static int n = 0;
@@ -197,86 +197,61 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA, sm_90a): D[regs] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 :: "r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Pins accumulator registers between an asynchronous wgmma and the wait that completes it: without it the compiler may move
+// reads of the accumulators above the wait.
+template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, single-CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// m64 x n64 x k16.  TA / TB: 0 = K-major, 1 = MN-major operand.  scale_d = 0 overwrites D.
+// Accumulator layout (thread t of the warpgroup, warp w = t / 32, lane l): d[4c + 2s + e] is row 16w + l/4 + 8s,
+// column 8c + 2(l%4) + e.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-        :: "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                 :: "r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread (thread t = lane t of the warp's quadrant).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout, sm_100):
+// Warp-specialised kernels of 3 warpgroups (384 threads, 168 registers each at launch): the TMA producer warpgroup gives
+// registers back and the two MMA warpgroups take them (128 x 40 + 256 x 232 <= 64 K), so the accumulators stay in registers.
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(kProducerRegs)); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kConsumerRegs)); }
+
+// wgmma shared-memory matrix descriptor (cute::GMMA::GmmaDescriptor, sm_90):
 //  [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4 |
-//  [46,48) version = 1 | [49,52) base offset = 0 | [61,64) layout type (2 = SWIZZLE_128B).
+//  [49,52) base offset = 0 (tiles are 1024-byte aligned) | [62,64) layout type (1 = SWIZZLE_128B).
+// K-major SW128 (rows of 64 bf16 = 128 bytes): SBO = 1024 (8-row groups), LBO unused; the k-th 16-element step starts 32k
+// bytes further.  MN-major SW128: LBO = stride between 64-element MN chunks, SBO = stride between 8-row K groups.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-// UMMA instruction descriptor for kind::f16 with bf16 operands and fp32 accumulation
-// (cute::UMMA::InstrDescriptor): c_format[4,6)=1(F32) a_format[7,10)=1(BF16) b_format[10,13)=1(BF16)
-// a_major bit15, b_major bit16 (0 = K-major, 1 = MN-major), n_dim[17,23) = N>>3, m_dim[24,29) = M>>4.
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(int m, int n, int a_mn_major, int b_mn_major) {
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= 1u << 7;
-    d |= 1u << 10;
-    d |= static_cast<uint32_t>(a_mn_major & 1) << 15;
-    d |= static_cast<uint32_t>(b_mn_major & 1) << 16;
-    d |= static_cast<uint32_t>(n >> 3) << 17;
-    d |= static_cast<uint32_t>(m >> 4) << 24;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
 

@@ -1,6 +1,6 @@
 // K5 — CSR / CSC build of the GCN aggregation pattern, and K9 — induced subgraph with relabelling.
 //
-// Reference behaviour replaced (per call, /root/reference): large/ours.py:26-33 (PyG degree -> edge weights ->
+// Reference behaviour replaced (per call, paths in the reference repository): large/ours.py:26-33 (PyG degree -> edge weights ->
 // torch_sparse.SparseTensor(row=col, col=row): argsort of target*N+source + rowptr), medium/models.py:22-37
 // (PyG gcn_norm: add_remaining_self_loops + degree), large/main-batch.py:139 (PyG subgraph, CPU, O(E) per batch).
 //
@@ -24,7 +24,7 @@ constexpr int kScanBlock = 1024;
 constexpr int kScanItems = 4;  // per thread -> 4096 per block
 
 // rows [row_begin, row_end) of a matrix with n_cols columns are built; edges whose key falls outside are skipped.
-// (ncu r2g/r2h: 0.86 ms for 124 M edges = the L2's atomic rate; issuing four independent loads per thread changes nothing.)
+// (bound by the L2's atomic rate; issuing four independent loads per thread changes nothing.)
 __global__ void csr_count_kernel(const int64_t* __restrict__ key, const int64_t* __restrict__ val, int64_t nnz,
                                  int64_t row_begin, int64_t row_end, int64_t n_cols, int drop_self_loops,
                                  int* __restrict__ counts, int* __restrict__ err) {
@@ -133,7 +133,7 @@ __global__ void csr_fill_kernel(const int64_t* __restrict__ key, const int64_t* 
                                 int64_t row_begin, int64_t row_end, int64_t n_cols, int drop_self_loops,
                                 const int64_t* __restrict__ rowptr, int* __restrict__ cursor, int32_t* __restrict__ col) {
     // [row_begin, row_end) is the row window of THIS launch (sgf_csr_build_rot runs one launch per window so that the scattered
-    // 4-byte writes of a launch stay inside an L2-sized piece of `col`); rowptr / cursor are indexed relative to shard_begin.
+    // 4-byte writes of a launch stay inside one piece of `col`); rowptr / cursor are indexed relative to shard_begin.
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
         int64_t k = key[e];
@@ -679,8 +679,10 @@ extern "C" int sgf_csr_build_rot(const int64_t* edge_index, int64_t nnz, int64_t
     if (rc) return rc;
     if (nnz > 0) {
         // The fill scatters 4-byte entries over `col`; when `col` is much larger than the L2 every write is a DRAM sector
-        // read-modify-write (5.7 ms for the 124 M edges of the products shape).  Row windows whose share of `col` fits the L2 turn
-        // them into L2 hits written back as whole lines, at the price of re-reading the keys once per window.
+        // read-modify-write.  Row windows confine the writes of a launch to a piece of `col`, so that more of them hit lines
+        // already in L2 and are written back whole, at the price of re-reading the keys once per window.  The 128 MB window
+        // exceeds the 50 MB L2 of an H100 yet builds the products-shaped CSR faster than a 40 MB one (13.9 vs 16.0 ms,
+        // scripts/bench_csr.py on an H100 at a 400 W power limit): fewer windows re-read the keys fewer times.
         const int64_t win_bytes = fill_window_bytes();
         int64_t nwin = win_bytes > 0 ? ((nnz + n) * 4 + win_bytes - 1) / win_bytes : 1;
         if (nwin > kMaxFillWindows) nwin = kMaxFillWindows;

@@ -1,17 +1,17 @@
-// Dense contractions of the SGFormer encoder on tcgen05 tensor cores (sm_100a).
+// Dense contractions of the SGFormer encoder on Hopper tensor cores (wgmma, sm_90a).
 //
 //  gemm_nt : out[rows, n_out] = epilogue( sum_seg A_seg[rows, k] . B_seg[n_out, k]^T )      "row-streaming"
 //            rows = nodes (huge), n_out, k <= a few hundred.  Replaces nn.Linear forward / input-gradient,
 //            q~.(K^T V) and the attention backward products (reference medium/ours.py:22,28,76-85; large/ours.py:38-40,
 //            123-128,141,199,275).  Both operands K-major bf16, TMA SWIZZLE_128B tiles, BM=128 x BN<=256(+16) x BK=64,
-//            4-stage smem ring, fp32 accumulators in TMEM (double-buffered when BN<=256), warp-specialised:
-//            warp0 = TMA producer, warp1 = MMA issuer + TMEM owner, warps 2-5 = epilogue (one TMEM lane quadrant each).
+//            3-stage smem ring, fp32 accumulators in registers, warp-specialised: warp 8 = TMA producer, warps 0-7 = two
+//            consumer warpgroups (64 rows of the tile each) that issue the wgmma and run the epilogue of their rows.
 //  gemm_tn : out[m, n] = alpha * sum_rows A[rows, m]^T B[rows, n]                               "node-contracting"
 //            Replaces K^T V (medium/ours.py:21), its backward q^T gnum and every weight gradient dW = dY^T X.
 //            Both operands are MN-major for the MMA (features contiguous), loaded as [64 feat x 64 node] boxes;
 //            the node range is split across CTAs, per-CTA partials go to a workspace and are reduced deterministically.
 //
-// Descriptor formats follow cute/arch/mma_sm100_desc.hpp and cute/atom/mma_traits_sm100.hpp (canonical SW128 layouts).
+// Descriptor formats follow cute/atom/mma_traits_sm90_gmma.hpp (canonical SW128 layouts).
 #include "common.cuh"
 #include "launch_count.h"
 #include "../../include/sgformer_b200.h"
@@ -67,25 +67,23 @@ static int make_tmap_bf16(CUtensorMap* tm, const void* base, int64_t rows, int64
 // ================================================================================================
 namespace nt {
 constexpr int BM = 128, BK = 64, STAGES = 3;
-constexpr int EPI_WARPS = 8;                      // two warps per TMEM lane quadrant
-constexpr int THREADS = 32 * (2 + EPI_WARPS);     // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr int A_BYTES = BM * BK * 2;            // 16 KB
+constexpr int MMA_WARPS = 8;                      // two consumer warpgroups: tile rows [0,64) and [64,128)
+constexpr int THREADS = 32 * (MMA_WARPS + 4);     // warps 0..7 MMA + epilogue, warp 8 TMA producer (warps 9..11 idle)
+constexpr int A_BYTES = BM * BK * 2;              // 16 KB
 constexpr int B_BYTES_MAX = (256 + 16) * BK * 2;  // 34 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES_MAX;
-constexpr int STG_BYTES = BM * 128;               // output staging: 128 rows x 128 bytes (SW128) = one 4 KB tile per epilogue warp ...
-constexpr int WSTG_BYTES = 32 * 128;              // ... of 32 rows (its TMEM lane quadrant), stored by the warp's own TMA store
+constexpr int WSTG_BYTES = 16 * 128;              // output staging: a warp's 16 rows x 128 bytes (SW128), stored by its own TMA store
 constexpr int BAR_BYTES = 512;
 constexpr int STAT_COLS = 1024;                   // fused column statistics cover n_out <= 1024
 constexpr int STAT_BYTES = 2 * STAT_COLS * 4;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 4 * STG_BYTES + BAR_BYTES + STAT_BYTES + 1024;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + MMA_WARPS * 2 * WSTG_BYTES + BAR_BYTES + STAT_BYTES + 1024;
 // Resident-B mode (p.b_res): the whole B operand of one n-block (all k-blocks) stays in shared memory across the row tiles
 // of a CTA, so that only A streams through the ring.  Without it every 128-row tile re-fetches K x n_block of weights from
-// L2 and the kernel runs into the L2->SM throughput cap (~12 TB/s) before the HBM roofline (ncu, profiles/r1b_*).
+// L2, and at short K the few k-blocks of a tile cannot cover that latency.
 constexpr int RES_BYTES = (256 + 16) * 256 * 2;   // 136 KB: K = 256 x (256 + 16-column tail)
 constexpr int RES_MAX_KB = 16;                    // one full/empty mbarrier pair per resident k-block
 constexpr int RES_STAGES = 3;                     // A-only ring
-constexpr int RES_STG = 2;                        // one staging tile per epilogue half
-constexpr int SMEM_BYTES_RES = RES_BYTES + RES_STAGES * A_BYTES + RES_STG * STG_BYTES + BAR_BYTES + STAT_BYTES + 1024;
+constexpr int SMEM_BYTES_RES = RES_BYTES + RES_STAGES * A_BYTES + MMA_WARPS * WSTG_BYTES + BAR_BYTES + STAT_BYTES + 1024;
 static_assert(SMEM_BYTES <= 232448 && SMEM_BYTES_RES <= 232448, "exceeds the 227 KB of dynamic shared memory per CTA");
 
 struct Seg {
@@ -93,7 +91,7 @@ struct Seg {
 };
 struct Params {
     int64_t rows;
-    int n_out, bn_main, has_tail, n_blocks;
+    int n_out, bn_main, bn_pad, has_tail, n_blocks;   // bn_pad: bn_main rounded up to the 64-column MMA chunk
     int64_t num_tiles;
     int b_res;          // 1: resident-B schedule (see RES_BYTES)
     int64_t chunk;      // b_res: row tiles per CTA between two reloads of B (only matters when n_blocks > 1)
@@ -126,40 +124,7 @@ __device__ __forceinline__ void store1(void* base, int dtype, int64_t off, float
     if (dtype == 1) static_cast<__nv_bfloat16*>(base)[off] = __float2bfloat16_rn(v);
     else static_cast<float*>(base)[off] = v;
 }
-// 32 consecutive elements at element offset `off` (vec: 16-byte aligned and all 32 valid; else the first nv, rest 0)
-__device__ __forceinline__ void load32(const void* base, int dtype, int64_t off, bool vec, int nv, float* f) {
-    if (vec) {
-        if (dtype == 1) {
-            const uint4* q = reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(base) + off);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) Vec16<__nv_bfloat16>::unpack(q[i], f + 8 * i);
-        } else {
-            const uint4* q = reinterpret_cast<const uint4*>(static_cast<const float*>(base) + off);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) Vec16<float>::unpack(q[i], f + 4 * i);
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = j < nv ? load1(base, dtype, off + j) : 0.f;
-    }
-}
-__device__ __forceinline__ void store32(void* base, int dtype, int64_t off, bool vec, int nv, const float* f) {
-    if (vec) {
-        if (dtype == 1) {
-            uint4* q = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(base) + off);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) q[i] = Vec16<__nv_bfloat16>::pack(f + 8 * i);
-        } else {
-            uint4* q = reinterpret_cast<uint4*>(static_cast<float*>(base) + off);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) q[i] = Vec16<float>::pack(f + 4 * i);
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) if (j < nv) store1(base, dtype, off + j, f[j]);
-    }
-}
-// The three warp roles walk the CTA's tiles in the same order.
+// The two warp roles walk the CTA's tiles in the same order.
 //  streaming:  tile = blockIdx.x + i*gridDim.x over (m_blk, n_blk) pairs, n_blk fastest.
 //  resident-B: the CTA owns row tiles m = blockIdx.x + i*gridDim.x; they are visited in chunks of p.chunk, and inside a chunk
 //              n_blk is the OUTER loop: B(n_blk) is loaded once per (chunk, n_blk) "group", the chunk's A tiles are re-read
@@ -214,38 +179,59 @@ struct TileIter {
 };
 
 // Epilogue feature bits.  A specialised instantiation gemm_nt_kernel<F> compiles exactly the features in F (present and
-// unconditional: bf16 output through the TMA-store path, every 32-column piece complete, bf16 16-byte-aligned addends); the
+// unconditional: bf16 output through the TMA-store path, every 32-column piece complete, bf16 aligned addends); the
 // F_GENERIC instantiation reads every feature from Params at run time and handles ragged widths, fp32 and unaligned tensors.
 enum : int { F_BIAS = 1, F_AUX = 2, F_RELU = 4, F_ROWSCALE = 8, F_ACCUM = 16, F_R1 = 32, F_ATTN = 64, F_GENERIC = 128 };
+
+// 16 addends of a 32-column piece in accumulator layout (d[4c + 2s + e]: row rows[s], column col0 + 8c + e)
+template <bool GEN>
+__device__ __forceinline__ void load_piece(const void* src, int dtype, int64_t ld, const int64_t* rows, const bool* row_ok,
+                                           int col0, int n_out, bool nc, float* d) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            const int col = col0 + 8 * c;
+            const int64_t off = rows[s] * ld + col;
+            float a0 = 0.f, a1 = 0.f;
+            if (!GEN) {
+                if (row_ok[s]) {
+                    const uint32_t* q = reinterpret_cast<const uint32_t*>(static_cast<const __nv_bfloat16*>(src) + off);
+                    unpack_bf16x2(nc ? __ldg(q) : *q, a0, a1);
+                }
+            } else {
+                if (row_ok[s] && col < n_out) a0 = load1(src, dtype, off);
+                if (row_ok[s] && col + 1 < n_out) a1 = load1(src, dtype, off + 1);
+            }
+            d[4 * c + 2 * s] = a0;
+            d[4 * c + 2 * s + 1] = a1;
+        }
+}
 
 template <int F>
 __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_constant__ Tmaps tm, const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    // streaming: [ring: STAGES x (A | B)] [staging 4 tiles];  resident: [B: RES_BYTES] [ring: RES_STAGES x A] [staging 2 tiles]
+    // streaming: [ring: STAGES x (A | B)] [staging];  resident: [B: RES_BYTES] [ring: RES_STAGES x A] [staging]
     const bool res = p.b_res != 0;
     uint8_t* bres = smem;
     uint8_t* ring = res ? smem + RES_BYTES : smem;
     const int ring_stages = res ? RES_STAGES : STAGES;
     const int ring_stride = res ? A_BYTES : STAGE_BYTES;
-    const int stg_per_warp = res ? 1 : 2;                 // warp-private [32 rows x 128 B] staging tiles
+    const int stg_per_warp = res ? 1 : 2;                 // warp-private [16 rows x 128 B] staging tiles
     uint8_t* staging = ring + ring_stages * ring_stride;
-    uint64_t* full = reinterpret_cast<uint64_t*>(staging + EPI_WARPS * stg_per_warp * WSTG_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(staging + MMA_WARPS * stg_per_warp * WSTG_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint64_t* bres_full = tmem_empty + 2;
+    uint64_t* bres_full = empty + STAGES;
     uint64_t* bres_empty = bres_full + RES_MAX_KB;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bres_empty + RES_MAX_KB);
     float* stat_sm = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + BAR_BYTES);   // [2][STAT_COLS]: sum, sumsq
-    static_assert((2 * STAGES + 4 + 2 * RES_MAX_KB) * 8 + 4 <= BAR_BYTES, "barrier area");
+    static_assert((2 * STAGES + 2 * RES_MAX_KB) * 8 <= BAR_BYTES, "barrier area");
     static_assert(RES_STAGES <= STAGES, "ring barriers");
     const bool want_stats = p.col_sum != nullptr || p.col_sumsq != nullptr;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int bn_total = p.bn_main + (p.has_tail ? 16 : 0);
-    const int acc_stages = bn_total <= 256 ? 2 : 1;
+    const uint32_t b_tx = p.bn_pad * BK * 2 + (p.has_tail ? 16 * BK * 2 : 0);
     if (want_stats)
         for (int i = threadIdx.x; i < 2 * STAT_COLS; i += THREADS) stat_sm[i] = 0.f;
 
@@ -256,24 +242,16 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
         }
         if (p.has_tail) tma_prefetch_desc(&tm.tail);
         if (p.tma_store) tma_prefetch_desc(&tm.out);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], EPI_WARPS); }
-        for (int s = 0; s < RES_MAX_KB; ++s) { mbar_init(&bres_full[s], 1); mbar_init(&bres_empty[s], 1); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
+        for (int s = 0; s < RES_MAX_KB; ++s) { mbar_init(&bres_full[s], 1); mbar_init(&bres_empty[s], MMA_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= MMA_WARPS) {
+        producer_regs();
+        if (warp == MMA_WARPS && lane == 0) {
             // ===== TMA producer =====
-            const uint32_t b_tx = p.bn_main * BK * 2 + (p.has_tail ? 16 * BK * 2 : 0);
             int stage = 0; uint32_t phase = 0;
             TileIter ti(p);
             while (ti.next()) {
@@ -288,7 +266,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
                             mbar_arrive_expect_tx(&full[stage], A_BYTES + b_tx);
                             tma_load_2d(sa, &tm.a[sg.a_idx], &full[stage], sg.a_koff + kb * BK, ti.m_blk * BM);
                             tma_load_2d(sb, &tm.b[sg.b_idx], &full[stage], sg.b_koff + kb * BK, ti.n_blk * p.bn_main);
-                            if (p.has_tail) tma_load_2d(sb + p.bn_main * BK * 2, &tm.tail, &full[stage], sg.b_koff + kb * BK, 0);
+                            if (p.has_tail) tma_load_2d(sb + p.bn_pad * BK * 2, &tm.tail, &full[stage], sg.b_koff + kb * BK, 0);
                         } else {
                             // A first (its ring slot frees early), then - on the first tile of a group - the k-block of B,
                             // as soon as the previous group's last tile has consumed the old one
@@ -299,7 +277,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
                                 uint8_t* sb = bres + (size_t)kbg * b_tx;
                                 mbar_arrive_expect_tx(&bres_full[kbg], b_tx);
                                 tma_load_2d(sb, &tm.b[sg.b_idx], &bres_full[kbg], sg.b_koff + kb * BK, ti.n_blk * p.bn_main);
-                                if (p.has_tail) tma_load_2d(sb + p.bn_main * BK * 2, &tm.tail, &bres_full[kbg], sg.b_koff + kb * BK, 0);
+                                if (p.has_tail) tma_load_2d(sb + p.bn_pad * BK * 2, &tm.tail, &bres_full[kbg], sg.b_koff + kb * BK, 0);
                             }
                         }
                         if (++stage == ring_stages) { stage = 0; phase ^= 1; }
@@ -307,344 +285,248 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            const uint32_t idesc_main = make_idesc_bf16(BM, p.bn_main, 0, 0);
-            const uint32_t idesc_tail = make_idesc_bf16(BM, 16, 0, 0);
-            const uint32_t b_tx = p.bn_main * BK * 2 + (p.has_tail ? 16 * BK * 2 : 0);
-            int stage = 0; uint32_t phase = 0;
-            int64_t it = 0;
-            TileIter ti(p);
-            for (; ti.next(); ++it) {
-                const int acc = (int)(it % acc_stages);
-                const uint32_t acc_phase = (uint32_t)((it / acc_stages) & 1);
-                mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-                tcgen05_fence_after();
-                const uint32_t d_main = tmem_base + acc * 256;
-                for (int kbg = 0; kbg < p.total_kb; ++kbg) {
-                    if (res && ti.first) mbar_wait(&bres_full[kbg], (uint32_t)(ti.group & 1));
-                    mbar_wait(&full[stage], phase);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(ring + stage * ring_stride);
-                    const uint32_t sb = res ? smem_u32(bres) + (uint32_t)kbg * b_tx : sa + A_BYTES;
+        return;
+    }
+    consumer_regs();
+
+    // ===== consumers: wgmma over the tile's k-blocks, then the epilogue of the warpgroup's 64 rows =====
+    constexpr bool GEN = (F & F_GENERIC) != 0;
+    const bool f_bias = GEN ? p.bias != nullptr : (F & F_BIAS) != 0;
+    const bool f_aux = GEN ? p.aux != nullptr : (F & F_AUX) != 0;
+    const bool f_relu = GEN ? p.relu != 0 : (F & F_RELU) != 0;
+    const bool f_rs = GEN ? p.row_scale != nullptr : (F & F_ROWSCALE) != 0;
+    const bool f_acc = GEN ? p.accumulate != 0 : (F & F_ACCUM) != 0;
+    const bool f_r1 = GEN ? p.r1_row != nullptr : (F & F_R1) != 0;
+    const bool f_attn = GEN ? (p.epi == SGF_EPI_ATTN_APPLY || p.epi == SGF_EPI_ATTN_GRAM) : (F & F_ATTN) != 0;
+    const bool f_tma = GEN ? p.tma_store != 0 : true;
+    const bool f_stats = GEN ? want_stats : false;
+    const int out_dtype = GEN ? p.out_dtype : 1;
+    const int wg = warp >> 2;      // warpgroup: tile rows [64 wg, 64 wg + 64)
+    const int wq = warp & 3;       // warp in the warpgroup: 16 of those rows
+    const int rr = lane >> 2;      // accumulator rows rr and rr + 8 of the warp's 16
+    const int cq = 2 * (lane & 3); // accumulator columns cq, cq + 1 of every 8
+    float alpha = p.alpha, beta = p.beta;
+    if (p.alpha_dev) alpha *= *p.alpha_dev;
+    if (p.beta_dev) beta *= *p.beta_dev;
+    const float nfv = (f_attn && p.nf_dev) ? *p.nf_dev : p.nf;
+    const int GW = out_dtype == 1 ? 64 : 32;              // columns per 128-byte staging row
+    const int ppg = GW / 32;                              // pieces per staging group (bf16: 2, fp32: 1)
+    const int n_pieces = (p.bn_main + 31) / 32;
+    const int nch = p.bn_pad / 64;                        // 64-column MMA chunks
+    uint8_t* wstg = staging + warp * stg_per_warp * WSTG_BYTES;
+    const uint32_t a_off = wg * 64 * BK * 2;
+
+    float acc[4][32];
+    float acct[8];
+    uint32_t gcount = 0;
+    int stage = 0; uint32_t phase = 0;
+    TileIter ti(p);
+    while (ti.next()) {
+        for (int kbg = 0; kbg < p.total_kb; ++kbg) {
+            if (res && ti.first) mbar_wait(&bres_full[kbg], (uint32_t)(ti.group & 1));
+            mbar_wait(&full[stage], phase);
+            const uint32_t sa = smem_u32(ring + stage * ring_stride) + a_off;
+            const uint32_t sb = res ? smem_u32(bres) + (uint32_t)kbg * b_tx : smem_u32(ring + stage * ring_stride) + A_BYTES;
+            wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t da = make_smem_desc_sw128(sa + k * 32, 0, 1024);
-                        const uint64_t db = make_smem_desc_sw128(sb + k * 32, 0, 1024);
-                        const uint32_t accum = (kbg > 0 || k > 0) ? 1u : 0u;
-                        umma_bf16(d_main, da, db, idesc_main, accum);
-                        if (p.has_tail) {
-                            const uint64_t dt = make_smem_desc_sw128(sb + p.bn_main * BK * 2 + k * 32, 0, 1024);
-                            umma_bf16(d_main + p.bn_main, da, dt, idesc_tail, accum);
-                        }
-                    }
-                    umma_commit(&empty[stage]);
-                    if (res && ti.last) umma_commit(&bres_empty[kbg]);
-                    if (kbg == p.total_kb - 1) umma_commit(&tmem_full[acc]);
-                    if (++stage == ring_stages) { stage = 0; phase ^= 1; }
-                }
+            for (int k = 0; k < BK / 16; ++k) {
+                const uint64_t da = make_smem_desc_sw128(sa + k * 32, 16, 1024);
+                const uint32_t sc = (kbg > 0 || k > 0) ? 1u : 0u;
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    if (j < nch) wgmma_n64<0, 0>(acc[j], da, make_smem_desc_sw128(sb + j * 8192 + k * 32, 16, 1024), sc);
+                if (p.has_tail) wgmma_n16<0, 0>(acct, da, make_smem_desc_sw128(sb + p.bn_pad * BK * 2 + k * 32, 16, 1024), sc);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) fence_regs(acc[j]);
+            fence_regs(acct);
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&empty[stage]);
+                if (res && ti.last) mbar_arrive(&bres_empty[kbg]);
+            }
+            if (++stage == ring_stages) { stage = 0; phase ^= 1; }
+        }
+
+        // -------- epilogue --------
+        const int m_blk = ti.m_blk, n_blk = ti.n_blk;
+        const int64_t row_w = (int64_t)m_blk * BM + wg * 64 + wq * 16;     // first row of this warp's 16
+        const int64_t rows[2] = {row_w + rr, row_w + rr + 8};
+        const bool row_ok[2] = {rows[0] < p.rows, rows[1] < p.rows};
+        const int col_base = n_blk * p.bn_main;
+        float rs[2] = {1.f, 1.f}, r1r[2] = {0.f, 0.f}, inv_den[2] = {1.f, 1.f};
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            if (f_rs && row_ok[s]) rs[s] = p.row_scale[rows[s]];
+            if (f_r1 && row_ok[s]) r1r[s] = p.r1_row[rows[s]];
+        }
+        if (f_attn) {
+            // tail column 0 of rows rr / rr + 8 is held by lane 4 rr
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+                const float den = __shfl_sync(0xffffffffu, acct[2 * s], lane & ~3) + nfv;
+                inv_den[s] = 1.f / den;
+                if (row_ok[s] && p.den_out && n_blk == 0 && (lane & 3) == 0) p.den_out[rows[s]] = den;
             }
         }
-    } else {
-        // ===== epilogue: TMEM -> registers -> (warp-private smem staging -> TMA store | direct global stores) =====
-        // Each warp owns the 32 rows of its TMEM lane quadrant and every other 128-byte column group (two warps per
-        // quadrant), stages a [32 x 128 B] tile and stores it with its own TMA store: no cross-warp synchronisation.
-        constexpr bool GEN = (F & F_GENERIC) != 0;
-        const bool f_bias = GEN ? p.bias != nullptr : (F & F_BIAS) != 0;
-        const bool f_aux = GEN ? p.aux != nullptr : (F & F_AUX) != 0;
-        const bool f_relu = GEN ? p.relu != 0 : (F & F_RELU) != 0;
-        const bool f_rs = GEN ? p.row_scale != nullptr : (F & F_ROWSCALE) != 0;
-        const bool f_acc = GEN ? p.accumulate != 0 : (F & F_ACCUM) != 0;
-        const bool f_r1 = GEN ? p.r1_row != nullptr : (F & F_R1) != 0;
-        const bool f_attn = GEN ? (p.epi == SGF_EPI_ATTN_APPLY || p.epi == SGF_EPI_ATTN_GRAM) : (F & F_ATTN) != 0;
-        const bool f_tma = GEN ? p.tma_store != 0 : true;
-        const bool f_stats = GEN ? want_stats : false;
-        const int out_dtype = GEN ? p.out_dtype : 1;
-        const int ew = warp - 2;     // 0..7
-        const int q = warp & 3;      // TMEM lane quadrant this warp may access
-        const int half = ew >> 2;    // the two warps of a quadrant alternate over column groups
-        float alpha = p.alpha, beta = p.beta;
-        if (p.alpha_dev) alpha *= *p.alpha_dev;
-        if (p.beta_dev) beta *= *p.beta_dev;
-        const int out_es = out_dtype == 1 ? 2 : 4, aux_es = p.aux_dtype == 1 ? 2 : 4;
-        const bool vec_ok = !GEN || (((reinterpret_cast<uintptr_t>(p.out) & 15) == 0) && ((p.ldo * out_es) % 16 == 0));
-        const bool aux_vec_ok = !GEN || !p.aux || (((reinterpret_cast<uintptr_t>(p.aux) & 15) == 0) && ((p.ld_aux * aux_es) % 16 == 0));
-        const bool vecf_ok = !GEN || ((!p.bias || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) &&
-                                      (!p.r1_col || (reinterpret_cast<uintptr_t>(p.r1_col) & 15) == 0));
-        const int GW = out_dtype == 1 ? 64 : 32;              // columns per 128-byte staging row
-        uint8_t* wstg = staging + ew * stg_per_warp * WSTG_BYTES;
-        const int r_local = q * 32 + lane;
-        // The addend of the epilogue (aux, else the old output when accumulating) is fetched one 32-column piece AHEAD as
-        // packed 16-byte chunks: a thread owns a whole row, so an un-prefetched load costs a DRAM latency per piece.
-        const void* pre_src = f_aux ? p.aux : (f_acc ? p.out : nullptr);
-        const int64_t pre_ld = f_aux ? p.ld_aux : p.ldo;
-        const bool pre_on = GEN ? (pre_src && (f_aux ? p.aux_dtype == 1 && aux_vec_ok : out_dtype == 1 && vec_ok)) : (f_aux || f_acc);
-        uint4 pre[4];
-        bool pre_ok = false;     // pre[] holds the addend of the NEXT piece to be processed
-        auto prefetch = [&](int64_t row, bool row_ok, int col0) {
-            pre_ok = pre_on && row_ok && (!GEN || col0 + 32 <= p.n_out);
-            if (pre_ok) {
-                const uint4* src = reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(pre_src) + row * pre_ld + col0);
+        // -------- 32-column pieces; piece pc covers tile columns [32 pc, 32 pc + 32) --------
 #pragma unroll
-                // L1-allocating loads: a thread reads its row 64 bytes at a time, the second half of each 128-byte line
-                // must hit L1 (ld.global.nc.L1::no_allocate here made the addend GEMMs 1.5x slower than r1b)
-                for (int c = 0; c < 4; ++c) pre[c] = f_aux ? __ldg(src + c) : src[c];
-            }
-        };
-        const int n_pieces = (p.bn_main + 31) / 32;
-        const int ppg = GW / 32;                                   // pieces per staging group (bf16: 2, fp32: 1)
-        const int n_groups = (n_pieces + ppg - 1) / ppg;
-        uint32_t gcount = 0;
-        int64_t it = 0;
-        TileIter ti(p);
-        for (; ti.next(); ++it) {
-            const int m_blk = ti.m_blk, n_blk = ti.n_blk;
-            const int acc = (int)(it % acc_stages);
-            const uint32_t acc_phase = (uint32_t)((it / acc_stages) & 1);
-            const int64_t row = (int64_t)m_blk * BM + r_local;
-            const bool row_ok = row < p.rows;
-            const int col_base = n_blk * p.bn_main;
-            if (half < n_groups) prefetch(row, row_ok, col_base + half * ppg * 32);   // overlaps the wait for the accumulator
-            const float rs = (f_rs && row_ok) ? p.row_scale[row] : 1.f;
-            const float r1r = (f_r1 && row_ok) ? p.r1_row[row] : 0.f;
-            mbar_wait(&tmem_full[acc], acc_phase);
-            tcgen05_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 256;
-            float inv_den = 1.f;
-            const float nfv = (f_attn && p.nf_dev) ? *p.nf_dev : p.nf;
-            if (f_attn) {
-                float t[16];
+        for (int pc = 0; pc < 8; ++pc) {
+            if (pc >= n_pieces) break;
+            const int g = pc / ppg, pp = pc % ppg;
+            const uint32_t buf = stg_per_warp == 2 ? (gcount & 1) : 0;
+            if (f_tma && pp == 0) {
+                if (lane == 0) {                                   // the store that last used this buffer has drained
+                    if (stg_per_warp == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
+                }
                 __syncwarp();
-                tmem_ld16(taddr + p.bn_main, t);
-                tmem_ld_wait();
-                const float den = t[0] + nfv;
-                inv_den = 1.f / den;
-                if (row_ok && p.den_out && half == 0 && n_blk == 0) p.den_out[row] = den;
             }
-            // -------- 32-column pieces; piece index pc covers tile columns [32*pc, 32*pc+32) --------
-            for (int g = half; g < n_groups; g += 2) {
-                const uint32_t buf = stg_per_warp == 2 ? (gcount & 1) : 0;
-                if (f_tma) {
-                    if (lane == 0) {                                   // the store that last used this buffer has drained
-                        if (stg_per_warp == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
-                    }
-                    __syncwarp();
+            float v[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) v[i] = acc[pc >> 1][(pc & 1) * 16 + i];
+            const int col0 = col_base + pc * 32 + cq;              // column of v[0]; v[4c + 2s + e] is column col0 + 8c + e
+            float ax[16], old[16];
+            if (f_aux) load_piece<GEN>(p.aux, p.aux_dtype, p.ld_aux, rows, row_ok, col0, p.n_out, true, ax);
+            if (f_acc) load_piece<GEN>(p.out, out_dtype, p.ldo, rows, row_ok, col0, p.n_out, false, old);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const int s = (i >> 1) & 1;
+                const int col = col0 + 8 * (i >> 2) + (i & 1);
+                const bool cok = !GEN || col < p.n_out;
+                float x = v[i];
+                if (f_attn) {
+                    // out = (acc + nf*aux + bias) / (tail + nf): ATTN_APPLY carries aux (= v), ATTN_GRAM the bias bt
+                    if (f_aux) x += nfv * ax[i];
+                    if (f_bias && cok) x += __ldg(p.bias + col);
+                    x *= inv_den[s];
+                } else {
+                    x *= alpha;
+                    if (f_aux) x += beta * ax[i];
+                    if (f_bias && cok) x += __ldg(p.bias + col);
+                    if (f_r1 && cok) x += r1r[s] * __ldg(p.r1_col + col);
+                    if (f_relu) x = fmaxf(x, 0.f);
+                    if (f_rs) x *= rs[s];
                 }
-                for (int pp = 0; pp < ppg; ++pp) {
-                    const int pc = g * ppg + pp;
-                    if (pc >= n_pieces) break;
-                    // take this piece's prefetched addend (kept packed), then put the next piece's in flight
-                    uint4 cur[4];
-                    const bool have_ad = pre_ok;
-                    if (have_ad) {
+                if (f_acc) x += old[i];
+                v[i] = x;
+            }
+            if (f_tma) {
+                // 128-byte staging rows, 16-byte chunks XOR-swizzled with (row & 7) (== TMA SWIZZLE_128B); OOB rows/cols
+                // are clipped by the TMA store, so garbage there is harmless
+                uint8_t* tile = wstg + buf * WSTG_BYTES;
 #pragma unroll
-                        for (int c = 0; c < 4; ++c) cur[c] = pre[c];
-                    }
-                    {
-                        int next_pc = -1;
-                        if (pp + 1 < ppg && pc + 1 < n_pieces) next_pc = pc + 1;
-                        else if (g + 2 < n_groups) next_pc = (g + 2) * ppg;
-                        if (next_pc >= 0) prefetch(row, row_ok, col_base + next_pc * 32); else pre_ok = false;
-                    }
-                    float v[32];
-                    __syncwarp();  // tcgen05.ld is .sync.aligned
-                    tmem_ld32(taddr + pc * 32, v);
-                    tmem_ld_wait();
-                    const int col0 = col_base + pc * 32;
-                    const int ncol = GEN ? (p.n_out - col0 < 32 ? p.n_out - col0 : 32) : 32;   // valid columns (may be <= 0)
-                    const bool full32 = ncol == 32;
-                    if (row_ok && ncol > 0) {
-                        if (f_attn) {
-                            // out = (acc + nf*aux + bias) / (tail + nf): ATTN_APPLY carries aux (= v), ATTN_GRAM the bias bt
-                            if (f_aux) {
-                                if (have_ad) {
+                for (int c = 0; c < 4; ++c)
 #pragma unroll
-                                    for (int c = 0; c < 4; ++c) {
-                                        float a8[8];
-                                        Vec16<__nv_bfloat16>::unpack(cur[c], a8);
-#pragma unroll
-                                        for (int j = 0; j < 8; ++j) v[8 * c + j] += nfv * a8[j];
-                                    }
-                                } else if constexpr (GEN) {
-                                    float ax[32];
-                                    load32(p.aux, p.aux_dtype, row * p.ld_aux + col0, full32 && aux_vec_ok, ncol, ax);
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) v[j] += nfv * ax[j];
-                                }
-                            }
-                            if (f_bias) {
-                                if (!GEN || (full32 && vecf_ok && (col0 & 3) == 0)) {
-                                    const float4* bp = reinterpret_cast<const float4*>(p.bias + col0);
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) { float4 b4 = __ldg(bp + j); v[4*j] += b4.x; v[4*j+1] += b4.y; v[4*j+2] += b4.z; v[4*j+3] += b4.w; }
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) if (j < ncol) v[j] += p.bias[col0 + j];
-                                }
-                            }
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] *= inv_den;
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] *= alpha;
-                            if (f_aux) {
-                                if (have_ad) {
-#pragma unroll
-                                    for (int c = 0; c < 4; ++c) {
-                                        float a8[8];
-                                        Vec16<__nv_bfloat16>::unpack(cur[c], a8);
-#pragma unroll
-                                        for (int j = 0; j < 8; ++j) v[8 * c + j] += beta * a8[j];
-                                    }
-                                } else if constexpr (GEN) {
-                                    float ax[32];
-                                    load32(p.aux, p.aux_dtype, row * p.ld_aux + col0, full32 && aux_vec_ok, ncol, ax);
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) v[j] += beta * ax[j];
-                                }
-                            }
-                            if (f_bias) {
-                                if (!GEN || (full32 && vecf_ok && (col0 & 3) == 0)) {
-                                    const float4* bp = reinterpret_cast<const float4*>(p.bias + col0);
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) { float4 b4 = __ldg(bp + j); v[4*j] += b4.x; v[4*j+1] += b4.y; v[4*j+2] += b4.z; v[4*j+3] += b4.w; }
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) if (j < ncol) v[j] += p.bias[col0 + j];
-                                }
-                            }
-                            if (f_r1) {
-                                if (!GEN || (full32 && vecf_ok && (col0 & 3) == 0)) {
-                                    const float4* cp = reinterpret_cast<const float4*>(p.r1_col + col0);
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) { float4 c4 = __ldg(cp + j); v[4*j] += r1r * c4.x; v[4*j+1] += r1r * c4.y; v[4*j+2] += r1r * c4.z; v[4*j+3] += r1r * c4.w; }
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) if (j < ncol) v[j] += r1r * p.r1_col[col0 + j];
-                                }
-                            }
-                            if (f_relu)
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                            if (f_rs)
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) v[j] *= rs;
-                        }
-                        if (f_acc) {
-                            if (have_ad && !f_aux) {
-#pragma unroll
-                                for (int c = 0; c < 4; ++c) {
-                                    float o8[8];
-                                    Vec16<__nv_bfloat16>::unpack(cur[c], o8);
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) v[8 * c + j] += o8[j];
-                                }
-                            } else if (GEN || f_aux) {
-                                float old[32];
-                                load32(p.out, out_dtype, row * p.ldo + col0, full32 && vec_ok, ncol, old);
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) v[j] += old[j];
-                            }
-                        }
-                        if constexpr (GEN) {
-                            if (!f_tma) store32(p.out, out_dtype, row * p.ldo + col0, full32 && vec_ok, ncol, v);
-                        }
-                    }
-                    if (f_tma) {
-                        // 128-byte staging row, 16-byte chunks XOR-swizzled with (row & 7) (== TMA SWIZZLE_128B); OOB rows/cols
-                        // are clipped by the TMA store, so garbage there is harmless
-                        uint8_t* rowp = wstg + buf * WSTG_BYTES + lane * 128;
+                    for (int s = 0; s < 2; ++s) {
+                        const int r = rr + 8 * s;
                         if (out_dtype == 1) {
-#pragma unroll
-                            for (int c = 0; c < 4; ++c) {
-                                const int chunk = (pp * 4 + c) ^ (lane & 7);
-                                *reinterpret_cast<uint4*>(rowp + chunk * 16) = Vec16<__nv_bfloat16>::pack(v + 8 * c);
-                            }
+                            const int chunk = (pp * 4 + c) ^ (r & 7);
+                            *reinterpret_cast<uint32_t*>(tile + r * 128 + chunk * 16 + 2 * cq) = pack_bf16x2(v[4 * c + 2 * s], v[4 * c + 2 * s + 1]);
                         } else {
+                            const int chunk = (2 * c + (cq >> 2)) ^ (r & 7);
+                            *reinterpret_cast<float2*>(tile + r * 128 + chunk * 16 + 4 * (cq & 3)) = make_float2(v[4 * c + 2 * s], v[4 * c + 2 * s + 1]);
+                        }
+                    }
+            } else if constexpr (GEN) {
 #pragma unroll
-                            for (int c = 0; c < 8; ++c) {
-                                const int chunk = c ^ (lane & 7);
-                                *reinterpret_cast<uint4*>(rowp + chunk * 16) = Vec16<float>::pack(v + 4 * c);
-                            }
-                        }
-                    }
-                }
-                if (f_tma) {
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) {
-                        tma_store_2d(&tm.out, wstg + buf * WSTG_BYTES, col_base + g * GW, m_blk * BM + q * 32);
-                        bulk_commit();
-                    }
-                    if (f_stats) {
-                        // column sums of the staged (already rounded) 32-row tile: lane l owns columns l (and l + 32 for bf16);
-                        // the buffer is rewritten only after this warp's next bulk_wait_read + __syncwarp
-                        const uint8_t* tile = wstg + buf * WSTG_BYTES;
-                        const int64_t valid_rows = p.rows - ((int64_t)m_blk * BM + q * 32);
-                        for (int cg = lane; cg < GW; cg += 32) {
-                            const int colg = col_base + g * GW + cg;
-                            if (colg >= p.n_out || colg >= col_base + p.bn_main) continue;
-                            float s1 = 0.f, s2 = 0.f;
-                            for (int r = 0; r < 32 && r < valid_rows; ++r) {
-                                float x;
-                                if (out_dtype == 1) {
-                                    const int chunk = (cg >> 3) ^ (r & 7);
-                                    x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(tile + r * 128 + chunk * 16 + (cg & 7) * 2));
-                                } else {
-                                    const int chunk = (cg >> 2) ^ (r & 7);
-                                    x = *reinterpret_cast<const float*>(tile + r * 128 + chunk * 16 + (cg & 3) * 4);
-                                }
-                                s1 += x;
-                                s2 += x * x;
-                            }
-                            atomicAdd(&stat_sm[colg], s1);
-                            atomicAdd(&stat_sm[STAT_COLS + colg], s2);
-                        }
-                    }
-                    ++gcount;
+                for (int i = 0; i < 16; ++i) {
+                    const int s = (i >> 1) & 1;
+                    const int col = col0 + 8 * (i >> 2) + (i & 1);
+                    if (row_ok[s] && col < p.n_out) store1(p.out, out_dtype, rows[s] * p.ldo + col, v[i]);
                 }
             }
-            __syncwarp();
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        }
-        if (f_tma && lane == 0) bulk_wait<0>();
-        if (f_stats) {
-            named_bar_sync(3, 32 * EPI_WARPS);
-            for (int i = threadIdx.x - 64; i < p.n_out; i += 32 * EPI_WARPS) {
-                if (p.col_sum) atomicAdd(&p.col_sum[i], stat_sm[i]);
-                if (p.col_sumsq) atomicAdd(&p.col_sumsq[i], stat_sm[STAT_COLS + i]);
+            if (f_tma && (pp == ppg - 1 || pc == n_pieces - 1)) {
+                fence_proxy_async_smem();
+                __syncwarp();
+                if (lane == 0) {
+                    tma_store_2d(&tm.out, wstg + buf * WSTG_BYTES, col_base + g * GW, (int32_t)row_w);
+                    bulk_commit();
+                }
+                if (f_stats) {
+                    // column sums of the staged (already rounded) 16-row tile: lane l owns columns l (and l + 32 for bf16);
+                    // the buffer is rewritten only after this warp's next bulk_wait_read + __syncwarp
+                    const uint8_t* tile = wstg + buf * WSTG_BYTES;
+                    const int64_t valid_rows = p.rows - row_w;
+                    for (int cg = lane; cg < GW; cg += 32) {
+                        const int colg = col_base + g * GW + cg;
+                        if (colg >= p.n_out || colg >= col_base + p.bn_main) continue;
+                        float s1 = 0.f, s2 = 0.f;
+                        for (int r = 0; r < 16 && r < valid_rows; ++r) {
+                            float x;
+                            if (out_dtype == 1) {
+                                const int chunk = (cg >> 3) ^ (r & 7);
+                                x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(tile + r * 128 + chunk * 16 + (cg & 7) * 2));
+                            } else {
+                                const int chunk = (cg >> 2) ^ (r & 7);
+                                x = *reinterpret_cast<const float*>(tile + r * 128 + chunk * 16 + (cg & 3) * 4);
+                            }
+                            s1 += x;
+                            s2 += x * x;
+                        }
+                        atomicAdd(&stat_sm[colg], s1);
+                        atomicAdd(&stat_sm[STAT_COLS + colg], s2);
+                    }
+                }
+                ++gcount;
             }
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    if (f_tma && lane == 0) bulk_wait<0>();
+    if (f_stats) {
+        named_bar_sync(3, 32 * MMA_WARPS);
+        for (int i = threadIdx.x; i < p.n_out; i += 32 * MMA_WARPS) {
+            if (p.col_sum) atomicAdd(&p.col_sum[i], stat_sm[i]);
+            if (p.col_sumsq) atomicAdd(&p.col_sumsq[i], stat_sm[STAT_COLS + i]);
+        }
     }
 }
 }  // namespace nt
 
 // ================================================================================================
+// node-contracting products (gemm_tn, gram): flushing the register accumulators
+// ================================================================================================
+// The error of one wgmma accumulator grows with the number of nodes it sums: measured on an H100, sgf_gram over 300 k rows of
+// bf16x3 operands (about 4500 rows per accumulator) missed fp64 by 2.7e-5 relative, beyond the 2e-5 that tests/test_gpu_kernels.py
+// allows (a bias consistent with truncating fp32 accumulation).  Every FLUSH_KB node blocks (1024 rows) a thread adds its
+// accumulators into its own fp32 workspace partial (round-to-nearest, fixed order: deterministic) and restarts them from zero.
+constexpr int FLUSH_KB = 16;
+// ws[col * mp + row] (+)= acc for the accumulator rows mrow, mrow + 8 and columns 64 j + 8c + cq + e < ncols of the chunks
+// j in [j0, 4); acc is zeroed.
+__device__ __forceinline__ void flush_acc(float (&acc)[4][32], float* ws, int mp, int mrow, int cq, int j0, int ncols, bool add) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        if (j < j0) continue;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const int col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
+            float* w = ws + (int64_t)col * mp + mrow + 8 * ((i >> 1) & 1);
+            if (col < ncols) *w = add ? *w + acc[j][i] : acc[j][i];
+            acc[j][i] = 0.f;
+        }
+    }
+}
+
+// ================================================================================================
 // gemm_tn
 // ================================================================================================
+// CTA (x, y): features [128 x, 128 x + 128) of A (one warpgroup per 64) against all n of B, over the y-th slice of the
+// node blocks.  CTAs that share a node slice run side by side, so the second read of B hits L2.
 namespace tn {
-constexpr int BKN = 64, STAGES = 3, THREADS = 192;
+constexpr int BKN = 64, STAGES = 4, MMA_WARPS = 8, THREADS = 32 * (MMA_WARPS + 4);   // + the producer warpgroup
 constexpr int CHUNK_BYTES = 64 * BKN * 2;   // one [64 feat x 64 node] box = 8 KB
-constexpr int A_BYTES = 4 * CHUNK_BYTES;    // up to 256 features
-constexpr int B_BYTES = 4 * CHUNK_BYTES;
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // 64 KB
+constexpr int A_BYTES = 2 * CHUNK_BYTES;    // the CTA's 128 features of A
+constexpr int B_BYTES = 4 * CHUNK_BYTES;    // up to 256 features of B
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // 48 KB
 constexpr int BAR_BYTES = 256;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;
 
 struct Params {
     int64_t rows;
-    int m, n, m_blocks, n_chunks, un;  // un = UMMA N (n rounded up to 16)
+    int m, n, mp, n_chunks, un;   // mp = m rounded up to 128, un = n rounded up to 16
     int64_t kb_total;
-    float* ws;  // [grid][un][m_blocks*128]
+    float* ws;  // [gridDim.y][un][mp]
     int n_pairs;                                  // partial products accumulated per node block (1, or the 6 of bf16x3)
     int a_off[SGF_TN_MAX_PAIRS], b_off[SGF_TN_MAX_PAIRS];   // column offset (elements) of the plane each product reads
 };
@@ -657,35 +539,27 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     // contiguous slice of 64-row node blocks for this CTA
-    const int64_t per = p.kb_total / gridDim.x, rem = p.kb_total % gridDim.x;
-    const int64_t kb0 = blockIdx.x * per + (blockIdx.x < rem ? blockIdx.x : rem);
-    const int64_t kb1 = kb0 + per + (blockIdx.x < rem ? 1 : 0);
-    const int a_chunks = p.m_blocks * 2;
+    const int64_t per = p.kb_total / gridDim.y, rem = p.kb_total % gridDim.y;
+    const int64_t kb0 = blockIdx.y * per + (blockIdx.y < rem ? blockIdx.y : rem);
+    const int64_t kb1 = kb0 + per + (blockIdx.y < rem ? 1 : 0);
+    const int m0 = blockIdx.x * 128;
+    const int a_chunks = (p.m - m0) >= 128 ? 2 : ((p.m - m0) + 63) / 64;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tm.a);
         tma_prefetch_desc(&tm.b);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= MMA_WARPS) {
+        producer_regs();
+        if (warp == MMA_WARPS && lane == 0) {
             const uint32_t stage_tx = (a_chunks + p.n_chunks) * CHUNK_BYTES;
             int stage = 0; uint32_t phase = 0;
             // all partial products of a node block before the next block: the planes re-read by later products hit L2
@@ -696,71 +570,60 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
                     uint8_t* sb = sa + A_BYTES;
                     mbar_arrive_expect_tx(&full[stage], stage_tx);
                     for (int c = 0; c < a_chunks; ++c)
-                        tma_load_2d(sa + c * CHUNK_BYTES, &tm.a, &full[stage], p.a_off[pr] + c * 64, (int32_t)(kb * BKN));
+                        tma_load_2d(sa + c * CHUNK_BYTES, &tm.a, &full[stage], p.a_off[pr] + m0 + c * 64, (int32_t)(kb * BKN));
                     for (int c = 0; c < p.n_chunks; ++c)
                         tma_load_2d(sb + c * CHUNK_BYTES, &tm.b, &full[stage], p.b_off[pr] + c * 64, (int32_t)(kb * BKN));
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_bf16(128, p.un, 1, 1);  // both operands MN-major
-            int stage = 0; uint32_t phase = 0;
-            for (int64_t kb = kb0; kb < kb1; ++kb) {
-                for (int pr = 0; pr < p.n_pairs; ++pr) {
-                    mbar_wait(&full[stage], phase);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-                    const uint32_t sb = sa + A_BYTES;
+        return;
+    }
+    consumer_regs();
+
+    const int wg = warp >> 2, wq = warp & 3;
+    const bool active = wg < a_chunks;
+    float acc[4][32];
 #pragma unroll
-                    for (int k = 0; k < BKN / 16; ++k) {
-                        // MN-major SW128: LBO = stride between 64-element feature chunks, SBO = stride between 8-row node groups
-                        const uint64_t db = make_smem_desc_sw128(sb + k * 2048, CHUNK_BYTES, 1024);
-                        const uint32_t accum = (kb > kb0 || pr > 0 || k > 0) ? 1u : 0u;
-                        for (int mb = 0; mb < p.m_blocks; ++mb) {
-                            const uint64_t da = make_smem_desc_sw128(sa + mb * 2 * CHUNK_BYTES + k * 2048, CHUNK_BYTES, 1024);
-                            umma_bf16(tmem_base + mb * 256, da, db, idesc, accum);
-                        }
-                    }
-                    umma_commit(&empty[stage]);
-                    if (kb == kb1 - 1 && pr == p.n_pairs - 1) umma_commit(tmem_full);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+    // partial [un][mp] of this node slice: accumulator row = feature of A, column = feature of B
+    float* ws = p.ws + (int64_t)blockIdx.y * p.un * p.mp;
+    const int mrow = m0 + wg * 64 + wq * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    bool flushed = false;
+    int stage = 0; uint32_t phase = 0;
+    for (int64_t kb = kb0; kb < kb1; ++kb) {
+        for (int pr = 0; pr < p.n_pairs; ++pr) {
+            mbar_wait(&full[stage], phase);
+            if (active) {
+                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * CHUNK_BYTES;
+                const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BKN / 16; ++k) {
+                    // MN-major SW128: LBO = stride between 64-element feature chunks, SBO = stride between 8-row node groups
+                    const uint64_t da = make_smem_desc_sw128(sa + k * 2048, CHUNK_BYTES, 1024);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+                        if (j < p.n_chunks) wgmma_n64<1, 1>(acc[j], da, make_smem_desc_sw128(sb + j * CHUNK_BYTES + k * 2048, CHUNK_BYTES, 1024), 1u);
                 }
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int mp = p.m_blocks * 128;
-        float* ws = p.ws + (int64_t)blockIdx.x * p.un * mp;
-        if (kb1 > kb0) {
-            mbar_wait(tmem_full, 0);
-            tcgen05_fence_after();
-        }
-        for (int mb = 0; mb < p.m_blocks; ++mb) {
-            const int mrow = mb * 128 + q * 32 + lane;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + mb * 256;
-            for (int c = 0; c < p.un / 16; ++c) {
-                float v[16];
-                if (kb1 > kb0) {
-                    __syncwarp();
-                    tmem_ld16(taddr + c * 16, v);
-                    tmem_ld_wait();
-                } else {
+                wgmma_commit();
+                wgmma_wait<0>();
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = 0.f;
-                }
-#pragma unroll
-                for (int j = 0; j < 16; ++j) ws[(int64_t)(c * 16 + j) * mp + mrow] = v[j];
+                for (int j = 0; j < 4; ++j) fence_regs(acc[j]);
             }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[stage]);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1) {
+            flush_acc(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
+            flushed = true;
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
+    flush_acc(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
 }
 
 // out[i,j] = alpha * sum_cta ws[cta][j][i] (+ beta*out[i,j]);  i < m, j < n
@@ -783,16 +646,16 @@ __global__ void tn_reduce_kernel(const float* __restrict__ ws, int nparts, int m
 // ================================================================================================
 // The node-contracting product of gemm_tn specialised for A == B (reference contractions it replaces: k^T v, k^T 1, ||q||^2,
 // ||k||^2 of medium/ours.py:16-31 — all functions of X^T X, see csrc/attn_gram.cu):
-//  * every [64 feat x 64 node] box is loaded ONCE and feeds both operands of the MMA (A and B descriptors point at the same
-//    shared-memory tile), so the kernel moves rows*h*2 bytes for 2*rows*h^2 flops (AI = h flop/B: 256 at h = 256, at the
-//    bf16 ridge) instead of twice that;
-//  * G is symmetric: only the blocks (0,0), (0,1) and (1,1) of the 2 x 2 block matrix are accumulated
-//    (M=128 x N=256 + M=128 x N=128 per k-step: 3/4 of the flops, 384 TMEM columns), the reduction kernel mirrors (0,1);
-//  * X^T 1 rides along as an N = 16 MMA against a constant all-ones tile (16 more TMEM columns per row block);
-//  * bf16x3 operands (fp32 mode): the six plane pairs of kernels._PAIRS3 accumulate into the same TMEM tiles.
+//  * every [64 feat x 64 node] box is loaded ONCE and feeds both operands of the MMA (A and B descriptors point into the same
+//    shared-memory tile), so the kernel moves rows*h*2 bytes for 2*rows*h^2 flops instead of twice that;
+//  * G is symmetric: of the 64 x 64 feature blocks only those with column block >= row block are accumulated, the
+//    reduction kernel mirrors the rest.  A warpgroup owns one row block; CTA x pairs row blocks x and 2*m_blocks-1-x so that
+//    both CTAs of h = 256 issue the same number of MMAs;
+//  * X^T 1 rides along as an N = 16 MMA against a constant all-ones tile;
+//  * bf16x3 operands (fp32 mode): the six plane pairs of kernels._PAIRS3 accumulate into the same registers.
 // The node range is split across the CTAs; per-CTA partials -> workspace -> fixed-order reduction (deterministic).
 namespace gramk {
-constexpr int BKN = 64, THREADS = 192;
+constexpr int BKN = 64, MMA_WARPS = 8, THREADS = 32 * (MMA_WARPS + 4);   // + the producer warpgroup
 constexpr int CHUNK_BYTES = 64 * BKN * 2;        // one [64 feat x 64 node] box = 8 KB
 constexpr int ONES_BYTES = CHUNK_BYTES;          // constant tile of bf16 1.0
 constexpr int BAR_BYTES = 256;
@@ -801,176 +664,143 @@ constexpr int MAX_STAGES = 8;
 
 struct Params {
     int64_t rows, kb_total;
-    int h, chunks, m_blocks, un, n_planes, stages;
+    int h, chunks, m_blocks, un, mp, n_planes, stages;
     int plane_off[3];                             // column offset (elements) of each plane
     int n_pairs, pa[6], pb[6];
-    int ncols;                                    // fp32 columns per CTA partial: un + (un - 128 if m_blocks == 2) + m_blocks
-    float* ws;                                    // [grid][ncols][128]
+    float* ws;                                    // [gridDim.y][un + 1][mp]: G rows (features) x columns, then X^T 1
 };
 
 __global__ void __launch_bounds__(THREADS, 1) gram_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    const int plane_bytes = p.chunks * CHUNK_BYTES;
-    const int stage_bytes = p.n_planes * plane_bytes;
-    uint8_t* ones = smem + p.stages * stage_bytes;
+    const int c0 = blockIdx.x;                       // first feature chunk this CTA reads
+    const int nld = p.chunks - c0;                   // chunks [c0, chunks) are loaded
+    const int plane_bytes = nld * CHUNK_BYTES;
+    const int stage_stride = p.n_planes * p.chunks * CHUNK_BYTES;
+    uint8_t* ones = smem + p.stages * stage_stride;
     uint64_t* full = reinterpret_cast<uint64_t*>(ones + ONES_BYTES);
     uint64_t* empty = full + MAX_STAGES;
-    uint64_t* tmem_full = empty + MAX_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-    static_assert((2 * MAX_STAGES + 1) * 8 + 4 <= BAR_BYTES, "barrier area");
+    static_assert(2 * MAX_STAGES * 8 <= BAR_BYTES, "barrier area");
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int64_t per = p.kb_total / gridDim.x, rem = p.kb_total % gridDim.x;
-    const int64_t kb0 = blockIdx.x * per + (blockIdx.x < rem ? blockIdx.x : rem);
-    const int64_t kb1 = kb0 + per + (blockIdx.x < rem ? 1 : 0);
+    const int64_t per = p.kb_total / gridDim.y, rem = p.kb_total % gridDim.y;
+    const int64_t kb0 = blockIdx.y * per + (blockIdx.y < rem ? blockIdx.y : rem);
+    const int64_t kb1 = kb0 + per + (blockIdx.y < rem ? 1 : 0);
 
     for (int i = threadIdx.x; i < ONES_BYTES / 4; i += THREADS) reinterpret_cast<uint32_t*>(ones)[i] = 0x3F803F80u;   // bf16 1.0 x2
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tm);
-        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
+        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
     fence_proxy_async_smem();        // the generic-proxy writes of the ones tile must be visible to the tensor core (async proxy)
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // TMEM columns: [0, un) block row 0 | [256, 256 + un - 128) block (1,1) | 384 + 16*mb: X^T 1
-    constexpr uint32_t COL_D1 = 256, COL_S = 384;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= MMA_WARPS) {
+        producer_regs();
+        if (warp == MMA_WARPS && lane == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int64_t kb = kb0; kb < kb1; ++kb) {
                 mbar_wait(&empty[stage], phase ^ 1);
-                uint8_t* sa = smem + stage * stage_bytes;
-                mbar_arrive_expect_tx(&full[stage], (uint32_t)stage_bytes);
+                uint8_t* sa = smem + stage * stage_stride;
+                mbar_arrive_expect_tx(&full[stage], (uint32_t)(p.n_planes * plane_bytes));
                 for (int pl = 0; pl < p.n_planes; ++pl)
-                    for (int c = 0; c < p.chunks; ++c)
-                        tma_load_2d(sa + pl * plane_bytes + c * CHUNK_BYTES, &tm, &full[stage], p.plane_off[pl] + c * 64, (int32_t)(kb * BKN));
+                    for (int c = 0; c < nld; ++c)
+                        tma_load_2d(sa + pl * plane_bytes + c * CHUNK_BYTES, &tm, &full[stage], p.plane_off[pl] + (c0 + c) * 64, (int32_t)(kb * BKN));
                 if (++stage == p.stages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc0 = make_idesc_bf16(128, p.un, 1, 1);                                   // both operands MN-major
-            const uint32_t idesc1 = make_idesc_bf16(128, p.m_blocks == 2 ? p.un - 128 : 16, 1, 1);
-            const uint32_t idescs = make_idesc_bf16(128, 16, 1, 1);
-            const uint32_t s_ones = smem_u32(ones);
-            int stage = 0; uint32_t phase = 0;
-            for (int64_t kb = kb0; kb < kb1; ++kb) {
-                mbar_wait(&full[stage], phase);
-                tcgen05_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-                for (int pr = 0; pr < p.n_pairs; ++pr) {
-                    const uint32_t a0 = sa + p.pa[pr] * plane_bytes, b0 = sa + p.pb[pr] * plane_bytes;
-#pragma unroll
-                    for (int k = 0; k < BKN / 16; ++k) {
-                        // MN-major SW128: LBO = stride between 64-element feature chunks, SBO = stride between 8-row node groups
-                        const uint32_t accum = (kb > kb0 || pr > 0 || k > 0) ? 1u : 0u;
-                        const uint64_t da0 = make_smem_desc_sw128(a0 + k * 2048, CHUNK_BYTES, 1024);
-                        const uint64_t db0 = make_smem_desc_sw128(b0 + k * 2048, CHUNK_BYTES, 1024);
-                        umma_bf16(tmem_base, da0, db0, idesc0, accum);
-                        if (p.m_blocks == 2) {
-                            const uint64_t da1 = make_smem_desc_sw128(a0 + 2 * CHUNK_BYTES + k * 2048, CHUNK_BYTES, 1024);
-                            const uint64_t db1 = make_smem_desc_sw128(b0 + 2 * CHUNK_BYTES + k * 2048, CHUNK_BYTES, 1024);
-                            umma_bf16(tmem_base + COL_D1, da1, db1, idesc1, accum);
-                        }
-                    }
-                }
-                for (int pl = 0; pl < p.n_planes; ++pl) {
-                    const uint32_t a0 = sa + pl * plane_bytes;
-#pragma unroll
-                    for (int k = 0; k < BKN / 16; ++k) {
-                        const uint32_t accum = (kb > kb0 || pl > 0 || k > 0) ? 1u : 0u;
-                        const uint64_t dones = make_smem_desc_sw128(s_ones + k * 2048, CHUNK_BYTES, 1024);
-                        for (int mb = 0; mb < p.m_blocks; ++mb) {
-                            const uint64_t da = make_smem_desc_sw128(a0 + mb * 2 * CHUNK_BYTES + k * 2048, CHUNK_BYTES, 1024);
-                            umma_bf16(tmem_base + COL_S + 16 * mb, da, dones, idescs, accum);
-                        }
-                    }
-                }
-                umma_commit(&empty[stage]);
-                if (kb == kb1 - 1) umma_commit(tmem_full);
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int l = q * 32 + lane;
-        float* ws = p.ws + (int64_t)blockIdx.x * p.ncols * 128;
-        const bool any = kb1 > kb0;
-        if (any) {
-            mbar_wait(tmem_full, 0);
-            tcgen05_fence_after();
-        }
-        const uint32_t tlane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-        auto dump = [&](uint32_t tcol, int ncol16, int ws_col0) {
-            for (int c = 0; c < ncol16; ++c) {
-                float v[16];
-                if (any) {
-                    __syncwarp();
-                    tmem_ld16(tlane + tcol + c * 16, v);
-                    tmem_ld_wait();
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = 0.f;
-                }
-#pragma unroll
-                for (int j = 0; j < 16; ++j) ws[(int64_t)(ws_col0 + c * 16 + j) * 128 + l] = v[j];
-            }
-        };
-        dump(0, p.un / 16, 0);
-        int col = p.un;
-        if (p.m_blocks == 2) { dump(COL_D1, (p.un - 128) / 16, col); col += p.un - 128; }
-        for (int mb = 0; mb < p.m_blocks; ++mb) {
-            float v[16];
-            if (any) {
-                __syncwarp();
-                tmem_ld16(tlane + COL_S + 16 * mb, v);
-                tmem_ld_wait();
-            } else {
-                v[0] = 0.f;
-            }
-            ws[(int64_t)(col + mb) * 128 + l] = v[0];
-        }
+        return;
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    consumer_regs();
+
+    const int wg = warp >> 2, wq = warp & 3;
+    const int ic = wg == 0 ? blockIdx.x : 2 * p.m_blocks - 1 - blockIdx.x;    // this warpgroup's row block
+    const bool active = ic < p.chunks;
+    float acc[4][32], accs[8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) accs[i] = 0.f;
+    const uint32_t s_ones = smem_u32(ones);
+    float* ws = p.ws + (int64_t)blockIdx.y * (p.un + 1) * p.mp;
+    const int mrow = ic * 64 + wq * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    bool flushed = false;
+    // G partial of the chunks j >= ic, then column 0 of the ones product (X^T 1) as workspace column un
+    auto flush = [&]() {
+        flush_acc(acc, ws, p.mp, mrow, cq, ic, p.un, flushed);
+        if (cq == 0) {
+            float* w = ws + (int64_t)p.un * p.mp + mrow;
+            w[0] = flushed ? w[0] + accs[0] : accs[0];
+            w[8] = flushed ? w[8] + accs[2] : accs[2];
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) accs[i] = 0.f;
+        flushed = true;
+    };
+    int stage = 0; uint32_t phase = 0;
+    for (int64_t kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full[stage], phase);
+        if (active) {
+            const uint32_t sa = smem_u32(smem + stage * stage_stride);
+            wgmma_fence();
+            for (int pr = 0; pr < p.n_pairs; ++pr) {
+                const uint32_t a0 = sa + p.pa[pr] * plane_bytes + (ic - c0) * CHUNK_BYTES, b0 = sa + p.pb[pr] * plane_bytes;
+#pragma unroll
+                for (int k = 0; k < BKN / 16; ++k) {
+                    // MN-major SW128: LBO = stride between 64-element feature chunks, SBO = stride between 8-row node groups
+                    const uint64_t da = make_smem_desc_sw128(a0 + k * 2048, CHUNK_BYTES, 1024);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+                        if (j >= ic && j < p.chunks)
+                            wgmma_n64<1, 1>(acc[j], da, make_smem_desc_sw128(b0 + (j - c0) * CHUNK_BYTES + k * 2048, CHUNK_BYTES, 1024), 1u);
+                }
+            }
+            for (int pl = 0; pl < p.n_planes; ++pl) {
+                const uint32_t a0 = sa + pl * plane_bytes + (ic - c0) * CHUNK_BYTES;
+#pragma unroll
+                for (int k = 0; k < BKN / 16; ++k)
+                    wgmma_n16<1, 1>(accs, make_smem_desc_sw128(a0 + k * 2048, CHUNK_BYTES, 1024),
+                                    make_smem_desc_sw128(s_ones + k * 2048, CHUNK_BYTES, 1024), 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) fence_regs(acc[j]);
+            fence_regs(accs);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[stage]);
+        if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1) flush();
     }
+    if (active) flush();
 }
 
-// G (both triangles) and s from the per-CTA partials, summed in CTA order (deterministic)
-__global__ void gram_reduce_kernel(const float* __restrict__ ws, int nparts, int ncols, int un, int m_blocks, int h, float* __restrict__ G,
+// G (both triangles) and s from the per-CTA partials, summed in CTA order (deterministic).  Entries below the block
+// diagonal were not accumulated: they read their mirror image.
+__global__ void gram_reduce_kernel(const float* __restrict__ ws, int nparts, int un, int mp, int h, float* __restrict__ G,
                                    int64_t ldg, float* __restrict__ s) {
-    const int total = ncols * 128;
+    const int total = h * h + h;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
-        const int c = t / 128, l = t % 128;
-        float acc = 0.f;
-        for (int part = 0; part < nparts; ++part) acc += ws[((int64_t)part * ncols + c) * 128 + l];
-        if (c < un) {                                       // block row 0: G[l][c], mirrored into block (1,0)
-            if (l < h && c < h) {
-                G[(int64_t)l * ldg + c] = acc;
-                if (m_blocks == 2 && c >= 128) G[(int64_t)c * ldg + l] = acc;
-            }
-        } else if (m_blocks == 2 && c < un + (un - 128)) {   // block (1,1)
-            const int i = 128 + l, j = 128 + (c - un);
-            if (i < h && j < h) G[(int64_t)i * ldg + j] = acc;
-        } else {                                            // X^T 1
-            const int mb = c - (ncols - m_blocks);
-            const int i = mb * 128 + l;
-            if (i < h) s[i] = acc;
+        int i, c;
+        if (t < h * h) {
+            const int r = t / h, q = t % h;
+            const bool upper = (q >> 6) >= (r >> 6);
+            i = upper ? r : q;
+            c = upper ? q : r;
+        } else {
+            i = t - h * h;
+            c = un;
         }
+        float acc = 0.f;
+        for (int part = 0; part < nparts; ++part) acc += ws[((int64_t)part * (un + 1) + c) * mp + i];
+        if (t < h * h) G[(int64_t)(t / h) * ldg + t % h] = acc;
+        else s[i] = acc;
     }
 }
 }  // namespace gramk
@@ -1000,18 +830,16 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
     p.n_out = a->n_out;
     const int n16 = (a->n_out + 15) / 16 * 16;
     p.n_blocks = (n16 + 255) / 256;
-    // a 16-column tail needs n-block + 16 <= 256 TMEM columns per accumulator stage to keep the two stages (MMA of tile i+1
-    // overlapping the epilogue of tile i): split a 256-wide output into two 128(+16) blocks (the tail is recomputed, cheap)
-    // ... unless the whole B (all k-blocks of the 256 + 16 columns) can stay resident in shared memory: then ONE n-block with a
-    // single 272-column accumulator stage reads A once and B never again (the split form re-reads the A tile and re-streams 73 KB of
-    // B per 128 x 128 output tile: 5.2 GB through L2 for the 1.25 GB attention apply at the products shape, 0.76 ms, L2-bound).
+    // a 256-wide output with a 16-column tail is one n-block when the whole B (all k-blocks of the 256 + 16 columns) can stay
+    // resident in shared memory: A is read once and B never again.  Otherwise it is split into two 128(+16) blocks (the tail
+    // is recomputed, cheap), so that a streamed stage of B fits the ring.
     bool tail_one_block = false;
     if (has_tail && n16 + 16 > 256) {
         static const bool res_ok = [] { const char* e = getenv("SGF_ATTN_RESIDENT"); return !(e && e[0] == '0'); }();
         int kb = 0;
         for (int s = 0; s < a->n_seg; ++s) kb += (a->seg_klen[s] + nt::BK - 1) / nt::BK;
         tail_one_block = res_ok && a->schedule != SGF_GEMM_STREAM_B && n16 <= 256 && kb <= nt::RES_MAX_KB &&
-                         (int64_t)(n16 + 16) * nt::BK * 2 * kb <= nt::RES_BYTES;
+                         (int64_t)((n16 + 63) / 64 * 64 + 16) * nt::BK * 2 * kb <= nt::RES_BYTES;
         if (!tail_one_block) p.n_blocks = 2;
     }
     // equal-width n-blocks: a multiple of 16 (UMMA N), and of 64 when there are several - the epilogue stores 128-byte
@@ -1019,6 +847,7 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
     p.bn_main = p.n_blocks == 1 ? n16 : ((n16 / p.n_blocks + 63) / 64) * 64;
     if (p.bn_main > 256) return SGF_ERR_UNSUPPORTED;
     p.n_blocks = (n16 + p.bn_main - 1) / p.bn_main;
+    p.bn_pad = (p.bn_main + 63) / 64 * 64;
     p.has_tail = has_tail ? 1 : 0;
     const int64_t m_blocks = (a->rows + nt::BM - 1) / nt::BM;
     p.num_tiles = m_blocks * p.n_blocks;
@@ -1038,8 +867,8 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
     }
     // explicit resident-B request: narrow the n-blocks until one block of B fits (A is then re-read from L2 per n-block)
     if (a->schedule == SGF_GEMM_RESIDENT_B && !has_tail) {
-        while ((int64_t)p.bn_main * nt::BK * 2 * p.total_kb > nt::RES_BYTES && p.bn_main > 64) {
-            p.bn_main -= 64;
+        while ((int64_t)p.bn_pad * nt::BK * 2 * p.total_kb > nt::RES_BYTES && p.bn_main > 64) {
+            p.bn_main = p.bn_pad = p.bn_pad - 64;
             p.n_blocks = (n16 + p.bn_main - 1) / p.bn_main;
         }
         p.num_tiles = m_blocks * p.n_blocks;
@@ -1048,7 +877,7 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
     for (int i = 0; i < a->n_a; ++i)
         if ((rc = make_tmap_bf16(&tm.a[i], a->a[i], a->rows, a->a_cols[i], a->lda[i], nt::BM))) return rc;
     for (int i = 0; i < a->n_b; ++i)
-        if ((rc = make_tmap_bf16(&tm.b[i], a->b[i], a->n_out, a->b_cols[i], a->ldb[i], p.bn_main))) return rc;
+        if ((rc = make_tmap_bf16(&tm.b[i], a->b[i], a->n_out, a->b_cols[i], a->ldb[i], p.bn_pad))) return rc;
     if (has_tail && (rc = make_tmap_bf16(&tm.tail, a->b_tail, 16, a->b_cols[0], a->ldb_tail, 16))) return rc;
 
     p.epi = a->epi;
@@ -1063,23 +892,22 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
     {
         const int es = a->out_dtype == 1 ? 2 : 4;
         p.tma_store = ((reinterpret_cast<uintptr_t>(a->out) & 15) == 0 && (a->ldo * es) % 16 == 0) ? 1 : 0;
-        if (p.tma_store && (rc = make_tmap_2d(&tm.out, a->out, a->out_dtype, a->rows, a->n_out, a->ldo, 32))) return rc;
+        if (p.tma_store && (rc = make_tmap_2d(&tm.out, a->out, a->out_dtype, a->rows, a->n_out, a->ldo, 16))) return rc;
         p.col_sum = a->col_sum; p.col_sumsq = a->col_sumsq;
         if ((p.col_sum || p.col_sumsq) && (!p.tma_store || a->n_out > nt::STAT_COLS)) return SGF_ERR_UNSUPPORTED;
     }
 
     // resident-B schedule whenever one n-block of B (all k-blocks) fits: see nt::RES_BYTES
     {
-        const int64_t b_tx = (int64_t)(p.bn_main + (has_tail ? 16 : 0)) * nt::BK * 2;
+        const int64_t b_tx = (int64_t)(p.bn_pad + (has_tail ? 16 : 0)) * nt::BK * 2;
         const bool fits = p.total_kb <= nt::RES_MAX_KB && b_tx * p.total_kb <= nt::RES_BYTES;
         if (a->schedule == SGF_GEMM_RESIDENT_B && !fits) return SGF_ERR_UNSUPPORTED;
-        // AUTO: resident when the whole B is one n-block (loaded once per CTA): same speed as streaming at K = 256 and 1.7x
-        // faster for short K (K = 100 -> 256: 0.32 vs 0.53 ms at 2.4 M rows), where a tile's few k-blocks cannot cover the TMA
-        // latency of re-fetching B.  With several n-blocks the per-chunk reload of B stalls the MMA (QKV 1.41 vs 1.15 ms).
+        // AUTO: resident when the whole B is one n-block (loaded once per CTA), where short K leaves a tile too few k-blocks
+        // to cover the latency of re-fetching B.  With several n-blocks the per-chunk reload of B stalls the MMA.
         p.b_res = (fits && (a->schedule == SGF_GEMM_RESIDENT_B || (a->schedule == SGF_GEMM_AUTO && p.n_blocks == 1))) ? 1 : 0;
-        // several n-blocks: B is re-loaded per (chunk, n-block); a chunk of 8 row tiles per CTA keeps the A tiles that are
-        // re-read for the following n-blocks inside L2 (148 CTAs x 8 x 128 rows x K x 2 B = 75 MB at K = 256)
-        p.chunk = p.n_blocks == 1 ? (int64_t)1 << 40 : 8;
+        // several n-blocks: B is re-loaded per (chunk, n-block); a chunk of 4 row tiles per CTA keeps the A tiles that are
+        // re-read for the following n-blocks inside the 50 MB L2 (132 CTAs x 4 x 128 rows x K x 2 B = 35 MB at K = 256)
+        p.chunk = p.n_blocks == 1 ? (int64_t)1 << 40 : 4;
     }
     // resident-B: one CTA per SM over ROW tiles (every CTA visits all n-blocks of its rows)
     const int64_t work = p.b_res ? m_blocks : p.num_tiles;
@@ -1136,14 +964,17 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
     return SGF_OK;
 }
 
-static inline int tn_grid(int64_t kb_total) { return (int)(kb_total < num_sms() ? kb_total : num_sms()); }
+// node slices per 128-feature block of A: one wave of CTAs over all blocks
+static inline int tn_splits(int64_t kb_total, int m_blocks) {
+    const int64_t cap = num_sms() / m_blocks > 0 ? num_sms() / m_blocks : 1;
+    return (int)(kb_total < cap ? (kb_total < 1 ? 1 : kb_total) : cap);
+}
 
 extern "C" int sgf_gemm_tn_ws_bytes(int32_t m, int32_t n, int64_t rows, size_t* bytes) {
     if (!bytes || m <= 0 || m > 256 || n <= 0 || n > 256 || rows < 0) return SGF_ERR_ARG;
     const int m_blocks = (m + 127) / 128, un = (n + 15) / 16 * 16;
     const int64_t kb_total = (rows + tn::BKN - 1) / tn::BKN;
-    int grid = tn_grid(kb_total < 1 ? 1 : kb_total);
-    *bytes = (size_t)grid * un * m_blocks * 128 * sizeof(float);
+    *bytes = (size_t)tn_splits(kb_total, m_blocks) * un * m_blocks * 128 * sizeof(float);
     return SGF_OK;
 }
 
@@ -1153,7 +984,8 @@ extern "C" int sgf_gemm_tn(const sgf_gemm_tn_args* a, void* stream) {
     tn::Params p;
     memset(&p, 0, sizeof(p));
     p.rows = a->rows; p.m = a->m; p.n = a->n;
-    p.m_blocks = (a->m + 127) / 128;
+    const int m_blocks = (a->m + 127) / 128;
+    p.mp = m_blocks * 128;
     p.un = (a->n + 15) / 16 * 16;
     p.n_chunks = (p.un + 63) / 64;
     p.kb_total = (a->rows + tn::BKN - 1) / tn::BKN;
@@ -1168,7 +1000,7 @@ extern "C" int sgf_gemm_tn(const sgf_gemm_tn_args* a, void* stream) {
         if (p.a_off[i] + a->m > a_span) a_span = p.a_off[i] + a->m;
         if (p.b_off[i] + a->n > b_span) b_span = p.b_off[i] + a->n;
     }
-    const int mp = p.m_blocks * 128;
+    const int mp = p.mp;
     int grid = 0;
     if (a->rows > 0) {
         size_t need = 0;
@@ -1184,8 +1016,8 @@ extern "C" int sgf_gemm_tn(const sgf_gemm_tn_args* a, void* stream) {
             SGF_CUDA_TRY(cudaFuncSetAttribute(tn::gemm_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tn::SMEM_BYTES));
             attr_set = true;
         }
-        grid = tn_grid(p.kb_total);
-        tn::gemm_tn_kernel<<<grid, tn::THREADS, tn::SMEM_BYTES, st>>>(tm, p);
+        grid = tn_splits(p.kb_total, m_blocks);
+        tn::gemm_tn_kernel<<<dim3(m_blocks, grid), tn::THREADS, tn::SMEM_BYTES, st>>>(tm, p);
         SGF_LAUNCH_CHECK(); count_launch();
     }
     int64_t total = (int64_t)a->n * mp;
@@ -1204,21 +1036,20 @@ static int gram_geometry(int h, int planes, int64_t rows, gramk::Params& p) {
     p.chunks = (h + 63) / 64;
     p.m_blocks = h > 128 ? 2 : 1;
     p.un = (h + 15) / 16 * 16;
+    p.mp = p.m_blocks * 128;
     p.n_planes = planes;
     p.kb_total = (rows + gramk::BKN - 1) / gramk::BKN;
     p.stages = gramk::SMEM_BUDGET / (planes * p.chunks * gramk::CHUNK_BYTES);
     if (p.stages > gramk::MAX_STAGES) p.stages = gramk::MAX_STAGES;
     if (p.stages < 2) return SGF_ERR_UNSUPPORTED;
-    p.ncols = p.un + (p.m_blocks == 2 ? p.un - 128 : 0) + p.m_blocks;
     return SGF_OK;
 }
-static inline int gram_grid(int64_t kb_total) { return (int)(kb_total < num_sms() ? (kb_total < 1 ? 1 : kb_total) : num_sms()); }
 
 extern "C" int sgf_gram_ws_bytes(int32_t h, int32_t planes, int64_t rows, size_t* bytes) {
     gramk::Params p;
     int rc = gram_geometry(h, planes, rows, p);
     if (rc || !bytes) return rc ? rc : SGF_ERR_ARG;
-    *bytes = (size_t)gram_grid(p.kb_total) * p.ncols * 128 * sizeof(float);
+    *bytes = (size_t)tn_splits(p.kb_total, p.m_blocks) * (p.un + 1) * p.mp * sizeof(float);
     return SGF_OK;
 }
 
@@ -1241,7 +1072,7 @@ extern "C" int sgf_gram(const void* x, int64_t ldx, int64_t rows, int32_t h, int
         p.n_pairs = 6;
         for (int i = 0; i < 6; ++i) { p.pa[i] = PA[i]; p.pb[i] = PB[i]; }
     }
-    const int grid = gram_grid(p.kb_total);
+    const int grid = tn_splits(p.kb_total, p.m_blocks);
     if (rows > 0) {
         CUtensorMap tm;
         memset(&tm, 0, sizeof(tm));
@@ -1253,12 +1084,12 @@ extern "C" int sgf_gram(const void* x, int64_t ldx, int64_t rows, int32_t h, int
             SGF_CUDA_TRY(cudaFuncSetAttribute(gramk::gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
             attr_set = 227 * 1024;
         }
-        gramk::gram_kernel<<<grid, gramk::THREADS, smem_bytes, st>>>(tm, p);
+        gramk::gram_kernel<<<dim3(p.m_blocks, grid), gramk::THREADS, smem_bytes, st>>>(tm, p);
         SGF_LAUNCH_CHECK(); count_launch();
     } else {
         SGF_CUDA_TRY(cudaMemsetAsync(ws, 0, need, st));
     }
-    gramk::gram_reduce_kernel<<<(p.ncols * 128 + 255) / 256, 256, 0, st>>>(p.ws, grid, p.ncols, p.un, p.m_blocks, h, G, ldg, s);
+    gramk::gram_reduce_kernel<<<(h * h + h + 255) / 256, 256, 0, st>>>(p.ws, grid, p.un, p.mp, h, G, ldg, s);
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }

@@ -125,10 +125,73 @@ struct Lane {
     }
 };
 
-// fold per-lane column accumulators of a block into global memory (fp32 atomics)
+// ------------------------------------------------------------------------------------------------
+// Deterministic cross-block sums.  fp32 atomics would add the blocks' partials in whatever order they arrive, so two runs of
+// the same step would differ in the last bits (and a training run would drift apart).  Instead every reducing call site of a
+// kernel owns a slot of the caller's workspace (sgf_reduce_ws_bytes): block b writes its partial to row b of the slot, and the
+// last block to arrive adds the rows in block order.  The launcher zeroes the slots' arrival counters on its stream.
+// ------------------------------------------------------------------------------------------------
+constexpr int kRedSlots = 5;
+constexpr size_t kRedHeader = 256;   // bytes of the workspace that hold the counters
+struct RedWs {
+    float* part;      // [kRedSlots][gridDim.x][width]
+    unsigned* cnt;    // [kRedSlots] arrival counters
+};
+
+// gout[0..n) += sum over the blocks of part[0..n) (shared memory of every block, complete), in block order
+__device__ __forceinline__ void grid_reduce_add(const float* part, int n, int width, int slot, float* gout, const RedWs& red) {
+    __shared__ unsigned s_last;
+    float* base = red.part + (size_t)slot * gridDim.x * width;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) base[(size_t)blockIdx.x * width + i] = part[i];
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(&red.cnt[slot], 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (s_last) {
+        // columns in tiles of w <= blockDim.x; the G = blockDim.x / w thread groups of a tile take every G-th block row (8 loads
+        // in flight per thread), then group sums are added in group order
+        __shared__ float s_grp[kRowBlock];
+        __threadfence();
+        for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+            const int w = n - i0 < (int)blockDim.x ? n - i0 : (int)blockDim.x;
+            const int G = blockDim.x / w, grp = threadIdx.x / w, i = i0 + threadIdx.x % w;
+            if (grp < G) {
+                float a[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                unsigned b = grp;
+                for (; b + 7 * G < gridDim.x; b += 8 * G)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) a[j] += __ldcg(base + (size_t)(b + j * G) * width + i);
+                for (; b < gridDim.x; b += G) a[0] += __ldcg(base + (size_t)b * width + i);
+                s_grp[grp * w + threadIdx.x % w] = ((a[0] + a[1]) + (a[2] + a[3])) + ((a[4] + a[5]) + (a[6] + a[7]));
+            }
+            __syncthreads();
+            if ((int)threadIdx.x < w) {
+                float t = 0.f;
+                for (int q = 0; q < G; ++q) t += s_grp[q * w + threadIdx.x];
+                gout[i0 + threadIdx.x] += t;
+            }
+            __syncthreads();
+        }
+    }
+    __syncthreads();
+}
+
+static inline int red_max_grid() { return num_sms() * 16; }      // >= every grid of a reducing launch (row_grid, ew_grid)
+
+// the caller's workspace as the kernels see it; zeroes the arrival counters on the stream
+static int red_args(void* ws, size_t ws_bytes, int64_t width, cudaStream_t st, RedWs& red) {
+    const size_t need = kRedHeader + (size_t)kRedSlots * red_max_grid() * (size_t)width * sizeof(float);
+    if (!ws || ws_bytes < need || (reinterpret_cast<uintptr_t>(ws) & 15)) return SGF_ERR_ARG;
+    red.cnt = static_cast<unsigned*>(ws);
+    red.part = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + kRedHeader);
+    SGF_CUDA_TRY(cudaMemsetAsync(ws, 0, kRedSlots * sizeof(unsigned), st));
+    return SGF_OK;
+}
+
+// fold per-lane column accumulators of a block into gout (deterministic: warps in order, then blocks in order)
 template <typename T, int CPL>
 __device__ __forceinline__ void flush_columns(const Lane<T, CPL>& L, float (&acc)[CPL][Vec16<T>::N], float* sm /* [h] */, int h,
-                                              float* gout) {
+                                              float* gout, int slot, const RedWs& red) {
     constexpr int VN = Vec16<T>::N;
     for (int i = threadIdx.x; i < h; i += blockDim.x) sm[i] = 0.f;
     __syncthreads();
@@ -138,16 +201,18 @@ __device__ __forceinline__ void flush_columns(const Lane<T, CPL>& L, float (&acc
 #pragma unroll
             for (int i = 0; i < VN; ++i) acc[c][i] += __shfl_xor_sync(0xffffffffu, acc[c][i], o);
     }
-    if (L.grp == 0) {
+    const int nw = blockDim.x >> 5;
+    for (int w = 0; w < nw; ++w) {
+        if ((int)(threadIdx.x >> 5) == w && L.grp == 0) {
 #pragma unroll
-        for (int c = 0; c < CPL; ++c)
-            if (L.cval[c])
+            for (int c = 0; c < CPL; ++c)
+                if (L.cval[c])
 #pragma unroll
-                for (int i = 0; i < VN; ++i) atomicAdd(&sm[L.coff[c] + i], acc[c][i]);
+                    for (int i = 0; i < VN; ++i) sm[L.coff[c] + i] += acc[c][i];
+        }
+        __syncthreads();
     }
-    __syncthreads();
-    for (int i = threadIdx.x; i < h; i += blockDim.x) atomicAdd(&gout[i], sm[i]);
-    __syncthreads();
+    grid_reduce_add(sm, h, h, slot, gout, red);
 }
 
 #define SGF_ZERO(a)                                   \
@@ -163,7 +228,7 @@ template <typename T, int CPL> __host__ __device__ constexpr int colstats_live()
 template <typename T, int CPL>
 __global__ void __launch_bounds__(kRowBlock, (colstats_live<T, CPL>() > 56 ? 2 : 3)) colstats_kernel(const T* __restrict__ x, int64_t ldx, int64_t rows, int h, int chunks,
                                                               int lpr_log2, const float* __restrict__ w, float* __restrict__ sum,
-                                                              float* __restrict__ sumsq) {
+                                                              float* __restrict__ sumsq, RedWs red) {
     constexpr int VN = Vec16<T>::N;
     extern __shared__ float sm[];
     Lane<T, CPL> L(chunks, lpr_log2);
@@ -195,8 +260,8 @@ __global__ void __launch_bounds__(kRowBlock, (colstats_live<T, CPL>() > 56 ? 2 :
             SGF_FOR_ELEMS { s1[c][i] += wr[u] * f[c][i]; s2[c][i] += f[c][i] * f[c][i]; }
         }
     }
-    if (sum) flush_columns<T, CPL>(L, s1, sm, h, sum);
-    if (sumsq) flush_columns<T, CPL>(L, s2, sm, h, sumsq);
+    if (sum) flush_columns<T, CPL>(L, s1, sm, h, sum, 0, red);
+    if (sumsq) flush_columns<T, CPL>(L, s2, sm, h, sumsq, 1, red);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -272,7 +337,7 @@ __global__ void __launch_bounds__(kRowBlock, 3) ln_bwd_kernel(const T* __restric
                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
                                                             const float* __restrict__ stats, int use_ln, int use_relu, float p,
                                                             SeedArg seed_arg, float gscale, T* __restrict__ dx, T* __restrict__ dr,
-                                                            float* __restrict__ dgamma, float* __restrict__ dbeta) {
+                                                            float* __restrict__ dgamma, float* __restrict__ dbeta, RedWs red) {
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     extern __shared__ float sm[];
@@ -355,8 +420,8 @@ __global__ void __launch_bounds__(kRowBlock, 3) ln_bwd_kernel(const T* __restric
             }
         }
     }
-    if (use_ln && dgamma) flush_columns<T, CPL>(L, dg, sm, h, dgamma);
-    if (use_ln && dbeta) flush_columns<T, CPL>(L, db, sm, h, dbeta);
+    if (use_ln && dgamma) flush_columns<T, CPL>(L, dg, sm, h, dgamma, 0, red);
+    if (use_ln && dbeta) flush_columns<T, CPL>(L, db, sm, h, dbeta, 1, red);
 }
 
 // LayerNorm backward of y = dropout(relu?(LN?(a*o + b*r))) fused with the row prologue of the Gram-form attention backward
@@ -374,7 +439,8 @@ __global__ void __launch_bounds__(kRowBlock, (CPL >= 2 ? 1 : MINB)) ln_bwd_attn_
                                                                     const float* __restrict__ den, T* __restrict__ gnum,
                                                                     float* __restrict__ gden, T* __restrict__ dr,
                                                                     float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                                                    float* __restrict__ cs, float* __restrict__ pg, float* __restrict__ sg) {
+                                                                    float* __restrict__ cs, float* __restrict__ pg, float* __restrict__ sg,
+                                                                    RedWs red) {
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     extern __shared__ float sm[];
@@ -483,12 +549,18 @@ __global__ void __launch_bounds__(kRowBlock, (CPL >= 2 ? 1 : MINB)) ln_bwd_attn_
             if (L.sub == 0) gden[r] = gd;
         }
     }
-    if (use_ln && dgamma) flush_columns<T, CPL>(L, dg, sm, h, dgamma);
-    if (use_ln && dbeta) flush_columns<T, CPL>(L, db, sm, h, dbeta);
-    flush_columns<T, CPL>(L, acs, sm, h, cs);
-    flush_columns<T, CPL>(L, apg, sm, h, pg);
+    if (use_ln && dgamma) flush_columns<T, CPL>(L, dg, sm, h, dgamma, 0, red);
+    if (use_ln && dbeta) flush_columns<T, CPL>(L, db, sm, h, dbeta, 1, red);
+    flush_columns<T, CPL>(L, acs, sm, h, cs, 2, red);
+    flush_columns<T, CPL>(L, apg, sm, h, pg, 3, red);
     asg = warp_sum(asg);
-    if (L.lane == 0 && asg != 0.f) atomicAdd(sg, asg);
+    if (threadIdx.x == 0) sm[0] = 0.f;
+    __syncthreads();
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {         // warps in order
+        if (L.lane == 0 && (int)(threadIdx.x >> 5) == w) sm[0] += asg;
+        __syncthreads();
+    }
+    grid_reduce_add(sm, 1, h, 4, sg, red);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -590,7 +662,7 @@ __global__ void __launch_bounds__(kRowBlock, 2) bn_bwd_kernel(const T* __restric
                                                                int64_t stat_rows, float* __restrict__ sums, T* __restrict__ dz,
                                                                T* __restrict__ dres,
                                                                int dres_acc, float* __restrict__ dz_colsum,
-                                                               const float* __restrict__ out_scale) {
+                                                               const float* __restrict__ out_scale, RedWs red) {
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     extern __shared__ float sm[];
@@ -740,10 +812,10 @@ __global__ void __launch_bounds__(kRowBlock, 2) bn_bwd_kernel(const T* __restric
     }
     if (RING) cp_async_wait<0>();
     if (!APPLY) {
-        flush_columns<T, CPL>(L, a1, sm, h, sums);
-        flush_columns<T, CPL>(L, a2, sm, h, sums + h);
+        flush_columns<T, CPL>(L, a1, sm, h, sums, 0, red);
+        flush_columns<T, CPL>(L, a2, sm, h, sums + h, 1, red);
     } else if (dz_colsum) {
-        flush_columns<T, CPL>(L, a1, sm, h, dz_colsum);
+        flush_columns<T, CPL>(L, a1, sm, h, dz_colsum, 0, red);
     }
 }
 
@@ -778,14 +850,10 @@ __global__ void __launch_bounds__(kRowBlock) axpby_kernel(const TI* __restrict__
 __global__ void __launch_bounds__(kRowBlock) pack_operand_kernel(const float* __restrict__ src, int64_t ld_src, int64_t rows, int cols,
                                                                   int transpose, __nv_bfloat16* __restrict__ dst, int64_t ld_dst,
                                                                   int kp, int64_t plane_ld, float* __restrict__ colsum,
-                                                                  const int64_t* __restrict__ row_index) {
+                                                                  const int64_t* __restrict__ row_index, RedWs red) {
     extern __shared__ float sm[];
     const int64_t rows_out = transpose ? cols : rows;
     const int cols_out = transpose ? (int)rows : cols;
-    if (colsum) {
-        for (int i = threadIdx.x; i < cols; i += blockDim.x) sm[i] = 0.f;
-        __syncthreads();
-    }
     const int64_t total = rows_out * kp;
     const int64_t per_block = (total + gridDim.x - 1) / gridDim.x;
     const int64_t t0 = (int64_t)blockIdx.x * per_block;
@@ -796,7 +864,6 @@ __global__ void __launch_bounds__(kRowBlock) pack_operand_kernel(const float* __
         float v = 0.f;
         if (c < cols_out) {
             v = transpose ? src[(int64_t)c * ld_src + r] : src[(row_index ? row_index[r] : r) * ld_src + c];
-            if (colsum) atomicAdd(&sm[transpose ? (int)r : c], v);
         }
         __nv_bfloat16 p0 = __float2bfloat16_rn(v);
         __nv_bfloat16* o = dst + r * ld_dst + c;
@@ -809,9 +876,24 @@ __global__ void __launch_bounds__(kRowBlock) pack_operand_kernel(const float* __
         }
     }
     if (colsum) {
+        // the block's share of every source column, summed in element order, then the blocks in order (deterministic)
+        for (int k = threadIdx.x; k < cols; k += blockDim.x) {
+            float s = 0.f;
+            if (!transpose) {                    // source column k = output column: elements t = r * kp + k
+                for (int64_t r = t0 / kp; r * kp < t1; ++r) {
+                    const int64_t t = r * kp + k;
+                    if (t >= t0 && t < t1) s += src[(row_index ? row_index[r] : r) * ld_src + k];
+                }
+            } else {                             // source column k = output row: elements t = k * kp + c, c < cols_out
+                const int64_t c0 = t0 - (int64_t)k * kp > 0 ? t0 - (int64_t)k * kp : 0;
+                const int64_t c1e = t1 - (int64_t)k * kp;
+                const int64_t c1 = c1e < cols_out ? c1e : cols_out;
+                for (int64_t c = c0; c < c1; ++c) s += src[c * ld_src + k];
+            }
+            sm[k] = s;
+        }
         __syncthreads();
-        for (int i = threadIdx.x; i < cols; i += blockDim.x)
-            if (sm[i] != 0.f) atomicAdd(&colsum[i], sm[i]);
+        grid_reduce_add(sm, cols, cols, 0, colsum, red);
     }
 }
 
@@ -1006,7 +1088,8 @@ __global__ void attn_prepare_bwd_kernel(const float* __restrict__ s_raw, const f
 // Replaces F.log_softmax + nn.NLLLoss on out[train_mask] (reference large/main.py:139-141) and their backward.
 __global__ void __launch_bounds__(kRowBlock) softmax_nll_kernel(const float* __restrict__ x, int64_t ldx, const int64_t* __restrict__ y,
                                                                  const uint8_t* __restrict__ mask, int64_t rows, int c, float scale,
-                                                                 float* __restrict__ loss, float* __restrict__ dx, int64_t lddx) {
+                                                                 float* __restrict__ loss, float* __restrict__ dx, int64_t lddx,
+                                                                 RedWs red) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -1030,7 +1113,16 @@ __global__ void __launch_bounds__(kRowBlock) softmax_nll_kernel(const float* __r
         }
     }
     acc = warp_sum(acc);
-    if (lane == 0 && acc != 0.f) atomicAdd(loss, acc * scale);
+    __shared__ float s_acc[kRowBlock / 32];
+    if (lane == 0) s_acc[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {                      // warps in order, then the blocks in order (deterministic)
+        float b = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) b += s_acc[w];
+        s_acc[0] = b * scale;
+    }
+    __syncthreads();
+    grid_reduce_add(s_acc, 1, 1, 0, loss, red);
 }
 
 // K11 - evaluation on the device: accuracy (argmax == label) and summed NLL of log_softmax over the rows idx[0..m) (all rows if
@@ -1118,8 +1210,8 @@ using namespace sgf;
         }                                                                                                  \
     } while (0)
 
-// SGF_BN_BWD_RING (default on): shared-memory staging ring in the BatchNorm backward (rows of <= 32 chunks).  Measured (r2m, same
-// box, products-shaped step): 92.61 ms/step with the register pipeline, 91.39 with the ring; the whole GPU suite passes with it.
+// SGF_BN_BWD_RING (default on): shared-memory staging ring in the BatchNorm backward (rows of <= 32 chunks) instead of the
+// register pipeline.
 static inline bool bn_bwd_ring() {
     static const bool v = [] { const char* e = std::getenv("SGF_BN_BWD_RING"); return e ? std::atoi(e) != 0 : true; }();
     return v;
@@ -1136,14 +1228,22 @@ static inline bool geom_for(int dtype, int h, RowGeom& g) {
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 static inline bool ld_ok(int dtype, int64_t ld) { return ld % (dtype == 0 ? 4 : 8) == 0; }
 
-extern "C" int sgf_colstats(const void* x, int64_t ldx, int64_t rows, int h, int dtype, const float* w, float* sum, float* sumsq,
+extern "C" int sgf_reduce_ws_bytes(int32_t width, size_t* bytes) {
+    if (width <= 0 || !bytes) return SGF_ERR_ARG;
+    *bytes = kRedHeader + (size_t)kRedSlots * red_max_grid() * (size_t)width * sizeof(float);
+    return SGF_OK;
+}
+
+extern "C" int sgf_colstats(const void* x, int64_t ldx, int64_t rows, int h, int dtype, const float* w, float* sum, float* sumsq, void* ws, size_t ws_bytes,
                             void* stream) {
     RowGeom g;
     if (!geom_for(dtype, h, g) || !aligned16(x) || !ld_ok(dtype, ldx) || rows < 0) return SGF_ERR_ARG;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
     SGF_DISPATCH_T_CPL(dtype, g.cpl, (colstats_kernel<T, CPL><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
-                                         (const T*)x, ldx, rows, h, g.chunks, g.lpr_log2, w, sum, sumsq)));
+                                         (const T*)x, ldx, rows, h, g.chunks, g.lpr_log2, w, sum, sumsq, red)));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1166,7 +1266,8 @@ extern "C" int sgf_ln_fwd(const void* x, const void* r, int64_t ld, int64_t rows
 
 extern "C" int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t ld, int64_t rows, int h, int dtype, float a,
                           float b, const float* gamma, const float* beta, const float* stats, int use_ln, int use_relu, float p,
-                          uint64_t seed, float gscale, void* dx, void* dr, float* dgamma, float* dbeta, void* stream) {
+                          uint64_t seed, float gscale, void* dx, void* dr, float* dgamma, float* dbeta, void* ws, size_t ws_bytes,
+                          void* stream) {
     RowGeom g;
     if (!geom_for(dtype, h, g) || !aligned16(x) || !aligned16(dy) || !aligned16(dx) || !aligned16(r) || !aligned16(dr) ||
         !ld_ok(dtype, ld) || rows < 0)
@@ -1174,9 +1275,11 @@ extern "C" int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t 
     if (use_ln && (!gamma || !beta || !stats)) return SGF_ERR_ARG;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
     SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (ln_bwd_kernel<T, CPL, DROP><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                          (const T*)dy, (const T*)x, (const T*)r, ld, rows, h, g.chunks, g.lpr_log2, a, b, gamma, beta,
-                                         stats, use_ln, use_relu, p, seed, gscale, (T*)dx, (T*)dr, dgamma, dbeta)));
+                                         stats, use_ln, use_relu, p, seed, gscale, (T*)dx, (T*)dr, dgamma, dbeta, red)));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1184,7 +1287,8 @@ extern "C" int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t 
 extern "C" int sgf_ln_bwd_attn(const void* dy, const void* o, const void* r, const void* xa, int64_t ld, int64_t rows, int h,
                                int dtype, float a, float b, const float* gamma, const float* beta, const float* stats, int use_ln,
                                int use_relu, float p, uint64_t seed, float gscale, const float* den, void* gnum, float* gden,
-                               void* dr, float* dgamma, float* dbeta, float* cs, float* pg, float* sg, void* stream) {
+                               void* dr, float* dgamma, float* dbeta, float* cs, float* pg, float* sg, void* ws, size_t ws_bytes,
+                               void* stream) {
     RowGeom g;
     if (!geom_for(dtype, h, g) || !aligned16(o) || !aligned16(dy) || !aligned16(gnum) || !aligned16(r) || !aligned16(dr) ||
         !aligned16(xa) || !ld_ok(dtype, ld) || rows < 0)
@@ -1193,24 +1297,25 @@ extern "C" int sgf_ln_bwd_attn(const void* dy, const void* o, const void* r, con
     if (use_ln && (!gamma || !beta || !stats)) return SGF_ERR_ARG;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    // resident CTAs per SM for the one-chunk-per-lane geometry: 2 (118 registers, no spills; default) or 3 (80 registers, ~20
-    // spilled): measured on a B200 at the products shape 89.58 vs 89.75 ms/step (r2b), i.e. no difference
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
+    // resident CTAs per SM for the one-chunk-per-lane geometry: 2 (no spills; default) or 3 (fewer registers, some spilled)
     static const int minb = [] { const char* e = getenv("SGF_LNATTN_BLOCKS"); return (e && e[0] == '3') ? 3 : 2; }();
     if (minb == 2 && !use_relu) {
         SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (ln_bwd_attn_kernel<T, CPL, DROP, false, 2><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                              (const T*)dy, (const T*)o, (const T*)r, (const T*)xa, ld, rows, h, g.chunks, g.lpr_log2, a, b,
                                              gamma, beta, stats, use_ln, p, seed, gscale, den, (T*)gnum, gden, (T*)dr, dgamma,
-                                             dbeta, cs, pg, sg)));
+                                             dbeta, cs, pg, sg, red)));
     } else if (use_relu) {
         SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (ln_bwd_attn_kernel<T, CPL, DROP, true, 3><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                              (const T*)dy, (const T*)o, (const T*)r, (const T*)xa, ld, rows, h, g.chunks, g.lpr_log2, a, b,
                                              gamma, beta, stats, use_ln, p, seed, gscale, den, (T*)gnum, gden, (T*)dr, dgamma,
-                                             dbeta, cs, pg, sg)));
+                                             dbeta, cs, pg, sg, red)));
     } else {
         SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (ln_bwd_attn_kernel<T, CPL, DROP, false, 3><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                              (const T*)dy, (const T*)o, (const T*)r, (const T*)xa, ld, rows, h, g.chunks, g.lpr_log2, a, b,
                                              gamma, beta, stats, use_ln, p, seed, gscale, den, (T*)gnum, gden, (T*)dr, dgamma,
-                                             dbeta, cs, pg, sg)));
+                                             dbeta, cs, pg, sg, red)));
     }
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
@@ -1250,7 +1355,7 @@ extern "C" int sgf_bn_fwd(const void* z, const void* res, const void* mix, int64
 extern "C" int sgf_bn_bwd_reduce(const void* dy, const void* dy2, const float* row_scale2, const void* z, int64_t ld, int64_t rows,
                                  int h, int dtype, const float* mean, const float* rstd, const float* gamma, const float* beta,
                                  const float* zbias, int use_bn, int use_relu, float p, uint64_t seed, float gscale, float* sums,
-                                 void* stream) {
+                                 void* ws, size_t ws_bytes, void* stream) {
     RowGeom g;
     if (!geom_for(dtype, h, g) || !aligned16(dy) || !aligned16(dy2) || !aligned16(z) || !ld_ok(dtype, ld) || rows < 0 || !sums ||
         (!dy && !dy2))
@@ -1258,6 +1363,8 @@ extern "C" int sgf_bn_bwd_reduce(const void* dy, const void* dy2, const float* r
     if (use_bn && (!mean || !rstd || !gamma || !beta)) return SGF_ERR_ARG;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
     if (g.cpl == 1 && bn_bwd_ring()) {
         const size_t smem = bn_bwd_ring_smem(h);
         SGF_DISPATCH_T_DROP(dtype, p > 0.f, {
@@ -1265,7 +1372,7 @@ extern "C" int sgf_bn_bwd_reduce(const void* dy, const void* dy2, const float* r
             bn_bwd_kernel<T, 1, false, DROP, true><<<row_grid(rows, g), kRowBlock, smem, st>>>(
                 (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean, rstd, gamma, beta, zbias,
                 use_bn, use_relu, 1, p, seed, gscale, (int64_t)0, sums, (T*)nullptr, (T*)nullptr, 0, (float*)nullptr,
-                (const float*)nullptr);
+                (const float*)nullptr, red);
         });
         SGF_LAUNCH_CHECK(); count_launch();
         return SGF_OK;
@@ -1273,7 +1380,7 @@ extern "C" int sgf_bn_bwd_reduce(const void* dy, const void* dy2, const float* r
     SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_bwd_kernel<T, CPL, false, DROP, false><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                          (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean,
                                          rstd, gamma, beta, zbias, use_bn, use_relu, 1, p, seed, gscale, (int64_t)0, sums,
-                                         (T*)nullptr, (T*)nullptr, 0, (float*)nullptr, (const float*)nullptr)));
+                                         (T*)nullptr, (T*)nullptr, 0, (float*)nullptr, (const float*)nullptr, red)));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1282,7 +1389,8 @@ extern "C" int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* ro
                                 int h, int dtype, const float* mean, const float* rstd, const float* gamma, const float* beta,
                                 const float* zbias, int use_bn, int use_relu, int training, float p, uint64_t seed, float gscale,
                                 int64_t stat_rows, const float* sums, void* dz, void* dres, int dres_accumulate,
-                                float* dz_colsum, const float* out_row_scale, void* stream) {
+                                float* dz_colsum, const float* out_row_scale, void* ws, size_t ws_bytes,
+                                void* stream) {
     RowGeom g;
     if (!geom_for(dtype, h, g) || !aligned16(dy) || !aligned16(dy2) || !aligned16(z) || !aligned16(dz) || !aligned16(dres) ||
         !ld_ok(dtype, ld) || rows < 0 || (!dy && !dy2))
@@ -1291,6 +1399,8 @@ extern "C" int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* ro
     if (use_bn && training && !sums) return SGF_ERR_ARG;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
     if (g.cpl == 1 && bn_bwd_ring()) {
         const size_t smem = bn_bwd_ring_smem(h);
         SGF_DISPATCH_T_DROP(dtype, p > 0.f, {
@@ -1298,7 +1408,7 @@ extern "C" int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* ro
             bn_bwd_kernel<T, 1, true, DROP, true><<<row_grid(rows, g), kRowBlock, smem, st>>>(
                 (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean, rstd, gamma, beta, zbias,
                 use_bn, use_relu, training, p, seed, gscale, stat_rows, const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate,
-                dz_colsum, out_row_scale);
+                dz_colsum, out_row_scale, red);
         });
         SGF_LAUNCH_CHECK(); count_launch();
         return SGF_OK;
@@ -1306,7 +1416,7 @@ extern "C" int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* ro
     SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_bwd_kernel<T, CPL, true, DROP, false><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                          (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean,
                                          rstd, gamma, beta, zbias, use_bn, use_relu, training, p, seed, gscale, stat_rows,
-                                         const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate, dz_colsum, out_row_scale)));
+                                         const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate, dz_colsum, out_row_scale, red)));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1340,23 +1450,27 @@ extern "C" int sgf_axpby(const void* x, int64_t ldx, int x_dtype, const void* y,
 }
 
 extern "C" int sgf_pack_operand(const float* src, int64_t ld_src, int64_t rows, int cols, int transpose, void* dst,
-                                int64_t ld_dst, int kp, int64_t plane_ld, float* colsum, const int64_t* row_index, void* stream) {
+                                int64_t ld_dst, int kp, int64_t plane_ld, float* colsum, const int64_t* row_index, void* ws,
+                                size_t ws_bytes, void* stream) {
     if (!src || !dst || rows <= 0 || cols <= 0 || kp <= 0 || (row_index && transpose)) return SGF_ERR_ARG;
     const int64_t cols_out = transpose ? rows : cols;
     if (kp < cols_out || (plane_ld > 0 && plane_ld < kp) || ld_dst < (plane_ld > 0 ? 2 * plane_ld + kp : kp)) return SGF_ERR_ARG;
     if (colsum && cols > 8192) return SGF_ERR_UNSUPPORTED;
     const int64_t rows_out = transpose ? cols : rows;
-    // 16-byte vectorised row pack (validated on a B200 in r2: the GPU suite passes with it and the arxiv-shaped fp32 step, which
-    // packs 28 activations per step into bf16x3 planes, goes from 8.98 to 7.86 ms); SGF_PACK_VEC=0 selects the scalar kernel
+    // 16-byte vectorised row pack (the arxiv-shaped fp32 step packs 28 activations per step into bf16x3 planes);
+    // SGF_PACK_VEC=0 selects the scalar kernel
     static const bool vec_on = [] { const char* e = getenv("SGF_PACK_VEC"); return !(e && e[0] == '0'); }();
     const bool vec = vec_on && !transpose && !colsum && cols % 8 == 0 && kp % 8 == 0 && ld_src % 4 == 0 && ld_dst % 8 == 0 &&
                      plane_ld % 8 == 0 && aligned16(src) && aligned16(dst);
+    RedWs red{nullptr, nullptr};
+    if (colsum)
+        if (int rc = red_args(ws, ws_bytes, cols, (cudaStream_t)stream, red)) return rc;
     if (vec)
         pack_rows_vec_kernel<<<ew_grid(rows_out * (kp / 8)), kRowBlock, 0, (cudaStream_t)stream>>>(
             src, ld_src, rows, cols, (__nv_bfloat16*)dst, ld_dst, kp, plane_ld, row_index);
     else
         pack_operand_kernel<<<ew_grid(rows_out * kp), kRowBlock, colsum ? cols * sizeof(float) : 0, (cudaStream_t)stream>>>(
-            src, ld_src, rows, cols, transpose, (__nv_bfloat16*)dst, ld_dst, kp, plane_ld, colsum, row_index);
+            src, ld_src, rows, cols, transpose, (__nv_bfloat16*)dst, ld_dst, kp, plane_ld, colsum, row_index, red);
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1420,14 +1534,17 @@ extern "C" int sgf_attn_prepare_bwd(const float* s_raw, const float* z_raw, cons
 }
 
 extern "C" int sgf_softmax_nll(const float* logits, int64_t ld, const int64_t* labels, const uint8_t* mask, int64_t rows, int c,
-                               float scale, float* loss, float* dlogits, int64_t ld_d, void* stream) {
+                               float scale, float* loss, float* dlogits, int64_t ld_d, void* ws, size_t ws_bytes,
+                               void* stream) {
     if (!logits || !labels || !loss || rows < 0 || c <= 0) return SGF_ERR_ARG;
     if (rows == 0) return SGF_OK;
     int64_t blocks = (rows * 32 + kRowBlock - 1) / kRowBlock;
     int64_t cap = (int64_t)num_sms() * 8;
     if (blocks > cap) blocks = cap;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, 1, (cudaStream_t)stream, red)) return rc;
     softmax_nll_kernel<<<(unsigned)blocks, kRowBlock, 0, (cudaStream_t)stream>>>(logits, ld, labels, mask, rows, c, scale, loss,
-                                                                               dlogits, ld_d);
+                                                                               dlogits, ld_d, red);
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }

@@ -27,10 +27,9 @@ constexpr int kSpmmBlock = 256;
 #ifndef SGF_SPMM_MIN_BLOCKS
 #define SGF_SPMM_MIN_BLOCKS 4
 #endif
-// Tuning knobs, measured on a B200 at the products shape (scripts/gpu_spmm_ab.sh, profiles/r1c_spmm_variants.txt): 4 rows in flight
-// x 4 CTAs/SM = 9.74 ms/launch; 8 rows x 3 CTAs/SM 9.72; software-pipelining the rowptr -> column-id -> feature-row chain
-// across a warp's rows (SGF_SPMM_PIPELINE=1) 10.0-10.8 ms.  The gather already saturates the memory system (1.03x the copy
-// bandwidth, 81 % of the DRAM peak in ncu); extra memory-level parallelism buys nothing, so the simple loop stays.
+// Tuning knobs (scripts/bench_spmm.py times the variants): rows in flight per lane group x CTAs per SM, and software-pipelining
+// the rowptr -> column-id -> feature-row chain across a warp's rows (SGF_SPMM_PIPELINE=1).  Once the gather saturates the memory
+// system extra memory-level parallelism buys nothing, so the simple loop is the default.
 #ifndef SGF_SPMM_PIPELINE
 #define SGF_SPMM_PIPELINE 0
 #endif
@@ -136,7 +135,7 @@ __device__ __forceinline__ void gather_range_flagged(const int32_t* __restrict__
 // One warp per output row, rows r = warp, warp + nwarps, ...; rows longer than max_len (> 0) are left to the segmented path
 // below.  SGF_SPMM_PIPELINE=1 software-pipelines the dependent chain rowptr -> column ids -> feature rows across the warp's work
 // items (an item = up to 32 neighbours of one row): while the gathers of item i are in flight, the column ids of item i+1 (same
-// row or the warp's next row) and the rowptr entries of the row after next are already loading (slower on B200, see above).
+// row or the warp's next row) and the rowptr entries of the row after next are already loading (off by default, see above).
 // Row range of a phased SpMM (row-sharded runs, dist.Comm._spmm_phased): the launch handles entries [lo[r], hi[r]) of every row r
 // (offsets relative to the row start; null = row start / row end), starts from the fp32 partial sums of the previous phases
 // (part_in, nullable) and either hands fp32 partials on (part_out) or scales and stores the finished row.

@@ -39,9 +39,8 @@ import torch.distributed as dist
 
 Tensor = torch.Tensor
 
-# Column chunks of the all-gather / SpMM pipeline of the `allgather` mode (1 = one blocking all-gather per SpMM).  Measured on
-# 2 B200s at the products shape (profiles/r1_scaling.md): 60.1 ms/step with 1 chunk, 61.2 with 2, 61.3 with 4 - NCCL's all-gather
-# kernels need SMs that the HBM-bound SpMM grid already fills; hence the copy-engine `push` mode.
+# Column chunks of the all-gather / SpMM pipeline of the `allgather` mode (1 = one blocking all-gather per SpMM).  More chunks do
+# not overlap: NCCL's all-gather kernels need SMs that the HBM-bound SpMM grid already fills; hence the copy-engine `push` mode.
 C4_CHUNKS = int(os.environ.get("SGF_C4_CHUNKS", "1"))
 C4_MIN_CHUNK_BYTES = 256      # gathered rows stay >= two full 128-byte lines per neighbour
 C4_MODE = os.environ.get("SGF_C4_MODE", "auto")
@@ -306,16 +305,14 @@ class Comm:
                 r = (rank - s) % w
                 K.memcpy_async(peers[r][s * b:s * b + n_loc], own)               # copy-engine peer copy over NVLink
                 # ... and the arrival flag behind it, ALSO by the copy engine: a 1-thread flag kernel of another stream is never
-                # scheduled while a consumer kernel holds the SMs spinning on that flag (measured on B200: tests/push_debug2.py
+                # scheduled while a consumer kernel holds the SMs spinning on that flag (tests/push_debug2.py
                 # stages S1/P2 trap, S2/P1 pass), whereas stream-ordered copy-engine writes need no SM
                 K.memcpy_async(st.peer_flags[r][k, s:s + 1], st.one)
             done = torch.cuda.Event()
             done.record(st.side)
         flags = st.flags[k]
-        # phased vs in-row waiting (measured, profiles/r2_scaling.md): the phases pay one fp32 write + read of the partial sums per
-        # boundary and shorter per-row gathers, the in-row wait overlaps nothing.  ms/step, phased vs flagged: products (512-byte
-        # rows) 49.8 / 49.7 at 2 GPUs, 29.9 / 30.9 at 4, 17.6 / 21.6 at 8; Pokec (128-byte rows) 7.8 / 7.1 at 2, 5.7 / 4.6 at 4,
-        # 3.4 / 3.5 at 8
+        # phased vs in-row waiting: the phases pay one fp32 write + read of the partial sums per boundary and shorter per-row
+        # gathers, the in-row wait overlaps nothing
         rowbytes = x_local.shape[1] * x_local.element_size()
         phased = self._groups_forced > 1 or (self._groups_forced == 0 and ((w >= 4 and rowbytes >= 512) or w >= 8))
         if self.c4_mode == "push-flagged" or heavy is not None or not phased:

@@ -1,11 +1,11 @@
-"""Hand-scheduled forward / backward of the SGFormer encoder on the sm_100a kernels.
+"""Hand-scheduled forward / backward of the SGFormer encoder on the sm_90a kernels.
 
 One schedule per branch — `trans_*` (TransConv: input MLP + linear-attention layers), `gconv_*` (GraphConv of
 large/100M), `gcn_*` (PyG-GCN backbone of medium), `head_*` (branch mix + fc) — each a forward that records what the
 backward needs in a `Tape`, and a backward that walks the tape and fills a gradient dict keyed by the reference's
 parameter names.  There is no autograd inside: torch.autograd sees a single Function (functional.py) per call.
 
-Reference semantics reproduced (paths into /root/reference): large/ours.py:25-42 (GraphConvLayer), :74-94 (GraphConv,
+Reference semantics reproduced (paths in the reference repository): large/ours.py:25-42 (GraphConvLayer), :74-94 (GraphConv,
 incl. the "residual always adds layer_[0]" quirk), :121-162 / medium/ours.py:14-46,74-100 (TransConvLayer +
 full_attention_conv), :194-219 / medium/ours.py:133-160 / 100M/ours.py:247-272 (TransConv, the two residual rules),
 medium/models.py:49-63 (GCN over PyG GCNConv), large/ours.py:265-276 (SGFormer.forward).

@@ -1,9 +1,9 @@
 """Host -> device input staging that overlaps the copy of step i+1 with the compute of step i.
 
 The reference moves the whole dataset to the device once (`large/main.py:83-85`) or, in the mini-batch driver, copies each
-batch synchronously inside the loop (`large/main-batch.py:141-143`: `x_i = x[idx_i].to(device)`).  On a B200 a full-batch
-products-shaped step is ~100 ms of compute and ~55 ms of PCIe traffic (3 GB of features and int64 edge indices), so a
-synchronous copy costs a third of the step; `HostFeeder` hides it behind the previous step with a second CUDA stream and
+batch synchronously inside the loop (`large/main-batch.py:141-143`: `x_i = x[idx_i].to(device)`).  A full-batch
+products-shaped step moves 3 GB of features and int64 edge indices over PCIe, a large share of the step when copied
+synchronously; `HostFeeder` hides it behind the previous step with a second CUDA stream and
 two persistent device slots (no allocation, no host synchronisation per step).
 """
 from __future__ import annotations

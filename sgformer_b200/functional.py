@@ -251,7 +251,7 @@ class AttentionFn(_TapeFunction):
 
 
 class LinearFn(Function):
-    """y = x W^T + b on the tcgen05 GEMMs (nn.Linear forward / backward)."""
+    """y = x W^T + b on the wgmma GEMMs (nn.Linear forward / backward)."""
 
     @staticmethod
     def forward(ctx, x, w, b, prec):

@@ -1,7 +1,7 @@
 """Graph structure cache: CSR of the GCN aggregation pattern (+ lazily its transpose) built once per edge list.
 
 The reference rebuilds degree -> edge weights -> sort -> CSR inside every GraphConvLayer.forward
-(/root/reference/large/ours.py:26-33); it is graph-constant, so it is hoisted here and keyed on the edge_index tensor."""
+(reference large/ours.py:26-33); it is graph-constant, so it is hoisted here and keyed on the edge_index tensor."""
 from __future__ import annotations
 
 from collections import OrderedDict

@@ -416,6 +416,20 @@ def operand_from_bf16(x: Tensor) -> Operand:
     return Operand(x, rows, k, k, 1)
 
 
+_red_bytes = {}
+
+
+def _red_ws(width: int, dev):
+    """Workspace of a launcher that sums across thread blocks in a fixed order (sgf_reduce_ws_bytes) -> (ptr, bytes); one per
+    call, so that calls on different streams never share it."""
+    if width not in _red_bytes:
+        n = C.c_size_t(0)
+        check(lib().sgf_reduce_ws_bytes(width, C.byref(n)), "sgf_reduce_ws_bytes")
+        _red_bytes[width] = n.value
+    ws = torch.empty(_red_bytes[width], dtype=torch.uint8, device=dev)
+    return ws, _red_bytes[width]
+
+
 def pack_operand(src: Tensor, transpose: bool = False, planes: int = 1, colsum: Optional[Tensor] = None,
                  row_index: Optional[Tensor] = None) -> Operand:
     """fp32 [r, c] -> bf16 Operand ([c, r] if transpose).  planes=3: bf16x3 split (fp32-accurate products).
@@ -432,8 +446,9 @@ def pack_operand(src: Tensor, transpose: bool = False, planes: int = 1, colsum: 
     rows_out, cols_out = (c, r) if transpose else (r, c)
     kp = ceil_to(cols_out, 64) if planes == 3 else ceil_to(cols_out, 8)
     dst = torch.empty((rows_out, kp * planes), dtype=torch.bfloat16, device=src.device)
+    ws, nws = _red_ws(c, src.device) if colsum is not None else (None, 0)
     check(lib().sgf_pack_operand(_p(src), ld, r, c, int(transpose), _p(dst), dst.stride(0), kp, kp if planes == 3 else 0,
-                                 _p(colsum), _p(row_index), _stream()), "sgf_pack_operand")
+                                 _p(colsum), _p(row_index), _p(ws), nws, _stream()), "sgf_pack_operand")
     return Operand(dst, rows_out, cols_out, kp, planes)
 
 
@@ -547,8 +562,8 @@ def gemm_nt(A: Sequence[Operand], B: Sequence[Operand], pairs: Sequence[Tuple[in
 # 0 auto / 1 stream B through the TMA ring / 2 B resident in shared memory (include/sgformer_b200.h: sgf_gemm_nt_args.schedule)
 GEMM_NT_SCHEDULE = int(os.environ.get("SGF_GEMM_NT_SCHEDULE", "0"))
 
-# Measured on B200 (products shape): accumulating the statistics in the GEMM epilogue costs more epilogue issue slots than the
-# separate 0.31 ms colstats pass it saves (105.3 vs 101.4 ms/step), so the fused path is opt-in.
+# Accumulating the statistics in the GEMM epilogue costs epilogue issue slots that can exceed the separate colstats pass it
+# saves, so the fused path is opt-in.
 FUSE_GEMM_STATS = os.environ.get("SGF_FUSED_STATS", "0") == "1"
 
 
@@ -611,8 +626,9 @@ def colstats(x: Tensor, w: Optional[Tensor] = None, want_sum: bool = True, want_
     blk = 2048 // x.element_size()      # the row kernels cover at most 2 KB of a row per launch
     for c0 in range(0, h, blk):
         c1 = min(h, c0 + blk)
+        ws, nws = _red_ws(c1 - c0, x.device)
         check(lib().sgf_colstats(_p(x[:, c0:c1]), ld, rows, c1 - c0, dcode(x), _p(wv), _p(s[c0:c1] if s is not None else None),
-                                 _p(q[c0:c1] if q is not None else None), _stream()), "sgf_colstats")
+                                 _p(q[c0:c1] if q is not None else None), _p(ws), nws, _stream()), "sgf_colstats")
     return s, q
 
 
@@ -642,8 +658,10 @@ def ln_bwd(dy: Tensor, x: Tensor, r: Optional[Tensor], a: float, b: float, gamma
     dx = new_like(x)
     dr = new_like(x) if want_dr else None
     _same_ld(ld, dy, r, dx, dr)
+    ws, nws = _red_ws(h, x.device)
     check(lib().sgf_ln_bwd(_p(dy), _p(x), _p(r), ld, rows, h, dcode(x), a, b, _p(gamma), _p(beta), _p(stats), int(use_ln),
-                           int(use_relu), p, seed, gscale, _p(dx), _p(dr), _p(dgamma), _p(dbeta), _stream()), "sgf_ln_bwd")
+                           int(use_relu), p, seed, gscale, _p(dx), _p(dr), _p(dgamma), _p(dbeta), _p(ws), nws, _stream()),
+          "sgf_ln_bwd")
     return dx, dr
 
 
@@ -661,9 +679,11 @@ def ln_bwd_attn(dy: Tensor, o: Tensor, r: Optional[Tensor], xa: Tensor, a: float
     gden = torch.empty(rows, dtype=torch.float32, device=dev)
     acc = torch.zeros(2 * h + 1, dtype=torch.float32, device=dev)
     cs, pg, sg = acc[:h], acc[h:2 * h], acc[2 * h:]
+    ws, nws = _red_ws(h, dev)
     check(lib().sgf_ln_bwd_attn(_p(dy), _p(o), _p(r), _p(xa), ld, rows, h, dcode(o), a, b, _p(gamma), _p(beta), _p(stats),
                                 int(use_ln), int(use_relu), p, seed, gscale, _p(_f32vec(den, rows, "den")), _p(gnum), _p(gden),
-                                _p(dr), _p(dgamma), _p(dbeta), _p(cs), _p(pg), _p(sg), _stream()), "sgf_ln_bwd_attn")
+                                _p(dr), _p(dgamma), _p(dbeta), _p(cs), _p(pg), _p(sg), _p(ws), nws, _stream()),
+          "sgf_ln_bwd_attn")
     return gnum, gden, dr, cs, pg, sg
 
 
@@ -709,10 +729,11 @@ def bn_bwd(dy: Optional[Tensor], dy2: Optional[Tensor], row_scale2: Optional[Ten
         if reduce_fn is not None:
             reduce_fn(sums)
     colsum = torch.zeros(h, dtype=torch.float32, device=z.device) if want_dz_colsum else None
+    ws, nws = _red_ws(h, z.device)
     check(lib().sgf_bn_bwd_apply(_p(dy), _p(dy2), _p(row_scale2), _p(z), ld, rows, h, dcode(z), _p(mean), _p(rstd),
                                  _p(gamma), _p(beta), _p(zbias), int(use_bn), int(use_relu), int(training), p, seed,
                                  gscale, int(stat_rows), _p(sums), _p(dz), _p(dres), int(dres_accumulate), _p(colsum),
-                                 _p(out_row_scale), _stream()), "sgf_bn_bwd_apply")
+                                 _p(out_row_scale), _p(ws), nws, _stream()), "sgf_bn_bwd_apply")
     return dz, sums, colsum
 
 
@@ -723,9 +744,10 @@ def bn_bwd_sums(dy, dy2, row_scale2, z: Tensor, mean, rstd, gamma, beta, zbias, 
     rows, h, ld = _mat(z, "z")
     _same_ld(ld, dy, dy2)
     sums = torch.zeros(2 * h, dtype=torch.float32, device=z.device)
+    ws, nws = _red_ws(h, z.device)
     check(lib().sgf_bn_bwd_reduce(_p(dy), _p(dy2), _p(row_scale2), _p(z), ld, rows, h, dcode(z), _p(mean), _p(rstd),
                                   _p(gamma), _p(beta), _p(zbias), int(use_bn), int(use_relu), p, seed, gscale, _p(sums),
-                                  _stream()), "sgf_bn_bwd_reduce")
+                                  _p(ws), nws, _stream()), "sgf_bn_bwd_reduce")
     return sums
 
 
@@ -932,8 +954,9 @@ def softmax_nll(logits: Tensor, labels: Tensor, mask: Optional[Tensor], scale: f
         m = mask.reshape(-1).to(torch.uint8).contiguous()
     loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
     d = torch.empty((rows, c), dtype=torch.float32, device=logits.device) if want_grad else None
-    check(lib().sgf_softmax_nll(_p(logits), ld, _p(labels), _p(m), rows, c, scale, _p(loss), _p(d), c, _stream()),
-          "sgf_softmax_nll")
+    ws, nws = _red_ws(1, logits.device)
+    check(lib().sgf_softmax_nll(_p(logits), ld, _p(labels), _p(m), rows, c, scale, _p(loss), _p(d), c, _p(ws), nws,
+                                _stream()), "sgf_softmax_nll")
     return loss, d
 
 

@@ -1,5 +1,5 @@
 """Drop-in for the reference's large/ours.py (`--method sgformer`, large/parse.py:35-39): same classes, constructor
-and forward signatures, attribute names and state_dict keys; computation on the sm_100a kernels."""
+and forward signatures, attribute names and state_dict keys; computation on the sm_90a kernels."""
 import torch
 import torch.nn as nn
 import torch.nn.functional as F

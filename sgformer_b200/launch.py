@@ -1,4 +1,4 @@
-"""Run an UNMODIFIED reference training script with the B200 `ours.py` in front of its own:
+"""Run an UNMODIFIED reference training script with the H100 `ours.py` in front of its own:
 
     python -m sgformer_b200.launch --variant large /path/to/SGFormer/large/main-batch.py --method sgformer --dataset pokec ...
 

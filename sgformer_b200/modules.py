@@ -30,7 +30,7 @@ def default_precision() -> str:
 
 def _require_cuda(what: str):
     if not torch.cuda.is_available():
-        raise RuntimeError(f"sgformer_b200: {what} needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError(f"sgformer_b200: {what} needs a CUDA device (sm_90a); there is no CPU fallback")
 
 
 class _Base(nn.Module):

@@ -1,10 +1,11 @@
-"""Helpers to import the UNMODIFIED reference modules from /root/reference through tests/ref_shims.
-Test infrastructure; only usable in the build container (the GPU box has no /root/reference)."""
+"""Helpers to import the UNMODIFIED reference modules from a reference checkout (SGFORMER_REFERENCE,
+default ../reference beside this repository) through tests/ref_shims, for tests/make_golden.py; the tests themselves use the committed fixtures."""
 import importlib
 import os
 import sys
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("SGFORMER_REFERENCE",
+                          os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "reference"))
 SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_shims")
 _VARIANT_DIR = {"large": "large", "100M": "100M", "medium": "medium"}
 

@@ -4,7 +4,7 @@
 
 Each fixture holds seeded inputs, the state_dict, and the reference's outputs / gradients.
 The committed fixtures are what pins oracle/ (tests/test_oracle_golden.py) and what the `-m gpu`
-parity tests compare the CUDA path with on the GPU box (which has no /root/reference)."""
+parity tests compare the CUDA path with, without a reference checkout."""
 import os
 import sys
 
@@ -226,6 +226,7 @@ def graph_prep_cases():
         full, _ = add_self_loops(nsl, num_nodes=n)
         out[name] = dict(n=n, edge_index=ei, to_undirected=und, remove_self_loops_raw=remove_self_loops(ei)[0],
                          add_self_loops_raw=add_self_loops(ei, num_nodes=n)[0], prepared=full)
+    out = {k: {kk: v.to(torch.int32) if torch.is_tensor(v) else v for kk, v in c.items()} for k, c in out.items()}   # < 1 MB
     torch.save(out, os.path.join(GOLD, "graph_prep.pt"))
     print("graph_prep", {k: tuple(v["prepared"].shape) for k, v in out.items()})
 
@@ -246,9 +247,103 @@ def get_attentions_cases():
     torch.save(out, os.path.join(GOLD, "get_attentions.pt"))
 
 
+def property_graph(n, e, seed, directed, isolated, dup, loops):
+    g = torch.Generator().manual_seed(seed)
+    hi = max(n - isolated, 1)
+    ei = torch.stack([torch.randint(0, hi, (e,), generator=g), torch.randint(0, hi, (e,), generator=g)])
+    if not directed:
+        ei = torch.cat([ei, ei.flip(0)], 1)
+    if dup:
+        ei = torch.cat([ei, ei[:, :dup]], 1)
+    if loops:
+        ar = torch.arange(hi)
+        ei = torch.cat([ei, torch.stack([ar, ar])], 1)
+    return ei
+
+
+def oracle_property_cases(count=25):
+    """Randomly drawn configurations and graphs (isolated nodes, directed/asymmetric edges, duplicates, self loops, odd sizes,
+    1-4 heads; fixed seed) with the outputs of the reference, eval and train mode: pins oracle/ (tests/test_oracle_vs_reference.py)."""
+    import random
+    rnd = random.Random(0)
+    out = []
+    for _ in range(count):
+        variant, n, h = rnd.choice(["large", "100M", "medium"]), rnd.randint(5, 90), rnd.choice([8, 16, 24])
+        heads, seed, directed = rnd.choice([1, 2, 4]), rnd.randint(0, 10 ** 6), rnd.random() < 0.5
+        isolated, dup, loops = rnd.randint(0, 3), rnd.randint(0, 9), rnd.random() < 0.5
+        flags = [rnd.random() < 0.5 for _ in range(9)]
+        aggregate, layers, tlayers = rnd.choice(["add", "cat"]), rnd.randint(1, 3), rnd.randint(1, 2)
+        d, c = 7, 4
+        use_weight = flags[0] or heads > 1        # use_weight=False forces one head (medium/ours.py:84)
+        if variant == "medium":
+            cfg = O.make_config("medium", d, h, c, num_layers=tlayers, num_heads=heads, alpha=0.3, dropout=0.0, use_bn=flags[1],
+                                use_residual=flags[2], use_weight=use_weight, gcn_num_layers=layers + 1, gcn_dropout=0.0,
+                                gcn_use_bn=flags[3], graph_weight=0.7, aggregate=aggregate)
+        else:
+            kw = dict(trans_num_layers=tlayers, trans_num_heads=heads, trans_dropout=0.0, trans_use_bn=flags[1],
+                      trans_use_residual=flags[2], trans_use_weight=use_weight, trans_use_act=flags[4], gnn_num_layers=layers,
+                      gnn_dropout=0.0, gnn_use_weight=flags[5], gnn_use_init=flags[6], gnn_use_bn=flags[3], gnn_use_residual=flags[7],
+                      gnn_use_act=flags[8], graph_weight=0.7, aggregate=aggregate)
+            if variant == "100M":
+                kw["alpha"] = 0.3
+            cfg = O.make_config(variant, d, h, c, **kw)
+        torch.manual_seed(seed)
+        model, _ = build_reference_model(variant, cfg)
+        sd = {k: v.clone() for k, v in model.state_dict().items()}
+        ei = property_graph(n, 3 * n, seed, directed, isolated, dup, loops)
+        x = torch.randn(n, d, generator=torch.Generator().manual_seed(seed + 1))
+        ref = {}
+        for training in (False, True):
+            model.train(training)
+            with torch.no_grad():
+                ref[training] = run_reference(variant, model, x, ei).clone()
+            model.load_state_dict(sd)   # undo BatchNorm running-stat updates
+        out.append(dict(cfg=cfg, state_dict=sd, edge_index=ei, x=x, ref_eval=ref[False], ref_train=ref[True]))
+    torch.save(out, os.path.join(GOLD, "oracle_property.pt"))
+    print("oracle_property", len(out))
+
+
+def parse_large_case():
+    """The SGFormer constructor call that the reference's own large/parse.py makes for the amazon2m recipe of large/run.sh:15-19
+    (positional and keyword arguments as data): tests/test_dropin_plumbing.py replays it against the drop-in."""
+    import argparse
+    import importlib
+    import json
+    from _refload import REF_ROOT, SHIMS
+    for name in ("parse", "ours", "gnns"):
+        sys.modules.pop(name, None)
+    saved = list(sys.path)
+    sys.path[:0] = [SHIMS, os.path.join(REF_ROOT, "large")]
+    try:
+        parse = importlib.import_module("parse")
+    finally:
+        sys.path[:] = saved
+    calls = []
+
+    class Record:
+        def __init__(self, *a, **kw):
+            calls.append(dict(args=list(a), kwargs=kw))
+
+        def to(self, device):
+            return self
+
+    parse.SGFormer = Record
+    argv = ("--method sgformer --hidden_channels 256 --gnn_num_layers 3 --gnn_dropout 0. --gnn_use_residual --gnn_use_weight "
+            "--gnn_use_bn --gnn_use_init --gnn_use_act --trans_num_layers 1 --trans_dropout 0. --trans_use_residual "
+            "--trans_use_weight --trans_use_bn --use_graph --graph_weight 0.5")
+    p = argparse.ArgumentParser()
+    parse.parser_add_main_args(p)
+    parse.parse_method(p.parse_args(argv.split()), 47, 100, "cpu")
+    assert len(calls) == 1
+    with open(os.path.join(GOLD, "parse_large_sgformer.json"), "w") as f:
+        json.dump(dict(argv=argv, **calls[0]), f, indent=1, sort_keys=True)
+        f.write("\n")
+    print("parse_large", calls[0])
+
+
 if __name__ == "__main__":
-    if len(sys.argv) > 1 and sys.argv[1] == "get_attentions":      # add this fixture without regenerating the others
-        get_attentions_cases()
+    if len(sys.argv) > 1 and sys.argv[1] in ("get_attentions", "oracle_property", "parse_large"):   # add one fixture, keep the others
+        {"get_attentions": get_attentions_cases, "oracle_property": oracle_property_cases, "parse_large": parse_large_case}[sys.argv[1]]()
         sys.exit(0)
     os.makedirs(GOLD, exist_ok=True)
     for nm, sp in CASES.items():
@@ -258,3 +353,5 @@ if __name__ == "__main__":
     evaluate_cases()
     graph_prep_cases()
     get_attentions_cases()
+    oracle_property_cases()
+    parse_large_case()

@@ -29,7 +29,7 @@ def test_library_builds_loads_and_exports_everything():
         assert hasattr(lib, s), f"libsgformer_b200.so does not export {s}"
     assert set(declared_symbols()) == set(_lib._SIGS), "ctypes signature table and header disagree"
     lib.sgf_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.sgf_version()
+    assert b"sm_90a" in lib.sgf_version()
 
 
 def test_struct_layouts_match_the_header():

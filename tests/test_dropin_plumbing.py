@@ -1,13 +1,10 @@
-"""The drop-in `ours.py` files export the reference's names and the reference's own parse.py builds OUR model through
-them (build container only: needs /root/reference; construction is CPU-safe, no compute)."""
-import argparse
+"""The drop-in `ours.py` files export the reference's names and build our model from the reference's recorded constructor call
+(construction is CPU-safe, no compute)."""
 import importlib
 import os
 import sys
 
 import pytest
-
-from _refload import REF_ROOT, SHIMS, reference_available
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -37,36 +34,16 @@ def test_dropin_exports(variant, names):
     assert mod.SGFormer.__module__.startswith("sgformer_b200")
 
 
-@pytest.mark.skipif(not reference_available(), reason="needs /root/reference (build container)")
 def test_reference_parse_builds_our_model_large():
-    parse = _import_from([os.path.join(ROOT, "sgformer_b200", "dropin", "large"), SHIMS, os.path.join(REF_ROOT, "large")], "parse")
-    p = argparse.ArgumentParser()
-    parse.parser_add_main_args(p)
-    # large/run.sh:15-19 (amazon2m recipe)
-    args = p.parse_args("--method sgformer --hidden_channels 256 --gnn_num_layers 3 --gnn_dropout 0. --gnn_use_residual "
-                        "--gnn_use_weight --gnn_use_bn --gnn_use_init --gnn_use_act --trans_num_layers 1 --trans_dropout 0. "
-                        "--trans_use_residual --trans_use_weight --trans_use_bn --use_graph --graph_weight 0.5".split())
-    model = parse.parse_method(args, 47, 100, "cpu")
+    """The constructor call of the reference's own large/parse.py for the amazon2m recipe (large/run.sh:15-19), recorded in
+    tests/golden/parse_large_sgformer.json by tests/make_golden.py parse_large, builds the drop-in model with that config."""
+    import json
+    with open(os.path.join(ROOT, "tests", "golden", "parse_large_sgformer.json")) as f:
+        call = json.load(f)
+    ours = _import_from([os.path.join(ROOT, "sgformer_b200", "dropin", "large")], "ours")
+    model = ours.SGFormer(*call["args"], **call["kwargs"]).to("cpu")
     assert type(model).__module__ == "sgformer_b200.large"
     cfg = model._cfg()
     assert cfg["gnn_use_init"] and cfg["gnn_num_layers"] == 3 and cfg["hidden"] == 256 and cfg["graph_weight"] == 0.5
     assert cfg["trans_use_act"] is False and cfg["trans_use_bn"] is True
     assert len(model.params1) > 0 and len(model.params2) > 0
-
-
-@pytest.mark.skipif(not reference_available(), reason="needs /root/reference (build container)")
-def test_reference_parse_builds_our_model_medium():
-    parse = _import_from([os.path.join(ROOT, "sgformer_b200", "dropin", "medium"), SHIMS, os.path.join(REF_ROOT, "medium")], "parse")
-    p = argparse.ArgumentParser()
-    parse.parser_add_main_args(p)
-    parse.parser_add_default_args(p.parse_args([])) if False else None
-    # medium/run.sh:2-8 (Cora recipe)
-    args = p.parse_args("--backbone gcn --dataset cora --lr 0.01 --num_layers 4 --hidden_channels 64 --weight_decay 5e-4 "
-                        "--dropout 0.5 --method ours --ours_layers 1 --use_graph --graph_weight 0.8 --ours_dropout 0.2 "
-                        "--use_residual --alpha 0.5 --ours_weight_decay 0.001".split())
-    parse.parser_add_default_args(args)
-    model = parse.parse_method(args.method, args, 7, 1433, "cpu")
-    assert type(model).__module__ == "sgformer_b200.medium"
-    from sgformer_b200.medium import _is_gcn_like
-    assert _is_gcn_like(model.gnn), "the reference's models.GCN (over the PyG shim) must be recognised for the fused path"
-    assert model.trans_conv.residual is False  # run.sh passes --use_residual (GNN flag), not --ours_use_residual

@@ -1,4 +1,4 @@
-"""Kernel-level parity on the B200: every C-ABI kernel against the oracle / its documented semantics.
+"""Kernel-level parity on the H100: every C-ABI kernel against the oracle / its documented semantics.
 
 Integer work (CSR build, subgraph) is compared bit-exactly with the numpy / C oracle; floating-point kernels against
 fp64 numpy (SpMM, attention contractions) or the torch-CPU statement of the kernel contract (tests/kernel_emu.py,
@@ -467,7 +467,7 @@ def test_pack_operand(K):
 
 
 # ------------------------------------------------------------------------------------------------
-# tcgen05 GEMMs
+# wgmma GEMMs
 # ------------------------------------------------------------------------------------------------
 def _ops(K, a, b, planes):
     """CUDA + emulated operands for fp32 sources a [rows,k], b [n,k]."""
@@ -847,3 +847,29 @@ def test_spmm_range_phases_equal_the_whole(K, dtype, h):
     _close(out.float(), whole.float(), tol, tol, "phased SpMM vs single launch")
     ref = emu.spmm(rpe, cle, dve, x.cpu())
     _close(out.float(), ref.float(), 2e-5 if dtype == torch.float32 else 2e-2, 1e-5, "phased SpMM vs contract")
+
+
+def test_cross_block_reductions_are_deterministic(K):
+    """Column sums and the loss reduced across thread blocks are bit-identical from run to run (blocks add in a fixed order,
+    no float atomics), so two runs of a training step compute the same."""
+    g = torch.Generator().manual_seed(11)
+    rows = 300_000
+    x = torch.randn(rows, 256, generator=g).to(DEV)
+    logits = torch.randn(rows, 47, generator=g).to(DEV)
+    y = torch.randint(0, 47, (rows,), generator=g).to(DEV)
+    for xx in (x, x.to(torch.bfloat16)):
+        a, b = K.colstats(xx), K.colstats(xx)
+        assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1]), "colstats"
+    l1, l2 = K.softmax_nll(logits, y, None, 1.0 / rows)[0], K.softmax_nll(logits, y, None, 1.0 / rows)[0]
+    assert torch.equal(l1, l2), "softmax_nll loss"
+    c1, c2 = torch.zeros(256, device=DEV), torch.zeros(256, device=DEV)
+    K.pack_operand(x, False, 1, colsum=c1)
+    K.pack_operand(x, False, 1, colsum=c2)
+    assert torch.equal(c1, c2), "pack_operand column sums"
+    _close(c1, x.double().sum(0).float(), 1e-5, 1e-3, "pack_operand column sums vs fp64")
+    xt = x[:5000].t().contiguous()                  # [256, 5000]: the column sums of the source are the row sums of x[:5000]
+    ct1, ct2 = torch.zeros(5000, device=DEV), torch.zeros(5000, device=DEV)
+    K.pack_operand(xt, True, 1, colsum=ct1)
+    K.pack_operand(xt, True, 1, colsum=ct2)
+    assert torch.equal(ct1, ct2), "transposed pack_operand column sums"
+    _close(ct1, x[:5000].double().sum(1).float(), 1e-5, 1e-3, "transposed pack_operand column sums vs fp64")

@@ -1,4 +1,4 @@
-"""Module-level parity on the B200: the drop-in nn.Modules against the golden fixtures generated from the unmodified
+"""Module-level parity on the H100: the drop-in nn.Modules against the golden fixtures generated from the unmodified
 reference (tests/make_golden.py) and against the CPU oracle on fresh seeded graphs.
 fp32 precision: 1e-4; bf16 precision: 1e-2 (BASELINE.json north_star)."""
 import glob

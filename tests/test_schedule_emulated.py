@@ -1,6 +1,6 @@
 """Checks the forward/backward *schedules* (sgformer_b200/engine.py + functional.py) against the golden fixtures of
 the reference, with the CUDA kernels replaced by their torch-CPU emulation (tests/kernel_emu.py).  Runs without a GPU.
-The kernels themselves are verified on the B200 by the `-m gpu` tests."""
+The kernels themselves are verified on the H100 by the `-m gpu` tests."""
 import glob
 import os
 
