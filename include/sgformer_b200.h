@@ -261,6 +261,11 @@ int sgf_colstats(const void* x, int64_t ldx, int64_t rows, int h, int dtype, con
 int sgf_ln_fwd(const void* x, const void* r, int64_t ld, int64_t rows, int h, int dtype, float a, float b,
                const float* gamma, const float* beta, int use_ln, int use_relu, float p, uint64_t seed,
                void* y, float* stats, void* stream);
+/* sgf_ln_fwd with a third input: u = a*x + b*r + c*gy (gy non-NULL, same dtype and pitch).  A DIFFormer layer
+ * (medium/difformer.py:129-137,202-206) mixes its attention output x, the previous layer r and the graph term gy = Â v here. */
+int sgf_ln_fwd_graph(const void* x, const void* r, const void* gy, int64_t ld, int64_t rows, int h, int dtype, float a, float b,
+                     float c, const float* gamma, const float* beta, int use_ln, int use_relu, float p, uint64_t seed, void* y,
+                     float* stats, void* stream);
 /* backward of sgf_ln_fwd for the upstream gradient gscale*dy: writes dx = a*du and (if dr != NULL) dr = b*du;
  * accumulates dgamma[c], dbeta[c] (fp32, caller-zeroed, nullable when !use_ln). */
 int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t ld, int64_t rows, int h, int dtype,
@@ -409,6 +414,11 @@ typedef struct {
 int sgf_attn_gram_ws_floats(int h, int m, int d, int64_t* n_floats /* host out */);
 int sgf_attn_gram_prepare_fwd(const sgf_attn_gram_args* args /* host */, void* stream);
 int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* args /* host */, void* stream);
+/* Value-sum mode (DIFFormer's `simple` kernel, medium/difformer.py:18-39): the numerator adds the column sum sum_l v_l instead of
+ * N v_n.  Same arguments and outputs as above, with  Bt = beta S^T Wq,  bt = beta S^T bq + v1/N  in the forward and
+ *   dWv = beta dS^T kx + cs s^T / N,   a4 += Wv^T cs / N     (everything else unchanged)  in the backward. */
+int sgf_attn_gram_prepare_fwd_vsum(const sgf_attn_gram_args* args /* host */, void* stream);
+int sgf_attn_gram_prepare_bwd_vsum(const sgf_attn_gram_args* args /* host */, void* stream);
 /* Dropout epoch.  Every kernel that takes (p, seed) draws its mask from hash(seed + epoch * odd, row, chunk); `epoch` is read from
  * the device word registered here (NULL, the default: epoch 0).  The host seed of a call is frozen into a captured CUDA graph;
  * a step that is captured and replayed registers an epoch word and puts sgf_advance_dropout_epoch at the top of the captured
@@ -426,6 +436,13 @@ int sgf_ln_bwd_attn(const void* dy, const void* o, const void* r, const void* xa
                     float p, uint64_t seed, float gscale, const float* den, void* gnum, float* gden, void* dr, float* dgamma,
                     float* dbeta, float* cs, float* pg, float* sg, void* ws,
                     size_t ws_bytes, void* stream);
+/* sgf_ln_bwd_attn for u = a*o + b*r + c*gy (sgf_ln_fwd_graph; no ReLU): additionally writes ys[r,:] = dinv[r] * c * du[r,:],
+ * the pre-scaled operand of the transposed SpMM that carries the gradient of the graph term gy = Â v back to v. */
+int sgf_ln_bwd_attn_graph(const void* dy, const void* o, const void* r, const void* xa, const void* gy, int64_t ld, int64_t rows, int h, int dtype,
+                          float a, float b, float c, const float* gamma, const float* beta, const float* stats, int use_ln, float p,
+                          uint64_t seed, float gscale, const float* den, const float* dinv, void* gnum, float* gden, void* dr,
+                          void* ys, float* dgamma, float* dbeta, float* cs, float* pg, float* sg, void* ws, size_t ws_bytes,
+                          void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused two-group Adam (SURVEY.md §8f-3; replaces torch.optim.Adam([{params1, trans_weight_decay}, {params2,

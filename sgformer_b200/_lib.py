@@ -120,11 +120,18 @@ _SIGS = {
                              _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sgf_ln_bwd_attn": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _f32, _f32, _vp, _vp, _vp, C.c_int, C.c_int,
                                   _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "sgf_ln_fwd_graph": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _f32, _f32, _f32, _vp, _vp, C.c_int, C.c_int,
+                                   _f32, _u64, _vp, _vp, _vp]),
+    "sgf_ln_bwd_attn_graph": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _f32, _f32, _f32, _vp, _vp, _vp,
+                                        C.c_int, _f32, _u64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _sz, _vp]),
     "sgf_gram_ws_bytes": (C.c_int, [_i32, _i32, _i64, C.POINTER(_sz)]),
     "sgf_gram": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i64, _vp, _i64, _vp, _vp, _sz, _vp]),
     "sgf_attn_gram_ws_floats": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(_i64)]),
     "sgf_attn_gram_prepare_fwd": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
     "sgf_attn_gram_prepare_bwd": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
+    "sgf_attn_gram_prepare_fwd_vsum": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
+    "sgf_attn_gram_prepare_bwd_vsum": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
     "sgf_adam_step": (C.c_int, [C.POINTER(AdamArgs), _vp]),
     "sgf_bn_finalize": (C.c_int, [_vp, _vp, _i64, C.c_int, _f32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sgf_bn_fwd": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int,

@@ -18,6 +18,9 @@
 //     dx  = gnum' Bt + x A3 + gden' (x) ct + 1 (x) a4,   A3 = cq Wq^T Wq + ck Wk^T Wk + beta (Wk^T dS Wv + (Wk^T dS Wv)^T),
 //     a4  = cq Wq^T bq + ck Wk^T bk + beta (Wk^T (dz + dS bv) + Wv^T dS^T bk)
 // (checked against autograd of the reference formula in fp64: tests/test_gram_attention_math.py).
+// Value-sum mode (DIFFormer's `simple` kernel, medium/difformer.py:18-39: the numerator adds sum_l v_l instead of N v_n):
+//     Bt = beta S^T Wq,  bt = beta S^T bq + v1/N;   dWv = beta dS^T kx + cs s^T / N,  a4 += Wv^T cs / N;  the rest is unchanged
+// (tests/test_difformer.py checks it, with the graph term of the layer, against autograd in fp64).
 // Everything here is O(h^3) work on matrices of at most a few hundred rows: one generic batched small-GEMM kernel
 // (several independent products per launch), a batched dot-product kernel and two scalar kernels.
 #include "common.cuh"
@@ -236,7 +239,7 @@ extern "C" int sgf_attn_gram_ws_floats(int h, int m, int d, int64_t* n_floats) {
     return SGF_OK;
 }
 
-extern "C" int sgf_attn_gram_prepare_fwd(const sgf_attn_gram_args* a, void* stream) {
+static int prepare_fwd(const sgf_attn_gram_args* a, bool vsum, void* stream) {
     if (!args_ok(a) || !a->ws) return SGF_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     const int h = a->h, m = a->m, d = a->d;
@@ -276,15 +279,19 @@ extern "C" int sgf_attn_gram_prepare_fwd(const sgf_attn_gram_args* a, void* stre
     SGF_LAUNCH_CHECK(); count_launch();
     {   // level 3: operands of the apply GEMM
         BatchBuilder bb;
-        { Op& o = bb.add(d, h, a->Bt, h); prod1(o, cf(1.f, beta), matT(a->S, d), mat(a->wq, a->ld_wq), m); addend(o, cf(1.f), mat(a->wv, a->ld_wv)); }
+        // value-sum mode: no per-node N v term in Bt; bt gains sum_l v_l / N = v1 / N, which already contains bv
+        { Op& o = bb.add(d, h, a->Bt, h); prod1(o, cf(1.f, beta), matT(a->S, d), mat(a->wq, a->ld_wq), m);
+          if (!vsum) addend(o, cf(1.f), mat(a->wv, a->ld_wv)); }
         { Op& o = bb.add(h, 1, a->tail, 1); prod1(o, cf(1.f, beta), matT(a->wq, a->ld_wq), vec(a->z1), m); }
-        { Op& o = bb.add(d, 1, a->bt, 1); prod1(o, cf(1.f, beta), matT(a->S, d), vec(a->bq), m); addend(o, cf(1.f), vec(a->bv)); }
+        { Op& o = bb.add(d, 1, a->bt, 1); prod1(o, cf(1.f, beta), matT(a->S, d), vec(a->bq), m);
+          if (vsum) addend(o, cf((float)(1.0 / (double)a->n_nodes)), vec(a->v1));
+          else addend(o, cf(1.f), vec(a->bv)); }
         if ((rc = bb.launch(st))) return rc;
     }
     return SGF_OK;
 }
 
-extern "C" int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* a, void* stream) {
+static int prepare_bwd(const sgf_attn_gram_args* a, bool vsum, void* stream) {
     if (!args_ok(a) || !a->P || !a->pg || !a->cs || !a->sg || !a->dwq || !a->dbq || !a->dwk || !a->dbk || !a->dwv || !a->dbv ||
         !a->bcat || !a->a4 || !a->ws)
         return SGF_ERR_ARG;
@@ -303,12 +310,14 @@ extern "C" int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* a, void* stre
     float* part = a->ws + (need - MAX_OPS * DOT_SPLIT);
     const int64_t ldc = d + h;       // pitch of bcat = [Bt^T | A3]
     float* A3 = a->bcat + d;
+    const float inv_n = (float)(1.0 / (double)a->n_nodes);
     int rc;
-    {   // level 1: dS, dz; the Bt^T half of the dx operand
+    {   // level 1: dS, dz; the Bt^T half of the dx operand (value-sum mode: a4 starts as Wv^T cs / N)
         BatchBuilder bb;
         { Op& o = bb.add(m, d, dS, d); prod1(o, cf(1.f), mat(a->wq, a->ld_wq), mat(a->P, d), h); rank1(o, cf(1.f), a->bq, 1, a->cs, 1); }
         { Op& o = bb.add(m, 1, dz, 1); prod1(o, cf(1.f), mat(a->wq, a->ld_wq), vec(a->pg), h); rank1(o, cf(1.f), a->bq, 1, a->sg, 0); }
         { Op& o = bb.add(h, d, a->bcat, ldc); addend(o, cf(1.f), matT(a->Bt, h)); }
+        if (vsum) { Op& o = bb.add(h, 1, a->a4, 1); prod1(o, cf(inv_n), matT(a->wv, a->ld_wv), vec(a->cs), d); }
         if ((rc = bb.launch(st))) return rc;
     }
     {   // level 2: c = beta (<dS,S> + <dz,z1>);  U = dS Wv, t1 = dS bv + dz, t2 = dS^T bk
@@ -334,12 +343,14 @@ extern "C" int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* a, void* stre
           rank1(o, cf(1.f, beta), dz, 1, a->s, 1); }
         { Op& o = bb.add(m, 1, a->dbk, 1); prod1(o, cf(1.f, beta), mat(dS, d), vec(a->v1), d); addend(o, cf(1.f, ck), vec(a->z1));
           rank1(o, cf(1.f, alpha), dz, 1, one, 0); }
-        { Op& o = bb.add(d, h, a->dwv, h); prod1(o, cf(1.f, beta), matT(dS, d), mat(a->kx, h), m); addend(o, cf(1.f), matT(a->P, d)); }
+        { Op& o = bb.add(d, h, a->dwv, h); prod1(o, cf(1.f, beta), matT(dS, d), mat(a->kx, h), m);
+          if (vsum) rank1(o, cf(inv_n), a->cs, 1, a->s, 1);      // d(sum_l v_l / N) instead of d(v_n)
+          else addend(o, cf(1.f), matT(a->P, d)); }
         { Op& o = bb.add(d, 1, a->dbv, 1); prod1(o, cf(1.f, beta), matT(dS, d), vec(a->z1), m); addend(o, cf(1.f), vec(a->cs)); }
         { Op& o = bb.add(h, h, A3, ldc); prod1(o, cf(1.f, cq), matT(a->wq, a->ld_wq), mat(a->wq, a->ld_wq), m);
           prod2(o, cf(1.f, ck), matT(a->wk, a->ld_wk), mat(a->wk, a->ld_wk), m); }
         { Op& o = bb.add(h, 1, a->a4, 1); prod1(o, cf(1.f, cq), matT(a->wq, a->ld_wq), vec(a->bq), m);
-          prod2(o, cf(1.f, ck), matT(a->wk, a->ld_wk), vec(a->bk), m); }
+          prod2(o, cf(1.f, ck), matT(a->wk, a->ld_wk), vec(a->bk), m); if (vsum) addend(o, cf(1.f), vec(a->a4)); }
         if ((rc = bb.launch(st))) return rc;
     }
     {   // level 4: A3 += beta (Wk^T U + U^T Wk),  a4 += beta (Wk^T t1 + Wv^T t2)     (E aliases C: read-then-write per element)
@@ -352,3 +363,8 @@ extern "C" int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* a, void* stre
     }
     return SGF_OK;
 }
+
+extern "C" int sgf_attn_gram_prepare_fwd(const sgf_attn_gram_args* a, void* stream) { return prepare_fwd(a, false, stream); }
+extern "C" int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* a, void* stream) { return prepare_bwd(a, false, stream); }
+extern "C" int sgf_attn_gram_prepare_fwd_vsum(const sgf_attn_gram_args* a, void* stream) { return prepare_fwd(a, true, stream); }
+extern "C" int sgf_attn_gram_prepare_bwd_vsum(const sgf_attn_gram_args* a, void* stream) { return prepare_bwd(a, true, stream); }

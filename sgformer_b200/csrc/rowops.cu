@@ -265,13 +265,13 @@ __global__ void __launch_bounds__(kRowBlock, (colstats_live<T, CPL>() > 56 ? 2 :
 }
 
 // ------------------------------------------------------------------------------------------------
-// LayerNorm family.  u = a*x + b*r; t = LN?(u); t = relu?(t); y = dropout(t)
-template <typename T, int CPL, bool DROP>
+// LayerNorm family.  u = a*x + b*r (+ c*gy when GY); t = LN?(u); t = relu?(t); y = dropout(t)
+template <typename T, int CPL, bool DROP, bool GY = false>
 __global__ void __launch_bounds__(kRowBlock, 3) ln_fwd_kernel(const T* __restrict__ x, const T* __restrict__ rr, int64_t ld, int64_t rows,
                                                             int h, int chunks, int lpr_log2, float a, float b,
                                                             const float* __restrict__ gamma, const float* __restrict__ beta, int use_ln,
                                                             int use_relu, float p, SeedArg seed_arg, T* __restrict__ y,
-                                                            float* __restrict__ stats) {
+                                                            float* __restrict__ stats, const T* __restrict__ gyy = nullptr, float cy = 0.f) {
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     Lane<T, CPL> L(chunks, lpr_log2);
@@ -301,6 +301,17 @@ __global__ void __launch_bounds__(kRowBlock, 3) ln_fwd_kernel(const T* __restric
             SGF_FOR_ELEMS u[c][i] = a * u[c][i] + b * t[c][i];
         } else {
             SGF_FOR_ELEMS u[c][i] = a * u[c][i];
+        }
+        if (GY) {                        // the graph term of a DIFFormer layer (not prefetched: it is read once)
+            uint4 ny[CPL];
+            if (live) L.load_raw(gyy, ld, r, ny);
+            else {
+#pragma unroll
+                for (int c = 0; c < CPL; ++c) ny[c] = make_uint4(0u, 0u, 0u, 0u);
+            }
+            float t[CPL][VN];
+            L.unpack(ny, t);
+            SGF_FOR_ELEMS u[c][i] += cy * t[c][i];
         }
         {
             const int64_t rn = r + L.row_step;
@@ -430,7 +441,7 @@ __global__ void __launch_bounds__(kRowBlock, 3) ln_bwd_kernel(const T* __restric
 // and the column sums cs = sum_r gnum'[r,:], pg = sum_r xa[r,:]*gden'[r], sg = sum_r gden'[r] that the h x h backward algebra
 // needs (sgf_attn_gram_prepare_bwd) accumulate in registers like dgamma / dbeta.  xa = the attention layer's input (== r when
 // the layer has a residual connection: then it is not loaded twice).
-template <typename T, int CPL, bool DROP, bool RELU, int MINB>
+template <typename T, int CPL, bool DROP, bool RELU, int MINB, bool GY = false>
 __global__ void __launch_bounds__(kRowBlock, (CPL >= 2 ? 1 : MINB)) ln_bwd_attn_kernel(const T* __restrict__ dy, const T* __restrict__ o, const T* __restrict__ rr,
                                                                     const T* __restrict__ xa, int64_t ld, int64_t rows, int h, int chunks,
                                                                     int lpr_log2, float a, float b, const float* __restrict__ gamma,
@@ -440,7 +451,9 @@ __global__ void __launch_bounds__(kRowBlock, (CPL >= 2 ? 1 : MINB)) ln_bwd_attn_
                                                                     float* __restrict__ gden, T* __restrict__ dr,
                                                                     float* __restrict__ dgamma, float* __restrict__ dbeta,
                                                                     float* __restrict__ cs, float* __restrict__ pg, float* __restrict__ sg,
-                                                                    RedWs red) {
+                                                                    RedWs red, const T* __restrict__ gyy = nullptr,
+                                                                    const float* __restrict__ dinv = nullptr, float cy = 0.f,
+                                                                    T* __restrict__ ys = nullptr) {
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     extern __shared__ float sm[];
@@ -483,6 +496,17 @@ __global__ void __launch_bounds__(kRowBlock, (CPL >= 2 ? 1 : MINB)) ln_bwd_attn_
             SGF_FOR_ELEMS u[c][i] = a * u[c][i] + b * t[c][i];
         } else {
             SGF_FOR_ELEMS u[c][i] = a * u[c][i];
+        }
+        if (GY) {                        // u also holds c*y (the forward's graph term)
+            uint4 ny[CPL];
+            if (live) L.load_raw(gyy, ld, r, ny);
+            else {
+#pragma unroll
+                for (int c = 0; c < CPL; ++c) ny[c] = make_uint4(0u, 0u, 0u, 0u);
+            }
+            float t[CPL][VN];
+            L.unpack(ny, t);
+            SGF_FOR_ELEMS u[c][i] += cy * t[c][i];
         }
         if (!xa_is_r) {
             if (live) L.load_raw(xa, ld, r, cr);
@@ -534,6 +558,11 @@ __global__ void __launch_bounds__(kRowBlock, (CPL >= 2 ? 1 : MINB)) ln_bwd_attn_
         if (live && dr) {
             SGF_FOR_ELEMS u[c][i] = b * gy[c][i];
             L.store(dr, ld, r, u);
+        }
+        if (GY && live) {                // dinv (.) (c*du): the operand of the transposed SpMM of the graph term
+            const float sr = cy * dinv[r];
+            SGF_FOR_ELEMS u[c][i] = sr * gy[c][i];
+            L.store(ys, ld, r, u);
         }
         // attention-backward prologue on ga = a*du
         L.unpack(co, u);                 // o again
@@ -1264,6 +1293,24 @@ extern "C" int sgf_ln_fwd(const void* x, const void* r, int64_t ld, int64_t rows
     return SGF_OK;
 }
 
+extern "C" int sgf_ln_fwd_graph(const void* x, const void* r, const void* gy, int64_t ld, int64_t rows, int h, int dtype, float a,
+                                float b, float c, const float* gamma, const float* beta, int use_ln, int use_relu, float p,
+                                uint64_t seed, void* y, float* stats, void* stream) {
+    RowGeom g;
+    if (!geom_for(dtype, h, g) || !x || !gy || !aligned16(x) || !aligned16(gy) || !aligned16(y) || !aligned16(r) || !ld_ok(dtype, ld) ||
+        rows < 0)
+        return SGF_ERR_ARG;
+    if (use_ln && (!gamma || !beta)) return SGF_ERR_ARG;
+    if (p < 0.f || p >= 1.f) return SGF_ERR_ARG;
+    if (rows == 0) return SGF_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (ln_fwd_kernel<T, CPL, DROP, true><<<row_grid(rows, g), kRowBlock, 0, st>>>(
+                                         (const T*)x, (const T*)r, ld, rows, h, g.chunks, g.lpr_log2, a, b, gamma, beta, use_ln,
+                                         use_relu, p, seed, (T*)y, stats, (const T*)gy, c)));
+    SGF_LAUNCH_CHECK(); count_launch();
+    return SGF_OK;
+}
+
 extern "C" int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t ld, int64_t rows, int h, int dtype, float a,
                           float b, const float* gamma, const float* beta, const float* stats, int use_ln, int use_relu, float p,
                           uint64_t seed, float gscale, void* dx, void* dr, float* dgamma, float* dbeta, void* ws, size_t ws_bytes,
@@ -1317,6 +1364,29 @@ extern "C" int sgf_ln_bwd_attn(const void* dy, const void* o, const void* r, con
                                              gamma, beta, stats, use_ln, p, seed, gscale, den, (T*)gnum, gden, (T*)dr, dgamma,
                                              dbeta, cs, pg, sg, red)));
     }
+    SGF_LAUNCH_CHECK(); count_launch();
+    return SGF_OK;
+}
+
+extern "C" int sgf_ln_bwd_attn_graph(const void* dy, const void* o, const void* r, const void* xa, const void* gy, int64_t ld, int64_t rows, int h,
+                                     int dtype, float a, float b, float c, const float* gamma, const float* beta, const float* stats,
+                                     int use_ln, float p, uint64_t seed, float gscale, const float* den, const float* dinv,
+                                     void* gnum, float* gden, void* dr, void* ys, float* dgamma, float* dbeta, float* cs, float* pg,
+                                     float* sg, void* ws, size_t ws_bytes, void* stream) {
+    RowGeom g;
+    if (!geom_for(dtype, h, g) || !aligned16(o) || !aligned16(dy) || !aligned16(gnum) || !aligned16(r) || !aligned16(dr) ||
+        !aligned16(xa) || !aligned16(gy) || !aligned16(ys) || !ld_ok(dtype, ld) || rows < 0)
+        return SGF_ERR_ARG;
+    if (!o || !dy || !xa || !gy || !den || !dinv || !gnum || !gden || !ys || !cs || !pg || !sg) return SGF_ERR_ARG;
+    if (use_ln && (!gamma || !beta || !stats)) return SGF_ERR_ARG;
+    if (rows == 0) return SGF_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
+    SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (ln_bwd_attn_kernel<T, CPL, DROP, false, 2, true><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
+                                         (const T*)dy, (const T*)o, (const T*)r, (const T*)xa, ld, rows, h, g.chunks, g.lpr_log2, a, b,
+                                         gamma, beta, stats, use_ln, p, seed, gscale, den, (T*)gnum, gden, (T*)dr, dgamma,
+                                         dbeta, cs, pg, sg, red, (const T*)gy, dinv, c, (T*)ys)));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }

@@ -207,8 +207,9 @@ def _identity_v(h: int, dev):
 
 
 def attention_gram_forward(P: Dict[str, Tensor], lp: str, x: Tensor, use_weight: bool, prec: Precision, tape: Optional[Tape],
-                           comm: Comm = SINGLE) -> Tensor:
-    """x: [N, h] layer input (activation) -> full_attention_conv(Wq x, Wk x, Wv x) [N, h], one head."""
+                           comm: Comm = SINGLE, vsum: bool = False) -> Tensor:
+    """x: [N, h] layer input (activation) -> full_attention_conv(Wq x, Wk x, Wv x) [N, h], one head.
+    vsum=True: DIFFormer's `simple` kernel (numerator + sum_l v_l instead of + N v_n, medium/difformer.py:18-39)."""
     n_loc, h = x.shape
     n = comm.n_global if comm.active else n_loc
     dev = x.device
@@ -216,7 +217,8 @@ def attention_gram_forward(P: Dict[str, Tensor], lp: str, x: Tensor, use_weight:
     G, s = K.gram(xop, x)
     comm.allreduce_(G, s)                                     # C1: h*h + h floats
     wv, bv = (P[lp + "Wv.weight"], P[lp + "Wv.bias"]) if use_weight else _identity_v(h, dev)
-    st = K.attn_gram_prepare_fwd(G, s, P[lp + "Wq.weight"], P[lp + "Wq.bias"], P[lp + "Wk.weight"], P[lp + "Wk.bias"], wv, bv, n)
+    prepare = K.attn_gram_prepare_fwd_vsum if vsum else K.attn_gram_prepare_fwd
+    st = prepare(G, s, P[lp + "Wq.weight"], P[lp + "Wq.bias"], P[lp + "Wk.weight"], P[lp + "Wk.bias"], wv, bv, n)
     bop = K.pack_operand(st.Bt, False, prec.planes)
     btail = K.pack_operand(st.tail, False, prec.planes)
     d = st.Bt.shape[0]
@@ -764,3 +766,215 @@ def head_backward(P, cfg: dict, tape: Tape, dlogits: Tensor, prec: Precision, gr
         outs.append(dj)
     grads["fc.weight"], grads["fc.bias"] = dw, db
     return outs
+
+
+# =================================================================================================
+# DIFFormer (medium/difformer.py, kernel='simple', one head)
+# =================================================================================================
+# Layer i:  o = Gram-form attention in value-sum mode (sgf_attn_gram_prepare_fwd_vsum),  y = Â v  with v = x Wv^T + bv
+# (gcn_conv, medium/difformer.py:63-79: in-degree normalisation over the edge targets, no self loops = Graph(self_loop_mode=0)),
+#   u = a*o + b*r + c*y,   x' = dropout(LN?(u))                                          (sgf_ln_fwd_graph)
+# with a, c the branch weights times alpha and b = 1-alpha (use_residual, r = layer input).  use_source adds alpha * x0 to u:
+# r = (1-alpha) x + alpha x0 (one extra row pass for layers after the first).  Backward: sgf_ln_bwd_attn_graph writes the attention
+# prologue and dinv (.) (c du); the transposed SpMM of that is dv, which adds dv^T x to dWv, 1^T dv to dbv and dv Wv to dx (a third
+# segment of the dx GEMM).
+def _difformer_coefs(cfg: dict, i: int):
+    """-> (a, b, c, s): u = a*o + b*r + c*y + s*x0 of layer i."""
+    gw = float(cfg["graph_weight"])
+    if not cfg["use_graph"]:
+        ca, cy = 1.0, 0.0
+    elif gw > 0:
+        ca, cy = 1.0 - gw, gw
+    else:
+        ca, cy = 1.0, 1.0
+    al = float(cfg["alpha"])
+    ka, kb = (al, 1.0 - al) if cfg["use_residual"] else (1.0, 0.0)
+    ks = ka if cfg["use_source"] else 0.0
+    return ka * ca, kb, ka * cy, ks
+
+
+def _difformer_v_scaled(P, lp: str, x: Tensor, use_weight: bool, prec: Precision, dinv: Tensor) -> Tensor:
+    """dinv (.) v: the pre-scaled SpMM operand of the graph term (row-scale epilogue of the V projection)."""
+    if not use_weight:
+        return K.axpby(x, None, 1.0, 0.0, row_scale=dinv)
+    h = x.shape[1]
+    return K.gemm_nt([K.as_operand(x, prec.planes, memo=True)], [_w(P, lp + "Wv.weight", prec)], [(0, 0, 0, 0, h)],
+                     P[lp + "Wv.weight"].shape[0], K.new_like(x), bias=P[lp + "Wv.bias"], row_scale=dinv)
+
+
+def difformer_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, graph: Optional[Graph], prec: Precision, training: bool,
+                      seed: int, tape: Optional[Tape]) -> Tensor:
+    """DIFFormer.forward (medium/difformer.py:184-211) -> fp32 logits [N, out_channels]."""
+    h, d_in, c_out, nl = cfg["hidden"], cfg["in_channels"], cfg["out_channels"], cfg["num_layers"]
+    check_width(h, prec, "hidden_channels")
+    n = xin.rows
+    dev = xin.data.device
+    p = float(cfg["dropout"]) if training else 0.0
+    use_ln, use_weight, use_graph = bool(cfg["use_bn"]), bool(cfg["use_weight"]), bool(cfg["use_graph"])
+    t0 = K.gemm_nt([xin], [_w(P, "fcs.0.weight", prec)], [(0, 0, 0, 0, d_in)], h, K.alloc_act(n, h, prec.act_dtype, dev),
+                   bias=P["fcs.0.bias"])
+    x, st0 = K.ln_fwd(t0, None, 1.0, 0.0, P.get("bns.0.weight"), P.get("bns.0.bias"), use_ln, True, p, seed + 101, tape is not None)
+    x0 = x
+    layers = []
+    for i in range(nl):
+        lp = f"convs.{i}."
+        a, b, c, s_ = _difformer_coefs(cfg, i)
+        at = Tape() if tape is not None else None
+        o = attention_gram_forward(P, lp, x, use_weight, prec, at, vsum=True)
+        if s_ and i > 0:
+            r, b = K.axpby(x, x0, b, s_), 1.0
+        elif s_ or b:
+            r, b = x, b + s_          # layer 0: x0 is the layer input
+        else:
+            r = None
+        gamma, beta = P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias")
+        if use_graph:
+            y = K.spmm(graph.rowptr, graph.col, graph.dinv, _difformer_v_scaled(P, lp, x, use_weight, prec, graph.dinv),
+                       heavy=graph.heavy)
+            xn, st = K.ln_fwd_graph(o, r, y, a, b, c, gamma, beta, use_ln, False, p, seed + 211 + i, tape is not None)
+        else:
+            xn, st = K.ln_fwd(o, r, a, b, gamma, beta, use_ln, False, p, seed + 211 + i, tape is not None)
+        layers.append(dict(x_in=x, attn=at, o=o, r=r, y=y if use_graph else None, st=st, coef=(a, b, c)))
+        x = xn
+    xop = K.as_operand(x, prec.planes)
+    logits = K.gemm_nt([xop], [_w(P, "fcs.1.weight", prec)], [(0, 0, 0, 0, h)], c_out,
+                       K.alloc_act(n, c_out, torch.float32, dev), bias=P["fcs.1.bias"])
+    if tape is not None:
+        tape.update(xin=xin, t0=t0, st0=st0, layers=layers, p=p, seed=seed, n=n, xop=xop)
+    return logits
+
+
+def difformer_backward(P: Dict[str, Tensor], cfg: dict, tape: Tape, graph: Optional[Graph], dlogits: Tensor, prec: Precision,
+                       grads: Dict[str, Tensor], want_dx: bool = False) -> Optional[Tensor]:
+    h, d_in, c_out, nl = cfg["hidden"], cfg["in_channels"], cfg["out_channels"], cfg["num_layers"]
+    n, p, seed = tape["n"], tape["p"], tape["seed"]
+    dev = dlogits.device
+    use_ln, use_weight, use_graph = bool(cfg["use_bn"]), bool(cfg["use_weight"]), bool(cfg["use_graph"])
+
+    def zeros(k):
+        return torch.zeros(k, dtype=torch.float32, device=dev)
+
+    # output Linear
+    dlogits = dlogits.contiguous().float()
+    db1 = zeros(c_out)
+    dl_op = K.pack_operand(dlogits, False, prec.planes, colsum=db1)
+    dw1 = torch.empty((c_out, h), dtype=torch.float32, device=dev)
+    K.gemm_tn(dl_op, tape["xop"], dw1)
+    grads["fcs.1.weight"], grads["fcs.1.bias"] = dw1, db1
+    dcur = K.alloc_act(n, h, prec.act_dtype, dev)
+    K.gemm_nt([dl_op], [_w(P, "fcs.1.weight", prec, transpose=True)], [(0, 0, 0, 0, c_out)], h, dcur)
+    gs = 1.0
+    dx0 = None                     # use_source: gradient of x0 collected from layers 1..L-1
+    if use_graph:
+        rp_t, col_t = graph.transpose()
+    for i in reversed(range(nl)):
+        L = tape["layers"][i]
+        lp = f"convs.{i}."
+        a, b, c = L["coef"]
+        _, _, _, s_ = _difformer_coefs(cfg, i)
+        x_in, at, r = L["x_in"], L["attn"], L["r"]
+        gamma, beta = P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias")
+        dg, db = (zeros(h), zeros(h)) if use_ln else (None, None)
+        if use_graph:
+            gnum, gden, dr, ys, cs, pg, sg = K.ln_bwd_attn_graph(dcur, L["o"], r, x_in, L["y"], a, b, c, gamma, beta, L["st"], use_ln, p,
+                                                                 seed + 211 + i, gs, r is not None, dg, db, at["den"], graph.dinv)
+        else:
+            gnum, gden, dr, cs, pg, sg = K.ln_bwd_attn(dcur, L["o"], r, x_in, a, b, gamma, beta, L["st"], use_ln, False, p,
+                                                       seed + 211 + i, gs, r is not None, dg, db, at["den"])
+        if use_ln:
+            grads[f"bns.{i + 1}.weight"], grads[f"bns.{i + 1}.bias"] = dg, db
+        # gradient of the layer input from r
+        kb = 1.0 - float(cfg["alpha"]) if cfg["use_residual"] else 0.0
+        if s_ and i > 0:           # r = kb*x + s*x0, b = 1: dr = du
+            dx0 = K.axpby(dr, dx0, s_, 1.0) if dx0 is not None else K.axpby(dr, None, s_, 0.0)
+            dprev, acc = (K.axpby(dr, None, kb, 0.0), True) if kb else (K.new_like(x_in), False)
+        elif r is not None:
+            dprev, acc = dr, True
+        else:
+            dprev, acc = K.new_like(x_in), False
+        # attention (value-sum Gram form) + graph term
+        st = at["st"]
+        d = gnum.shape[1]
+        gnum_op = K.as_operand(gnum, prec.planes)
+        pmat = torch.empty((h, d), dtype=torch.float32, device=dev)
+        K.gemm_tn(at["xop"], gnum_op, pmat)
+        dwq, dbq, dwk, dbk, dwv, dbv, bcat, a4 = K.attn_gram_prepare_bwd(st, pmat, pg, cs, sg)
+        grads[lp + "Wq.weight"], grads[lp + "Wq.bias"] = dwq, dbq
+        grads[lp + "Wk.weight"], grads[lp + "Wk.bias"] = dwk, dbk
+        A, B = [gnum_op, at["xop"]], [K.pack_operand(bcat, False, prec.planes)]
+        pairs = [(0, 0, 0, 0, d), (1, 0, 0, d, h)]
+        dv_pair = None
+        if use_graph:
+            dv = K.spmm(rp_t, col_t, graph.dinv, ys, heavy=graph.heavy_t)       # dinv (.) A^T (dinv (.) c du)
+            dv_op = K.as_operand(dv, prec.planes)
+            if use_weight:
+                K.gemm_tn(dv_op, at["xop"], dwv, beta=1.0)
+                K.colstats(dv, want_sumsq=False, sum_out=dbv)
+            wv = P[lp + "Wv.weight"] if use_weight else _identity_v(h, dev)[0]
+            A.append(dv_op)
+            B.append(K.pack_operand(wv, True, prec.planes))
+            dv_pair = (2, 0, 1, 0, d)
+            if prec.planes == 1:            # dv Wv as a third segment of the dx GEMM
+                pairs.append(dv_pair)
+                dv_pair = None
+        if use_weight:
+            grads[lp + "Wv.weight"], grads[lp + "Wv.bias"] = dwv, dbv
+        K.gemm_nt(A, B, pairs, h, dprev, bias=a4, r1_row=gden, r1_col=st.tail[0], accumulate=acc)
+        if dv_pair is not None:         # bf16x3: 3 x 6 partial products exceed the GEMM's 16 segments
+            K.gemm_nt([A[2]], [B[1]], [(0, 0, 0, 0, d)], h, dprev, accumulate=True)
+        if i == 0 and dx0 is not None:
+            dprev = K.axpby(dprev, dx0, 1.0, 1.0)
+        dcur, gs = dprev, 1.0
+    dg, db = (zeros(h), zeros(h)) if use_ln else (None, None)
+    dt0, _ = K.ln_bwd(dcur, tape["t0"], None, 1.0, 0.0, P.get("bns.0.weight"), P.get("bns.0.bias"), tape["st0"], use_ln, True, p,
+                      seed + 101, gs, False, dg, db)
+    if use_ln:
+        grads["bns.0.weight"], grads["bns.0.bias"] = dg, db
+    dt0_op = K.as_operand(dt0, prec.planes)
+    dw0 = torch.empty((h, d_in), dtype=torch.float32, device=dev)
+    K.gemm_tn(dt0_op, tape["xin"], dw0)
+    grads["fcs.0.weight"] = dw0
+    grads["fcs.0.bias"], _ = K.colstats(dt0, want_sumsq=False)
+    if want_dx:
+        dx = torch.empty((n, d_in), dtype=torch.float32, device=dev)
+        K.gemm_nt([dt0_op], [_w(P, "fcs.0.weight", prec, transpose=True)], [(0, 0, 0, 0, h)], d_in, dx)
+        return dx
+    return None
+
+
+def difformer_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precision) -> List[Tensor]:
+    """DIFFormer.get_attentions (medium/difformer.py:213-228) for use_graph=False: per layer the [N, N] matrix
+    q~ k~^T / (q~ . sum_l k~_l + N).  The N x N product is one tensor-core GEMM of q and k with alpha = 1/(||q|| ||k||) read from
+    the device and 1/den as its row scale (trans_attentions); the layer stack runs the Gram form.  Inference only, O(N^2) memory
+    like the reference: meant for small graphs."""
+    h, d_in, nl = cfg["hidden"], cfg["in_channels"], cfg["num_layers"]
+    check_width(h, prec, "hidden_channels")
+    n = xin.rows
+    dev = xin.data.device
+    use_ln, use_weight = bool(cfg["use_bn"]), bool(cfg["use_weight"])
+    t0 = K.gemm_nt([xin], [_w(P, "fcs.0.weight", prec)], [(0, 0, 0, 0, d_in)], h, K.alloc_act(n, h, prec.act_dtype, dev),
+                   bias=P["fcs.0.bias"])
+    x, _ = K.ln_fwd(t0, None, 1.0, 0.0, P.get("bns.0.weight"), P.get("bns.0.bias"), use_ln, True, 0.0, 0, False)
+    x0 = x
+    out = []
+    for i in range(nl):
+        lp = f"convs.{i}."
+        a, b, _, s_ = _difformer_coefs(cfg, i)
+        at = Tape()
+        o = attention_gram_forward(P, lp, x, use_weight, prec, at, vsum=True)
+        wqk, bqk = torch.cat([P[lp + "Wq.weight"], P[lp + "Wk.weight"]], 0), torch.cat([P[lp + "Wq.bias"], P[lp + "Wk.bias"]], 0)
+        qk = torch.empty((n, K.ceil_to(2 * h, 8)), dtype=prec.act_dtype, device=dev)[:, :2 * h]
+        K.gemm_nt([K.as_operand(x, prec.planes)], [K.pack_operand(wqk, False, prec.planes)], [(0, 0, 0, 0, h)], 2 * h, qk, bias=bqk)
+        inv_den = at["den"].reciprocal()        # [N]: the Gram denominator is the reference's normaliser / N
+        att = K.alloc_act(n, n, torch.float32, dev)
+        K.gemm_nt([K.as_operand(qk[:, :h], prec.planes)], [K.as_operand(qk[:, h:], prec.planes)], [(0, 0, 0, 0, h)], n, att,
+                  alpha=1.0 / at["n"], alpha_dev=at["st"].sc[K.SC_ALPHA:K.SC_ALPHA + 1], row_scale=inv_den)
+        out.append(att)
+        if s_ and i > 0:
+            r, b = K.axpby(x, x0, b, s_), 1.0
+        elif s_ or b:
+            r, b = x, b + s_
+        else:
+            r = None
+        x, _ = K.ln_fwd(o, r, a, b, P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias"), use_ln, False, 0.0, 0, False)
+    return out

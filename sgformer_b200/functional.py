@@ -140,6 +140,33 @@ class SGFormerFn(_TapeFunction):
         return (dx, None, None, None, None, None, None, *_grad_list(names, params, grads))
 
 
+class DIFFormerFn(_TapeFunction):
+    """DIFFormer (medium/difformer.py:147-211, kernel='simple', one head): input MLP, Gram-form attention layers with the graph
+    term, output Linear in one schedule (engine.difformer_forward / _backward).  Returns fp32 logits [N, c]."""
+
+    @staticmethod
+    def forward(ctx, x: Tensor, graph: Optional[Graph], cfg: dict, prec: E.Precision, training: bool, names, *params):
+        P = _pdict(names, params)
+        need_tape = _want_tape(ctx)
+        K.operand_memo_begin()
+        tape = E.Tape() if need_tape else None
+        logits = E.difformer_forward(P, cfg, E.input_operand(x, prec), graph, prec, training, E.next_seed(), tape)
+        if need_tape:
+            ctx.state = (cfg, prec, graph, names, params, tape, x.requires_grad)
+        else:
+            K.operand_memo_clear()
+        return logits
+
+    @staticmethod
+    def backward(ctx, dlogits: Tensor):
+        cfg, prec, graph, names, params, tape, want_dx = ctx.state
+        grads: Dict[str, Tensor] = {}
+        dx = E.difformer_backward(_pdict(names, params), cfg, tape, graph, dlogits, prec, grads, want_dx=want_dx)
+        ctx.state = None
+        K.operand_memo_clear()
+        return (dx, None, None, None, None, None, *_grad_list(names, params, grads))
+
+
 class TransConvFn(_TapeFunction):
     """Standalone TransConv branch.  Returns [N, h] in x's dtype."""
 

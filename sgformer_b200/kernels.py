@@ -617,10 +617,12 @@ def gemm_tn(A: Operand, B: Operand, out: Tensor, *, transpose_out: bool = False,
 # ------------------------------------------------------------------------------------------------
 # row-streaming kernels
 # ------------------------------------------------------------------------------------------------
-def colstats(x: Tensor, w: Optional[Tensor] = None, want_sum: bool = True, want_sumsq: bool = True):
+def colstats(x: Tensor, w: Optional[Tensor] = None, want_sum: bool = True, want_sumsq: bool = True,
+             sum_out: Optional[Tensor] = None):
+    """-> (column sums | None, column sums of squares | None).  sum_out (fp32 [h]): the sums are added to it instead."""
     _use(x)
     rows, h, ld = _mat(x, "x")
-    s = torch.zeros(h, dtype=torch.float32, device=x.device) if want_sum else None
+    s = sum_out if sum_out is not None else (torch.zeros(h, dtype=torch.float32, device=x.device) if want_sum else None)
     q = torch.zeros(h, dtype=torch.float32, device=x.device) if want_sumsq else None
     wv = _f32vec(w, rows, "w")
     blk = 2048 // x.element_size()      # the row kernels cover at most 2 KB of a row per launch
@@ -685,6 +687,42 @@ def ln_bwd_attn(dy: Tensor, o: Tensor, r: Optional[Tensor], xa: Tensor, a: float
                                 _p(dr), _p(dgamma), _p(dbeta), _p(cs), _p(pg), _p(sg), _p(ws), nws, _stream()),
           "sgf_ln_bwd_attn")
     return gnum, gden, dr, cs, pg, sg
+
+
+def ln_fwd_graph(x: Tensor, r: Optional[Tensor], gy: Tensor, a: float, b: float, c: float, gamma: Optional[Tensor],
+                 beta: Optional[Tensor], use_ln: bool, use_relu: bool, p: float, seed: int, want_stats: bool = True):
+    """ln_fwd of u = a*x + b*r + c*gy (sgf_ln_fwd_graph): the row pass of a DIFFormer layer."""
+    _use(x)
+    rows, h, ld = _mat(x, "x")
+    y = new_like(x)
+    _same_ld(ld, r, gy, y)
+    stats = torch.empty((rows, 2), dtype=torch.float32, device=x.device) if (use_ln and want_stats) else None
+    check(lib().sgf_ln_fwd_graph(_p(x), _p(r), _p(gy), ld, rows, h, dcode(x), a, b, c, _p(gamma), _p(beta), int(use_ln),
+                                 int(use_relu), p, seed, _p(y), _p(stats), _stream()), "sgf_ln_fwd_graph")
+    return y, stats
+
+
+def ln_bwd_attn_graph(dy: Tensor, o: Tensor, r: Optional[Tensor], xa: Tensor, gy: Tensor, a: float, b: float, c: float, gamma, beta, stats,
+                      use_ln: bool, p: float, seed: int, gscale: float, want_dr: bool, dgamma: Optional[Tensor],
+                      dbeta: Optional[Tensor], den: Tensor, dinv: Tensor):
+    """ln_bwd_attn for u = a*o + b*r + c*gy, also writing ys = dinv (.) (c*du) (sgf_ln_bwd_attn_graph).
+    -> (gnum' [rows,h], gden' fp32 [rows], dr | None, ys [rows,h], cs [h], pg [h], sg [1])."""
+    _use(o)
+    rows, h, ld = _mat(o, "o")
+    gnum = new_like(o)
+    ys = new_like(o)
+    dr = new_like(o) if want_dr else None
+    _same_ld(ld, dy, r, xa, gy, gnum, dr, ys)
+    dev = o.device
+    gden = torch.empty(rows, dtype=torch.float32, device=dev)
+    acc = torch.zeros(2 * h + 1, dtype=torch.float32, device=dev)
+    cs, pg, sg = acc[:h], acc[h:2 * h], acc[2 * h:]
+    ws, nws = _red_ws(h, dev)
+    check(lib().sgf_ln_bwd_attn_graph(_p(dy), _p(o), _p(r), _p(xa), _p(gy), ld, rows, h, dcode(o), a, b, c, _p(gamma), _p(beta), _p(stats),
+                                      int(use_ln), p, seed, gscale, _p(_f32vec(den, rows, "den")), _p(_f32vec(dinv, rows, "dinv")),
+                                      _p(gnum), _p(gden), _p(dr), _p(ys), _p(dgamma), _p(dbeta), _p(cs), _p(pg), _p(sg), _p(ws),
+                                      nws, _stream()), "sgf_ln_bwd_attn_graph")
+    return gnum, gden, dr, ys, cs, pg, sg
 
 
 def bn_finalize(sum_: Optional[Tensor], sumsq: Optional[Tensor], rows: int, h: int, zbias: Optional[Tensor],
@@ -864,7 +902,7 @@ def gram(xop: Operand, x: Tensor):
 class GramState:
     """fp32 device tensors written by sgf_attn_gram_prepare_fwd and re-read by its backward (h x h algebra on the weights)."""
     __slots__ = ("wq", "bq", "wk", "bk", "wv", "bv", "G", "s", "kx", "qx", "vx", "z1", "q1", "v1", "S", "Bt", "tail", "bt", "sc",
-                 "n", "h", "m", "d", "ws")
+                 "n", "h", "m", "d", "ws", "vsum")
 
 
 def _w2(t: Tensor, name: str) -> Tensor:
@@ -886,11 +924,13 @@ def _gram_args(st: GramState) -> AttnGramArgs:
 
 
 def attn_gram_prepare_fwd(G: Tensor, s: Tensor, wq: Tensor, bq: Tensor, wk: Tensor, bk: Tensor, wv: Tensor, bv: Tensor,
-                          n: int) -> GramState:
+                          n: int, vsum: bool = False) -> GramState:
     """h x h algebra between the two passes (sgf_attn_gram_prepare_fwd): from G = x^T x, s = x^T 1 and the projection weights
-    -> Bt [d,h], tail [16,h] (row 0 = ct), bt [d], sc[SC_DEN] such that out = (x Bt^T + bt)/(x ct + sc[SC_DEN])."""
+    -> Bt [d,h], tail [16,h] (row 0 = ct), bt [d], sc[SC_DEN] such that out = (x Bt^T + bt)/(x ct + sc[SC_DEN]).
+    vsum=True: DIFFormer's numerator (column sum of v instead of N v; sgf_attn_gram_prepare_fwd_vsum)."""
     _use(G)
     st = GramState()
+    st.vsum = bool(vsum)
     st.wq, st.wk, st.wv = _w2(wq, "Wq"), _w2(wk, "Wk"), _w2(wv, "Wv")
     st.bq, st.bk, st.bv = (t.contiguous() for t in (bq, bk, bv))
     st.m, st.h = wq.shape
@@ -913,8 +953,17 @@ def attn_gram_prepare_fwd(G: Tensor, s: Tensor, wq: Tensor, bq: Tensor, wk: Tens
     nws = C.c_int64(0)
     check(lib().sgf_attn_gram_ws_floats(h, m, d, C.byref(nws)), "sgf_attn_gram_ws_floats")
     st.ws = torch.empty(max(nws.value, 1), dtype=torch.float32, device=dev)
-    check(lib().sgf_attn_gram_prepare_fwd(C.byref(_gram_args(st)), _stream()), "sgf_attn_gram_prepare_fwd")
+    if st.vsum:
+        check(lib().sgf_attn_gram_prepare_fwd_vsum(C.byref(_gram_args(st)), _stream()), "sgf_attn_gram_prepare_fwd_vsum")
+    else:
+        check(lib().sgf_attn_gram_prepare_fwd(C.byref(_gram_args(st)), _stream()), "sgf_attn_gram_prepare_fwd")
     return st
+
+
+def attn_gram_prepare_fwd_vsum(G: Tensor, s: Tensor, wq: Tensor, bq: Tensor, wk: Tensor, bk: Tensor, wv: Tensor, bv: Tensor,
+                               n: int) -> GramState:
+    """attn_gram_prepare_fwd in value-sum mode (DIFFormer); attn_gram_prepare_bwd then runs the matching backward."""
+    return attn_gram_prepare_fwd(G, s, wq, bq, wk, bk, wv, bv, n, vsum=True)
 
 
 def attn_gram_prepare_bwd(st: GramState, P: Tensor, pg: Tensor, cs: Tensor, sg: Tensor):
@@ -936,7 +985,10 @@ def attn_gram_prepare_bwd(st: GramState, P: Tensor, pg: Tensor, cs: Tensor, sg: 
     a.P, a.pg, a.cs, a.sg = _p(P), _p(_f32vec(pg, h, "pg")), _p(_f32vec(cs, d, "cs")), _p(_f32vec(sg, 1, "sg"))
     for k_ in sizes:
         setattr(a, k_, _p(out[k_]))
-    check(lib().sgf_attn_gram_prepare_bwd(C.byref(a), _stream()), "sgf_attn_gram_prepare_bwd")
+    if st.vsum:
+        check(lib().sgf_attn_gram_prepare_bwd_vsum(C.byref(a), _stream()), "sgf_attn_gram_prepare_bwd_vsum")
+    else:
+        check(lib().sgf_attn_gram_prepare_bwd(C.byref(a), _stream()), "sgf_attn_gram_prepare_bwd")
     return out["dwq"], out["dbq"], out["dwk"], out["dbk"], out["dwv"], out["dbv"], out["bcat"], out["a4"]
 
 
