@@ -73,13 +73,17 @@ def _layer(cfg, sd, i, x, x0, edge_index, with_graph=True):
     return _ln(sd, f"bns.{i + 1}", c, cfg), (q, k)
 
 
+def _dropout(x, p, training):
+    return F.dropout(x, p=p, training=training)
+
+
 def difformer_forward(cfg, sd, x, edge_index, training=False):
     p = cfg["dropout"]
-    h = F.dropout(F.relu(_ln(sd, "bns.0", _lin(sd, "fcs.0", x), cfg)), p, training)
+    h = _dropout(F.relu(_ln(sd, "bns.0", _lin(sd, "fcs.0", x), cfg)), p, training)
     x0 = h
     for i in range(cfg["num_layers"]):
         h, _ = _layer(cfg, sd, i, h, x0, edge_index)
-        h = F.dropout(h, p, training)
+        h = _dropout(h, p, training)
     return _lin(sd, "fcs.1", h)
 
 

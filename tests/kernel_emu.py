@@ -10,6 +10,8 @@ from typing import Optional
 
 import torch
 
+from dropout_mask import apply_kernel_dropout
+
 EPI_AFFINE, EPI_ATTN_APPLY, EPI_ATTN_GRAM = 0, 1, 2
 
 
@@ -212,17 +214,17 @@ def _ln_core(x, r, a, b, gamma, beta, use_ln, use_relu):
 
 
 def ln_fwd(x, r, a, b, gamma, beta, use_ln, use_relu, p, seed, want_stats=True):
-    assert p == 0.0, "emulation supports dropout p=0 only"
     u, xh, t, mean, rstd = _ln_core(x, r, a, b, gamma, beta, use_ln, use_relu)
     if use_relu:
         t = t.clamp_min(0)
+    t = apply_kernel_dropout(t, seed, p)
     stats = torch.stack([mean, rstd], 1) if use_ln else None
     return _st(new_like(x), t), stats
 
 
 def ln_bwd(dy, x, r, a, b, gamma, beta, stats, use_ln, use_relu, p, seed, gscale, want_dr, dgamma, dbeta):
     u, xh, t, mean, rstd = _ln_core(x, r, a, b, gamma, beta, use_ln, use_relu)
-    g = gscale * dy.float()
+    g = apply_kernel_dropout(gscale * dy.float(), seed, p)
     if use_relu:
         g = g * (t > 0)
     if use_ln:
@@ -241,7 +243,7 @@ def ln_bwd_attn(dy, o, r, xa, a, b, gamma, beta, stats, use_ln, use_relu, p, see
     """sgf_ln_bwd_attn: LayerNorm backward of u = a*o + b*r fused with the attention-backward row prologue:
     g = a*du;  gnum' = g/den~;  gden' = -(g.o)/den~;  dr = b*du;  column sums cs = sum gnum', pg = sum xa*gden', sg = sum gden'."""
     u, xh, t, mean, rstd = _ln_core(o, r, a, b, gamma, beta, use_ln, use_relu)
-    g = gscale * _f(dy)
+    g = apply_kernel_dropout(gscale * _f(dy), seed, p)
     if use_relu:
         g = g * (t > 0)
     if use_ln:
@@ -281,10 +283,10 @@ def _bn_pre(z, mean, rstd, gamma, beta, zbias, use_bn):
 
 
 def bn_fwd(z, res, mix, mean, rstd, gamma, beta, zbias, use_bn, use_relu, p, seed, gw, row_scale, want_y, want_scaled, ys_out=None):
-    assert p == 0.0
     _, t = _bn_pre(z, mean, rstd, gamma, beta, zbias, use_bn)
     if use_relu:
         t = t.clamp_min(0)
+    t = apply_kernel_dropout(t, seed, p)            # before the residual
     if res is not None:
         t = t + res.float()
     ys = _st(new_like(z), t * row_scale[:, None]) if want_scaled else None
@@ -304,7 +306,7 @@ def _bn_g(dy, dy2, row_scale2, gscale):
 
 
 def bn_bwd_sums(dy, dy2, row_scale2, z, mean, rstd, gamma, beta, zbias, use_bn, use_relu, p, seed, gscale):
-    g = _bn_g(dy, dy2, row_scale2, gscale)
+    g = apply_kernel_dropout(_bn_g(dy, dy2, row_scale2, gscale), seed, p)
     xh, pre = _bn_pre(z, mean, rstd, gamma, beta, zbias, use_bn)
     if use_relu:
         g = g * (pre > 0)
@@ -317,7 +319,8 @@ def bn_bwd(dy, dy2, row_scale2, z, mean, rstd, gamma, beta, zbias, use_bn, use_r
     if dres is not None:
         _st(dres, graw + (dres.float() if dres_accumulate else 0.0))
     xh, pre = _bn_pre(z, mean, rstd, gamma, beta, zbias, use_bn)
-    g = graw * (pre > 0) if use_relu else graw
+    g = apply_kernel_dropout(graw, seed, p)           # dres takes the gradient before the dropout mask
+    g = g * (pre > 0) if use_relu else g
     sums = None
     if use_bn and training:
         sums = torch.cat([g.sum(0), (g * xh).sum(0)])

@@ -8,6 +8,7 @@ this module."""
 import torch
 
 import kernel_emu as _base
+from dropout_mask import apply_kernel_dropout
 from kernel_emu import *  # noqa: F401,F403
 from kernel_emu import _f, _st, new_like
 
@@ -53,16 +54,14 @@ def attn_gram_prepare_bwd(st, P, pg, cs, sg):
 
 def ln_fwd_graph(x, r, gy, a, b, c, gamma, beta, use_ln, use_relu, p, seed, want_stats=True):
     """sgf_ln_fwd_graph: ln_fwd of u = a*x + b*r + c*gy."""
-    assert p == 0.0, "emulation supports dropout p=0 only"
     u = a * _f(x) + (b * _f(r) if r is not None else 0.0) + c * _f(gy)
     return _base.ln_fwd(u, None, 1.0, 0.0, gamma, beta, use_ln, use_relu, p, seed, want_stats)
 
 
 def ln_bwd_attn_graph(dy, o, r, xa, gy, a, b, c, gamma, beta, stats, use_ln, p, seed, gscale, want_dr, dgamma, dbeta, den, dinv):
     """sgf_ln_bwd_attn_graph: sgf_ln_bwd_attn for u = a*o + b*r + c*gy, plus ys = dinv (.) (c*du)."""
-    assert p == 0.0, "emulation supports dropout p=0 only"
     u = a * _f(o) + (b * _f(r) if r is not None else 0.0) + c * _f(gy)
-    g = gscale * _f(dy)
+    g = apply_kernel_dropout(gscale * _f(dy), seed, p)
     if use_ln:
         mean = u.mean(1)
         rstd = (u.var(1, unbiased=False) + 1e-5).rsqrt()
