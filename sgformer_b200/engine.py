@@ -13,7 +13,6 @@ medium/models.py:49-63 (GCN over PyG GCNConv), large/ours.py:265-276 (SGFormer.f
 from __future__ import annotations
 
 import itertools
-import os
 from collections import OrderedDict
 from dataclasses import dataclass
 from typing import Dict, List, Optional
@@ -61,6 +60,15 @@ _seed_counter = itertools.count(1)
 def next_seed() -> int:
     """Per-forward dropout seed: deterministic under torch.manual_seed, no device sync."""
     return ((torch.initial_seed() * 0x9E3779B1) ^ (next(_seed_counter) * 0x85EBCA6B)) & 0x7FFFFFFFFFFFFFFF
+
+
+# Offsets of the dropout calls from the forward's seed (+ the layer index where marked).  A backward recomputes its
+# forward's mask from the same seed, so both read these; changing a value changes every mask a training step draws.
+_SEED_STEM = 101            # TransConv / DIFFormer input stem
+_SEED_LAYER = 211           # + i: TransConv / DIFFormer layer i
+_SEED_GCONV_STEM = 307      # GraphConv input layer
+_SEED_GCONV_LAYER = 401     # + i: GraphConv layer i
+_SEED_GCN_LAYER = 503       # + i: GCN layer i
 
 
 def check_width(h: int, prec: Precision, what: str):
@@ -193,8 +201,6 @@ def attention_backward(tape: Tape, g: Tensor, gscale: float, prec: Precision, dq
 # The backward contracts P = x^T gnum', x^T gden' the same way: dWq, dWk, dWv come out of h x h algebra, dx is one
 # two-segment GEMM [gnum' | x] . [Bt | A3] (sgf_attn_gram_prepare_bwd).  Forward traffic 3 N h b instead of 12 N h b,
 # 4 N h^2 flops instead of 10 N h^2; identical mathematics (fp64 check: tests/test_gram_attention_math.py).
-GRAM_ATTENTION = os.environ.get("SGF_GRAM_ATTENTION", "1") == "1"
-
 _eye_cache: dict = {}
 
 
@@ -233,18 +239,31 @@ def attention_gram_forward(P: Dict[str, Tensor], lp: str, x: Tensor, use_weight:
 
 def attention_gram_backward(P: Dict[str, Tensor], lp: str, tape: Tape, x: Tensor, gnum: Tensor, gden: Tensor, cs: Tensor,
                             pg: Tensor, sg: Tensor, use_weight: bool, prec: Precision, dprev: Tensor, accumulate: bool,
-                            grads: Dict[str, Tensor], comm: Comm = SINGLE):
+                            grads: Dict[str, Tensor], comm: Comm = SINGLE, *, dv: Optional[Tensor] = None):
     """gnum' = g/den~ [N,h], gden' = -(g.o)/den~ [N] and their column sums (sgf_ln_bwd_attn) -> parameter gradients and
-    dprev (+)= d/dx of the attention (through q, k and v)."""
+    dprev (+)= d/dx of the attention (through q, k and v).  dv: a further gradient of v = x Wv^T + bv (DIFFormer's graph
+    term, from the transposed SpMM), added to dWv, dbv and dprev; single device only, as it is not all-reduced."""
     st = tape["st"]
     h = x.shape[1]
     d = gnum.shape[1]
     dev = x.device
+    xop = tape["xop"]
     gnum_op = K.as_operand(gnum, prec.planes)
     pmat = torch.empty((h, d), dtype=torch.float32, device=dev)
-    K.gemm_tn(tape["xop"], gnum_op, pmat)
+    K.gemm_tn(xop, gnum_op, pmat)
     comm.allreduce_(pmat, pg, cs, sg)                         # C2
     dwq, dbq, dwk, dbk, dwv, dbv, bcat, a4 = K.attn_gram_prepare_bwd(st, pmat, pg, cs, sg)
+    A, B = [gnum_op, xop], [K.pack_operand(bcat, False, prec.planes)]
+    pairs = [(0, 0, 0, 0, d), (1, 0, 0, d, h)]
+    if dv is not None:
+        dv_op = K.as_operand(dv, prec.planes)
+        if use_weight:
+            K.gemm_tn(dv_op, xop, dwv, beta=1.0)
+            K.colstats(dv, want_sumsq=False, sum_out=dbv)
+        A.append(dv_op)
+        B.append(K.pack_operand(P[lp + "Wv.weight"] if use_weight else _identity_v(h, dev)[0], True, prec.planes))
+        if prec.planes == 1:            # dv Wv as a third segment of the dx GEMM
+            pairs.append((2, 0, 1, 0, d))
     grads[lp + "Wq.weight"], grads[lp + "Wq.bias"] = dwq, dbq
     grads[lp + "Wk.weight"], grads[lp + "Wk.bias"] = dwk, dbk
     names = [lp + "Wq.weight", lp + "Wq.bias", lp + "Wk.weight", lp + "Wk.bias"]
@@ -252,9 +271,9 @@ def attention_gram_backward(P: Dict[str, Tensor], lp: str, tape: Tape, x: Tensor
         grads[lp + "Wv.weight"], grads[lp + "Wv.bias"] = dwv, dbv
         names += [lp + "Wv.weight", lp + "Wv.bias"]
     _mark_global(grads, comm, *names)          # built from all-reduced contractions: already global sums
-    bop = K.pack_operand(bcat, False, prec.planes)
-    K.gemm_nt([gnum_op, tape["xop"]], [bop], [(0, 0, 0, 0, d), (1, 0, 0, d, h)], h, dprev, bias=a4, r1_row=gden,
-              r1_col=st.tail[0], accumulate=accumulate)
+    K.gemm_nt(A, B, pairs, h, dprev, bias=a4, r1_row=gden, r1_col=st.tail[0], accumulate=accumulate)
+    if dv is not None and prec.planes != 1:     # bf16x3: 3 x 6 partial products exceed the GEMM's 16 segments
+        K.gemm_nt([A[2]], [B[1]], [(0, 0, 0, 0, d)], h, dprev, accumulate=True)
 
 
 # =================================================================================================
@@ -275,51 +294,85 @@ def _qkv_weight(P, pfx: str, use_weight: bool) -> (Tensor, Tensor):
     return torch.cat(ws, 0), torch.cat(bs, 0)
 
 
+def _project_qkv(P, lp: str, xop: K.Operand, use_weight: bool, prec: Precision, stats: bool):
+    """q | k (| v when use_weight) of a layer with materialised projections, in one GEMM of the layer input -> qkv [N, nout]
+    and, with `stats`, the column sums and sums of squares its epilogue accumulates (else None, None)."""
+    wcat, bcat = _qkv_weight(P, lp, use_weight)
+    nout = wcat.shape[0]
+    dev = wcat.device
+    qkv = torch.empty((xop.rows, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
+    csum, csq = (torch.zeros(nout, dtype=torch.float32, device=dev), torch.zeros(nout, dtype=torch.float32, device=dev)) \
+        if stats else (None, None)
+    K.gemm_nt([xop], [K.pack_operand(wcat, False, prec.planes)], [(0, 0, 0, 0, xop.k)], nout, qkv, bias=bcat, col_sum=csum,
+              col_sumsq=csq)
+    return qkv, csum, csq
+
+
+def _stem_forward(P, pfx: str, xin: K.Operand, h: int, use_ln: bool, prec: Precision, p: float = 0.0, seed: int = 0,
+                  want_stats: bool = False):
+    """Input Linear fcs.0, then LayerNorm?/ReLU/dropout (TransConv, DIFFormer) -> (t0, x, LayerNorm statistics)."""
+    t0 = K.alloc_act(xin.rows, h, prec.act_dtype, xin.data.device)
+    K.gemm_nt([xin], [_w(P, pfx + "fcs.0.weight", prec)], [(0, 0, 0, 0, xin.k)], h, t0, bias=P[pfx + "fcs.0.bias"])
+    x, st = K.ln_fwd(t0, None, 1.0, 0.0, P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), use_ln, True, p, seed, want_stats)
+    return t0, x, st
+
+
+def _stem_backward(P, pfx: str, tape: Tape, dout: Tensor, gscale: float, use_ln: bool, prec: Precision,
+                   grads: Dict[str, Tensor], want_dx: bool) -> Optional[Tensor]:
+    """Backward of _stem_forward (its t0, xin and statistics read from `tape`): fills the fcs.0 and bns.0 gradients and, with
+    want_dx, returns the gradient of the raw features."""
+    t0, xin = tape["t0"], tape["xin"]
+    n, h = t0.shape
+    d_in = xin.k
+    dev = dout.device
+    dg, db = (torch.zeros(h, dtype=torch.float32, device=dev), torch.zeros(h, dtype=torch.float32, device=dev)) if use_ln \
+        else (None, None)
+    dt0, _ = K.ln_bwd(dout, t0, None, 1.0, 0.0, P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), tape["st0"], use_ln, True,
+                      tape["p"], tape["seed"] + _SEED_STEM, gscale, False, dg, db)
+    if use_ln:
+        grads[pfx + "bns.0.weight"], grads[pfx + "bns.0.bias"] = dg, db
+    dt0_op = K.as_operand(dt0, prec.planes)
+    dw0 = torch.empty((h, d_in), dtype=torch.float32, device=dev)
+    K.gemm_tn(dt0_op, xin, dw0)
+    grads[pfx + "fcs.0.weight"] = dw0
+    grads[pfx + "fcs.0.bias"], _ = K.colstats(dt0, want_sumsq=False)
+    if not want_dx:
+        return None
+    dx = torch.empty((n, d_in), dtype=torch.float32, device=dev)
+    K.gemm_nt([dt0_op], [_w(P, pfx + "fcs.0.weight", prec, transpose=True)], [(0, 0, 0, 0, h)], d_in, dx)
+    return dx
+
+
 def trans_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precision, training: bool, seed: int,
                   tape: Optional[Tape], pfx: str = "trans_conv.", comm: Comm = SINGLE) -> Tensor:
-    h, H, d_in = cfg["hidden"], cfg["num_heads"], cfg["in_channels"]
+    h, H = cfg["hidden"], cfg["num_heads"]
     check_width(h, prec, "hidden_channels")
-    n = xin.rows
-    dev = xin.data.device
     p = float(cfg["trans_dropout"]) if training else 0.0
     use_ln = bool(cfg["trans_use_bn"])
-    act = K.alloc_act(n, h, prec.act_dtype, dev)
-    t0 = K.gemm_nt([xin], [_w(P, pfx + "fcs.0.weight", prec)], [(0, 0, 0, 0, d_in)], h, act, bias=P[pfx + "fcs.0.bias"])
-    x, st = K.ln_fwd(t0, None, 1.0, 0.0, P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), use_ln, True, p,
-                     seed + 101, tape is not None)
+    t0, x, st = _stem_forward(P, pfx, xin, h, use_ln, prec, p, seed + _SEED_STEM, tape is not None)
     if tape is not None:
-        tape.update(xin=xin, t0=t0, st0=st, layers=[], p=p, seed=seed, n=n)
+        tape.update(xin=xin, t0=t0, st0=st, layers=[], p=p, seed=seed, n=xin.rows)
     ca, cb, use_res = _res_coef(cfg)
     use_weight = bool(cfg["trans_use_weight"])
     if not use_weight and H != 1:
         raise ValueError("use_weight=False requires num_heads == 1 (medium/ours.py:84)")
     for i in range(cfg["trans_num_layers"]):
         lp = f"{pfx}convs.{i}."
-        if GRAM_ATTENTION and H == 1:
-            at = Tape() if tape is not None else None
-            a = attention_gram_forward(P, lp, x, use_weight, prec, at, comm)
-            y, st = K.ln_fwd(a, x if use_res else None, ca, cb, P.get(f"{pfx}bns.{i + 1}.weight"), P.get(f"{pfx}bns.{i + 1}.bias"),
-                             use_ln, bool(cfg["trans_use_act"]), p, seed + 211 + i, tape is not None)
-            if tape is not None:
-                tape["layers"].append(dict(x_in=x, attn=at, a=a, st=st, gram=True))
-            x = y
-            continue
-        wcat, bcat = _qkv_weight(P, lp, use_weight)
-        nout = wcat.shape[0]
-        qkv = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
-        csum = torch.zeros(nout, dtype=torch.float32, device=dev)
-        csq = torch.zeros(nout, dtype=torch.float32, device=dev)
-        K.gemm_nt([K.as_operand(x, prec.planes, memo=True)], [K.pack_operand(wcat, False, prec.planes)], [(0, 0, 0, 0, h)], nout, qkv,
-                  bias=bcat, col_sum=csum, col_sumsq=csq)        # K^T 1, ||Q||^2, ||K||^2 fall out of the projection's epilogue
-        q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
-        v = qkv[:, 2 * H * h:] if use_weight else x
         at = Tape() if tape is not None else None
-        o = attention_forward(q, k, v, H, prec, at, comm, stats=(csq[:H * h], csum[H * h:2 * H * h], csq[H * h:2 * H * h]))
-        a = K.head_mean(o, H, h) if H > 1 else o
+        if H == 1:
+            a = attention_gram_forward(P, lp, x, use_weight, prec, at, comm)
+            saved = dict(gram=True)
+        else:
+            # K^T 1, ||Q||^2, ||K||^2 fall out of the projection's epilogue
+            qkv, csum, csq = _project_qkv(P, lp, K.as_operand(x, prec.planes, memo=True), use_weight, prec, stats=True)
+            q, k, v = qkv[:, :H * h], qkv[:, H * h:2 * H * h], qkv[:, 2 * H * h:]
+            o = attention_forward(q, k, v, H, prec, at, comm, stats=(csq[:H * h], csum[H * h:2 * H * h], csq[H * h:2 * H * h]))
+            a = K.head_mean(o, H, h)
+            saved = dict(nout=qkv.shape[1])
         y, st = K.ln_fwd(a, x if use_res else None, ca, cb, P.get(f"{pfx}bns.{i + 1}.weight"), P.get(f"{pfx}bns.{i + 1}.bias"),
-                         use_ln, bool(cfg["trans_use_act"]), p, seed + 211 + i, tape is not None)
+                         use_ln, bool(cfg["trans_use_act"]), p, seed + _SEED_LAYER + i, tape is not None)
         if tape is not None:
-            tape["layers"].append(dict(x_in=x, qkv=qkv, attn=at, a=a, st=st, nout=nout))
+            tape["layers"].append(dict(saved, x_in=x, attn=at, a=a, st=st))
         x = y
     return x
 
@@ -331,23 +384,18 @@ def trans_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Prec
     tensor-core GEMM of the concatenated heads (sum over heads of per-head dot products) with 1/(H ||q|| ||k||) read from the
     device and the row normaliser as its row scale; the layer stack itself runs the un-fused attention (q, k materialised).
     Inference only (no dropout, no tape), O(N^2) memory like the reference: meant for small graphs."""
-    h, H, d_in = cfg["hidden"], cfg["num_heads"], cfg["in_channels"]
+    h, H = cfg["hidden"], cfg["num_heads"]
     check_width(h, prec, "hidden_channels")
     n = xin.rows
     dev = xin.data.device
     use_ln = bool(cfg["trans_use_bn"])
     ca, cb, use_res = _res_coef(cfg)
     use_weight = bool(cfg["trans_use_weight"])
-    t0 = K.gemm_nt([xin], [_w(P, pfx + "fcs.0.weight", prec)], [(0, 0, 0, 0, d_in)], h, K.alloc_act(n, h, prec.act_dtype, dev),
-                   bias=P[pfx + "fcs.0.bias"])
-    x, _ = K.ln_fwd(t0, None, 1.0, 0.0, P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), use_ln, True, 0.0, 0, False)
+    _, x, _ = _stem_forward(P, pfx, xin, h, use_ln, prec)
     out = []
     for i in range(cfg["trans_num_layers"]):
         lp = f"{pfx}convs.{i}."
-        wcat, bcat = _qkv_weight(P, lp, use_weight)
-        nout = wcat.shape[0]
-        qkv = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
-        K.gemm_nt([K.as_operand(x, prec.planes)], [K.pack_operand(wcat, False, prec.planes)], [(0, 0, 0, 0, h)], nout, qkv, bias=bcat)
+        qkv, _, _ = _project_qkv(P, lp, K.as_operand(x, prec.planes), use_weight, prec, stats=False)
         q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
         v = qkv[:, 2 * H * h:] if use_weight else x
         at = Tape()
@@ -365,83 +413,49 @@ def trans_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Prec
 
 def trans_backward(P, cfg: dict, tape: Tape, dout: Tensor, gscale: float, prec: Precision, grads: Dict[str, Tensor],
                    pfx: str = "trans_conv.", want_dx: bool = False, comm: Comm = SINGLE) -> Optional[Tensor]:
-    h, H, d_in = cfg["hidden"], cfg["num_heads"], cfg["in_channels"]
+    h, H = cfg["hidden"], cfg["num_heads"]
     n, p, seed = tape["n"], tape["p"], tape["seed"]
     dev = dout.device
     use_ln = bool(cfg["trans_use_bn"])
     ca, cb, use_res = _res_coef(cfg)
     use_weight = bool(cfg["trans_use_weight"])
 
-    def zeros(k):
-        return torch.zeros(k, dtype=torch.float32, device=dev)
-
     dcur, gs = dout, gscale
     for i in reversed(range(cfg["trans_num_layers"])):
         L = tape["layers"][i]
-        lp = f"{pfx}convs.{i}."
-        dg, db = (zeros(h), zeros(h)) if use_ln else (None, None)
+        lp, bn = f"{pfx}convs.{i}.", f"{pfx}bns.{i + 1}."
+        x_in, at = L["x_in"], L["attn"]
+        dg, db = (torch.zeros(h, dtype=torch.float32, device=dev), torch.zeros(h, dtype=torch.float32, device=dev)) if use_ln \
+            else (None, None)
         if L.get("gram"):
-            x_in, at = L["x_in"], L["attn"]
-            gnum, gden, dr, cs, pg, sg = K.ln_bwd_attn(dcur, L["a"], x_in if use_res else None, x_in, ca, cb,
-                                                       P.get(f"{pfx}bns.{i + 1}.weight"), P.get(f"{pfx}bns.{i + 1}.bias"), L["st"],
-                                                       use_ln, bool(cfg["trans_use_act"]), p, seed + 211 + i, gs, use_res, dg, db,
-                                                       at["den"])
-            if use_ln:
-                grads[f"{pfx}bns.{i + 1}.weight"], grads[f"{pfx}bns.{i + 1}.bias"] = dg, db
+            gnum, gden, dr, cs, pg, sg = K.ln_bwd_attn(dcur, L["a"], x_in if use_res else None, x_in, ca, cb, P.get(bn + "weight"),
+                                                       P.get(bn + "bias"), L["st"], use_ln, bool(cfg["trans_use_act"]), p,
+                                                       seed + _SEED_LAYER + i, gs, use_res, dg, db, at["den"])
             dprev = dr if dr is not None else K.new_like(x_in)
             attention_gram_backward(P, lp, at, x_in, gnum, gden, cs, pg, sg, use_weight, prec, dprev, dr is not None, grads, comm)
-            dcur, gs = dprev, 1.0
-            continue
-        x_in, qkv, at, nout = L["x_in"], L["qkv"], L["attn"], L["nout"]
-        da, dr = K.ln_bwd(dcur, L["a"], x_in if use_res else None, ca, cb, P.get(f"{pfx}bns.{i + 1}.weight"),
-                          P.get(f"{pfx}bns.{i + 1}.bias"), L["st"], use_ln, bool(cfg["trans_use_act"]), p, seed + 211 + i, gs,
-                          use_res, dg, db)
+        else:       # materialised q, k, v: several heads, so use_weight is set
+            nout = L["nout"]
+            da, dr = K.ln_bwd(dcur, L["a"], x_in if use_res else None, ca, cb, P.get(bn + "weight"), P.get(bn + "bias"), L["st"],
+                              use_ln, bool(cfg["trans_use_act"]), p, seed + _SEED_LAYER + i, gs, use_res, dg, db)
+            # head mean: every head receives da / H; da has pitch h, per-head slices of g are the same columns for all heads
+            dqkv = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
+            dprev = dr if dr is not None else K.new_like(x_in)
+            attention_backward(at, _tile_heads(da, H), 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h],
+                               dqkv[:, 2 * H * h:], comm=comm)
+            wcat, _ = _qkv_weight(P, lp, use_weight)
+            dqkv_op = K.as_operand(dqkv, prec.planes)
+            K.gemm_nt([dqkv_op], [K.pack_operand(wcat, True, prec.planes)], [(0, 0, 0, 0, nout)], h, dprev,
+                      accumulate=dr is not None)
+            dw = torch.empty((nout, h), dtype=torch.float32, device=dev)
+            K.gemm_tn(dqkv_op, K.as_operand(x_in, prec.planes, memo=True), dw)
+            dbias, _ = K.colstats(dqkv, want_sumsq=False)
+            for j, nm in enumerate(("Wq", "Wk", "Wv")):
+                grads[lp + nm + ".weight"] = dw[j * H * h:(j + 1) * H * h]
+                grads[lp + nm + ".bias"] = dbias[j * H * h:(j + 1) * H * h]
         if use_ln:
-            grads[f"{pfx}bns.{i + 1}.weight"], grads[f"{pfx}bns.{i + 1}.bias"] = dg, db
-        # head mean: every head receives da / H; da has pitch h, per-head slices of g are the same columns for all heads
-        dqkv = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
-        dprev = dr
-        if dprev is None:
-            dprev = K.new_like(x_in)
-            first_write = True
-        else:
-            first_write = False
-        g_all = da if H == 1 else _tile_heads(da, H)
-        if use_weight:
-            attention_backward(at, g_all, 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h], dqkv[:, 2 * H * h:],
-                               comm=comm)
-        else:
-            # V is the layer input itself: its gradient goes straight into dprev
-            attention_backward(at, g_all, 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h], dprev,
-                               dv_accumulate=not first_write, comm=comm)
-            first_write = False
-        wcat, _ = _qkv_weight(P, lp, use_weight)
-        dqkv_op = K.as_operand(dqkv, prec.planes)
-        K.gemm_nt([dqkv_op], [K.pack_operand(wcat, True, prec.planes)], [(0, 0, 0, 0, nout)], h, dprev,
-                  accumulate=not first_write)
-        dw = torch.empty((nout, h), dtype=torch.float32, device=dev)
-        K.gemm_tn(dqkv_op, K.as_operand(x_in, prec.planes, memo=True), dw)
-        dbias, _ = K.colstats(dqkv, want_sumsq=False)
-        names = ["Wq", "Wk"] + (["Wv"] if use_weight else [])
-        for j, nm in enumerate(names):
-            grads[lp + nm + ".weight"] = dw[j * H * h:(j + 1) * H * h]
-            grads[lp + nm + ".bias"] = dbias[j * H * h:(j + 1) * H * h]
+            grads[bn + "weight"], grads[bn + "bias"] = dg, db
         dcur, gs = dprev, 1.0
-    dg, db = (zeros(h), zeros(h)) if use_ln else (None, None)
-    dt0, _ = K.ln_bwd(dcur, tape["t0"], None, 1.0, 0.0, P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), tape["st0"],
-                      use_ln, True, p, seed + 101, gs, False, dg, db)
-    if use_ln:
-        grads[pfx + "bns.0.weight"], grads[pfx + "bns.0.bias"] = dg, db
-    dt0_op = K.as_operand(dt0, prec.planes)
-    dw0 = torch.empty((h, d_in), dtype=torch.float32, device=dev)
-    K.gemm_tn(dt0_op, tape["xin"], dw0)
-    grads[pfx + "fcs.0.weight"] = dw0
-    grads[pfx + "fcs.0.bias"], _ = K.colstats(dt0, want_sumsq=False)
-    if want_dx:
-        dx = torch.empty((n, d_in), dtype=torch.float32, device=dev)
-        K.gemm_nt([dt0_op], [_w(P, pfx + "fcs.0.weight", prec, transpose=True)], [(0, 0, 0, 0, h)], d_in, dx)
-        return dx
-    return None
+    return _stem_backward(P, pfx, tape, dcur, gs, use_ln, prec, grads, want_dx)
 
 
 def _tile_heads(da: Tensor, heads: int) -> Tensor:
@@ -503,7 +517,7 @@ def gconv_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, t
     last_is_input = nl == 0
     # the pre-scaled SpMM operand is written where the halo exchange wants it (slot 0 of the step's symmetric buffer when pushed)
     x0, cur_s = K.bn_fwd(z0, None, mix if last_is_input else None, mean0, rstd0, P.get(pfx + "bns.0.weight"),
-                         P.get(pfx + "bns.0.bias"), None, use_bn, True, p, seed + 307, gw, dinv, True, not last_is_input,
+                         P.get(pfx + "bns.0.bias"), None, use_bn, True, p, seed + _SEED_GCONV_STEM, gw, dinv, True, not last_is_input,
                          ys_out=None if last_is_input else comm.operand_out(n, h, prec.act_dtype, dev))
     if tape is not None:
         tape.update(xin=xin, z0=z0, mean0=mean0, rstd0=rstd0, x0=x0, layers=[], p=p, seed=seed, n=n, training=training,
@@ -527,7 +541,7 @@ def gconv_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, t
         name = f"{pfx}bns.{i + 1}."
         mean, rstd = _bn_stats(z, P, name, use_bn, training, comm=comm, pre=st)
         yo, ys = K.bn_fwd(z, x0 if use_res else None, mix if last else None, mean, rstd, P.get(name + "weight"),
-                          P.get(name + "bias"), None, use_bn, use_act, p, seed + 401 + i, gw, dinv, last, not last,
+                          P.get(name + "bias"), None, use_bn, use_act, p, seed + _SEED_GCONV_LAYER + i, gw, dinv, last, not last,
                           ys_out=None if last else comm.operand_out(n, h, prec.act_dtype, dev))
         if tape is not None:
             tape["layers"].append(dict(y=y, z=z, mean=mean, rstd=rstd))
@@ -548,7 +562,6 @@ def gconv_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: P
     use_bn, use_res, use_act = bool(cfg["gnn_use_bn"]), bool(cfg["gnn_use_residual"]), bool(cfg["gnn_use_act"])
     use_init, use_weight = bool(cfg["gnn_use_init"]), bool(cfg["gnn_use_weight"])
     dinv = graph.dinv
-    rowptr_t, col_t = graph.transpose()
     x0 = tape["x0"]
     red = comm.allreduce_ if comm.active else None
     nstat = comm.n_global if comm.active else 0
@@ -565,14 +578,11 @@ def gconv_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: P
             res_acc = True
         dz, sums, colsum = K.bn_bwd(dy_plain, dy_scaled, dinv if dy_scaled is not None else None, L["z"], L["mean"],
                                     L["rstd"], P.get(name + "weight"), P.get(name + "bias"), None, use_bn, use_act, training,
-                                    p, seed + 401 + i, gs, dres=dx0 if use_res else None, dres_accumulate=res_acc,
+                                    p, seed + _SEED_GCONV_LAYER + i, gs, dres=dx0 if use_res else None, dres_accumulate=res_acc,
                                     want_dz_colsum=use_init or use_weight, reduce_fn=red, stat_rows=nstat)
         gs = 1.0
-        if use_bn and training:
-            grads[name + "bias"], grads[name + "weight"] = sums[:h], sums[h:]
-            _mark_global(grads, comm, name + "bias", name + "weight")     # the BN sums were all-reduced between the phases
-        elif use_bn:
-            grads[name + "bias"], grads[name + "weight"] = _eval_bn_param_grads(dy_plain, dy_scaled, dinv, L, P, name, use_act)
+        if use_bn:
+            _bn_param_grads(grads, comm, P, name, sums, dy_plain, dy_scaled, dinv, L["z"], L["mean"], L["rstd"], use_act)
         if use_init or use_weight:
             wname = f"{pfx}convs.{i}.W.weight"
             dz_op = K.as_operand(dz, prec.planes)
@@ -606,13 +616,9 @@ def gconv_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: P
         g_plain, g_scaled = dx0, dy_scaled
     dz0, sums, colsum = K.bn_bwd(g_plain, g_scaled, dinv if g_scaled is not None else None, tape["z0"], tape["mean0"],
                                  tape["rstd0"], P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), None, use_bn, True,
-                                 training, p, seed + 307, gs, want_dz_colsum=True, reduce_fn=red, stat_rows=nstat)
-    if use_bn and training:
-        grads[pfx + "bns.0.bias"], grads[pfx + "bns.0.weight"] = sums[:h], sums[h:]
-        _mark_global(grads, comm, pfx + "bns.0.bias", pfx + "bns.0.weight")
-    elif use_bn:
-        grads[pfx + "bns.0.bias"], grads[pfx + "bns.0.weight"] = _eval_bn_param_grads(
-            g_plain, g_scaled, dinv, dict(z=tape["z0"], mean=tape["mean0"], rstd=tape["rstd0"]), P, pfx + "bns.0.", True)
+                                 training, p, seed + _SEED_GCONV_STEM, gs, want_dz_colsum=True, reduce_fn=red, stat_rows=nstat)
+    if use_bn:
+        _bn_param_grads(grads, comm, P, pfx + "bns.0.", sums, g_plain, g_scaled, dinv, tape["z0"], tape["mean0"], tape["rstd0"], True)
     dz0_op = K.as_operand(dz0, prec.planes)
     dw0 = torch.empty((h, d_in), dtype=torch.float32, device=dev)
     K.gemm_tn(dz0_op, tape["xin"], dw0)
@@ -631,12 +637,18 @@ def _mark_global(grads: dict, comm: Comm, *names: str):
         grads.setdefault("__global__", set()).update(names)
 
 
-def _eval_bn_param_grads(dy, dy2, dinv, L, P, name, use_relu):
-    """BatchNorm affine gradients in eval mode (running statistics; rare: eval-mode backward)."""
-    h = L["z"].shape[1]
-    sums = K.bn_bwd_sums(dy, dy2, dinv if dy2 is not None else None, L["z"], L["mean"], L["rstd"], P[name + "weight"],
-                         P[name + "bias"], None, True, use_relu, 0.0, 0, 1.0)
-    return sums[:h], sums[h:]
+def _bn_param_grads(grads: dict, comm: Comm, P, name: str, sums: Optional[Tensor], dy, dy2, dinv, z: Tensor, mean, rstd,
+                    use_relu: bool):
+    """Stores the affine gradients of the BatchNorm `name`.  Training: `sums` = (sum g, sum g*xhat) from bn_bwd, which
+    all-reduced them between its phases.  Eval (sums is None; rare: eval-mode backward): computed here from the running
+    statistics and the gradient (dy, dy2) that entered bn_bwd."""
+    if sums is None:
+        sums = K.bn_bwd_sums(dy, dy2, dinv if dy2 is not None else None, z, mean, rstd, P[name + "weight"], P[name + "bias"], None,
+                             True, use_relu, 0.0, 0, 1.0)
+    else:
+        _mark_global(grads, comm, name + "bias", name + "weight")
+    h = z.shape[1]
+    grads[name + "bias"], grads[name + "weight"] = sums[:h], sums[h:]
 
 
 def _slice_rows(op: K.Operand, r0: int, r1: int) -> K.Operand:
@@ -673,9 +685,9 @@ def gcn_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, tra
             layers.append(dict(s=s, cur_op=cur_op, cur_k=cur_k, hout=hout))
         else:
             name = f"{pfx}bns.{i}."
-            mean, rstd = _bn_stats(s, P, name, use_bn, training, zbias=zb, comm=comm) if use_bn else (None, None)
+            mean, rstd = _bn_stats(s, P, name, use_bn, training, zbias=zb, comm=comm)
             y, _ = K.bn_fwd(s, None, None, mean, rstd, P.get(name + "weight"), P.get(name + "bias"), zb, use_bn, True, p,
-                            seed + 503 + i, 1.0, None, True, False)
+                            seed + _SEED_GCN_LAYER + i, 1.0, None, True, False)
             layers.append(dict(s=s, cur_op=cur_op, cur_k=cur_k, hout=hout, mean=mean, rstd=rstd))
             cur_op, cur_k = K.as_operand(y, prec.planes), hout
     if tape is not None:
@@ -690,7 +702,6 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
     dev = dout.device
     use_bn = bool(cfg["gcn_use_bn"])
     dinv = graph.dinv
-    rowptr_t, col_t = graph.transpose()
     red = comm.allreduce_ if comm.active else None
     nstat = comm.n_global if comm.active else 0
     gs = tape["gw"] if tape["mixed"] else 1.0
@@ -707,11 +718,10 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         else:
             name = f"{pfx}bns.{i}."
             dzs, sums, colsum = K.bn_bwd(dcur, None, None, L["s"], L.get("mean"), L.get("rstd"), P.get(name + "weight"),
-                                         P.get(name + "bias"), zb, use_bn, True, training, p, seed + 503 + i, gs,
+                                         P.get(name + "bias"), zb, use_bn, True, training, p, seed + _SEED_GCN_LAYER + i, gs,
                                          want_dz_colsum=zb is not None, out_row_scale=dinv, reduce_fn=red, stat_rows=nstat)
-            if use_bn and training:
-                grads[name + "bias"], grads[name + "weight"] = sums[:hout], sums[hout:]
-                _mark_global(grads, comm, name + "bias", name + "weight")
+            if use_bn and training:     # not in eval: those sums would also need the conv bias (zbias) the eval path omits
+                _bn_param_grads(grads, comm, P, name, sums, dcur, None, None, L["s"], L["mean"], L["rstd"], True)
         gs = 1.0
         if zb is not None:
             grads[f"{pfx}convs.{i}.bias"] = colsum
@@ -733,22 +743,24 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
 # =================================================================================================
 # head: fc over the mixed / concatenated branches
 # =================================================================================================
-def head_forward(P, cfg: dict, feats: List[Tensor], prec: Precision, tape: Optional[Tape]) -> Tensor:
-    """feats = [m] ('add', branches already mixed) or [x1, x2] ('cat').  large/ours.py:269-275.  Logits are fp32."""
+def head_forward(P, cfg: dict, feats: List[Tensor], prec: Precision, tape: Optional[Tape], pfx: str = "fc.") -> Tensor:
+    """feats = [m] ('add', branches already mixed) or [x1, x2] ('cat').  large/ours.py:269-275.  Logits are fp32.
+    pfx: the Linear's parameter prefix (DIFFormer's output Linear is "fcs.1.")."""
     h, c = cfg["hidden"], cfg["out_channels"]
     n = feats[0].shape[0]
-    w = _w(P, "fc.weight", prec)
+    w = _w(P, pfx + "weight", prec)
     ops = [K.as_operand(f, prec.planes) for f in feats]
     pairs = [(j, 0, 0, j * h, h) for j in range(len(feats))]
     # pitch padded to a 16-byte multiple (c = 47 -> 48 floats): the GEMM epilogue can then use its TMA-store path
     out = K.alloc_act(n, c, torch.float32, feats[0].device)
-    K.gemm_nt(ops, [w], pairs, c, out, bias=P["fc.bias"])
+    K.gemm_nt(ops, [w], pairs, c, out, bias=P[pfx + "bias"])
     if tape is not None:
         tape.update(ops=ops, nfeat=len(feats))
     return out
 
 
-def head_backward(P, cfg: dict, tape: Tape, dlogits: Tensor, prec: Precision, grads: Dict[str, Tensor]) -> List[Tensor]:
+def head_backward(P, cfg: dict, tape: Tape, dlogits: Tensor, prec: Precision, grads: Dict[str, Tensor],
+                  pfx: str = "fc.") -> List[Tensor]:
     h, c = cfg["hidden"], cfg["out_channels"]
     n = dlogits.shape[0]
     dev = dlogits.device
@@ -757,14 +769,14 @@ def head_backward(P, cfg: dict, tape: Tape, dlogits: Tensor, prec: Precision, gr
     dl_op = K.pack_operand(dlogits, False, prec.planes, colsum=db)
     nf = tape["nfeat"]
     dw = torch.empty((c, nf * h), dtype=torch.float32, device=dev)
-    wt = _w(P, "fc.weight", prec, transpose=True)   # [nf*h, c]
+    wt = _w(P, pfx + "weight", prec, transpose=True)   # [nf*h, c]
     outs = []
     for j in range(nf):
         K.gemm_tn(dl_op, tape["ops"][j], dw[:, j * h:(j + 1) * h])
         dj = K.alloc_act(n, h, prec.act_dtype, dev)
         K.gemm_nt([dl_op], [_slice_rows(wt, j * h, (j + 1) * h)], [(0, 0, 0, 0, c)], h, dj)
         outs.append(dj)
-    grads["fc.weight"], grads["fc.bias"] = dw, db
+    grads[pfx + "weight"], grads[pfx + "bias"] = dw, db
     return outs
 
 
@@ -802,18 +814,23 @@ def _difformer_v_scaled(P, lp: str, x: Tensor, use_weight: bool, prec: Precision
                      P[lp + "Wv.weight"].shape[0], K.new_like(x), bias=P[lp + "Wv.bias"], row_scale=dinv)
 
 
+def _difformer_residual(x: Tensor, x0: Tensor, i: int, b: float, s: float):
+    """-> (r, b): the residual operand of layer i and its coefficient in u, with use_source's s*x0 folded in."""
+    if s and i > 0:
+        return K.axpby(x, x0, b, s), 1.0
+    if s or b:
+        return x, b + s          # layer 0: x0 is the layer input
+    return None, b
+
+
 def difformer_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, graph: Optional[Graph], prec: Precision, training: bool,
                       seed: int, tape: Optional[Tape]) -> Tensor:
     """DIFFormer.forward (medium/difformer.py:184-211) -> fp32 logits [N, out_channels]."""
-    h, d_in, c_out, nl = cfg["hidden"], cfg["in_channels"], cfg["out_channels"], cfg["num_layers"]
+    h, nl = cfg["hidden"], cfg["num_layers"]
     check_width(h, prec, "hidden_channels")
-    n = xin.rows
-    dev = xin.data.device
     p = float(cfg["dropout"]) if training else 0.0
     use_ln, use_weight, use_graph = bool(cfg["use_bn"]), bool(cfg["use_weight"]), bool(cfg["use_graph"])
-    t0 = K.gemm_nt([xin], [_w(P, "fcs.0.weight", prec)], [(0, 0, 0, 0, d_in)], h, K.alloc_act(n, h, prec.act_dtype, dev),
-                   bias=P["fcs.0.bias"])
-    x, st0 = K.ln_fwd(t0, None, 1.0, 0.0, P.get("bns.0.weight"), P.get("bns.0.bias"), use_ln, True, p, seed + 101, tape is not None)
+    t0, x, st0 = _stem_forward(P, "", xin, h, use_ln, prec, p, seed + _SEED_STEM, tape is not None)
     x0 = x
     layers = []
     for i in range(nl):
@@ -821,49 +838,29 @@ def difformer_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, graph: Op
         a, b, c, s_ = _difformer_coefs(cfg, i)
         at = Tape() if tape is not None else None
         o = attention_gram_forward(P, lp, x, use_weight, prec, at, vsum=True)
-        if s_ and i > 0:
-            r, b = K.axpby(x, x0, b, s_), 1.0
-        elif s_ or b:
-            r, b = x, b + s_          # layer 0: x0 is the layer input
-        else:
-            r = None
+        r, b = _difformer_residual(x, x0, i, b, s_)
         gamma, beta = P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias")
         if use_graph:
             y = K.spmm(graph.rowptr, graph.col, graph.dinv, _difformer_v_scaled(P, lp, x, use_weight, prec, graph.dinv),
                        heavy=graph.heavy)
-            xn, st = K.ln_fwd_graph(o, r, y, a, b, c, gamma, beta, use_ln, False, p, seed + 211 + i, tape is not None)
+            xn, st = K.ln_fwd_graph(o, r, y, a, b, c, gamma, beta, use_ln, False, p, seed + _SEED_LAYER + i, tape is not None)
         else:
-            xn, st = K.ln_fwd(o, r, a, b, gamma, beta, use_ln, False, p, seed + 211 + i, tape is not None)
+            xn, st = K.ln_fwd(o, r, a, b, gamma, beta, use_ln, False, p, seed + _SEED_LAYER + i, tape is not None)
         layers.append(dict(x_in=x, attn=at, o=o, r=r, y=y if use_graph else None, st=st, coef=(a, b, c)))
         x = xn
-    xop = K.as_operand(x, prec.planes)
-    logits = K.gemm_nt([xop], [_w(P, "fcs.1.weight", prec)], [(0, 0, 0, 0, h)], c_out,
-                       K.alloc_act(n, c_out, torch.float32, dev), bias=P["fcs.1.bias"])
+    logits = head_forward(P, cfg, [x], prec, tape, "fcs.1.")
     if tape is not None:
-        tape.update(xin=xin, t0=t0, st0=st0, layers=layers, p=p, seed=seed, n=n, xop=xop)
+        tape.update(xin=xin, t0=t0, st0=st0, layers=layers, p=p, seed=seed, n=xin.rows)
     return logits
 
 
 def difformer_backward(P: Dict[str, Tensor], cfg: dict, tape: Tape, graph: Optional[Graph], dlogits: Tensor, prec: Precision,
                        grads: Dict[str, Tensor], want_dx: bool = False) -> Optional[Tensor]:
-    h, d_in, c_out, nl = cfg["hidden"], cfg["in_channels"], cfg["out_channels"], cfg["num_layers"]
-    n, p, seed = tape["n"], tape["p"], tape["seed"]
+    h, nl = cfg["hidden"], cfg["num_layers"]
+    p, seed = tape["p"], tape["seed"]
     dev = dlogits.device
     use_ln, use_weight, use_graph = bool(cfg["use_bn"]), bool(cfg["use_weight"]), bool(cfg["use_graph"])
-
-    def zeros(k):
-        return torch.zeros(k, dtype=torch.float32, device=dev)
-
-    # output Linear
-    dlogits = dlogits.contiguous().float()
-    db1 = zeros(c_out)
-    dl_op = K.pack_operand(dlogits, False, prec.planes, colsum=db1)
-    dw1 = torch.empty((c_out, h), dtype=torch.float32, device=dev)
-    K.gemm_tn(dl_op, tape["xop"], dw1)
-    grads["fcs.1.weight"], grads["fcs.1.bias"] = dw1, db1
-    dcur = K.alloc_act(n, h, prec.act_dtype, dev)
-    K.gemm_nt([dl_op], [_w(P, "fcs.1.weight", prec, transpose=True)], [(0, 0, 0, 0, c_out)], h, dcur)
-    gs = 1.0
+    dcur = head_backward(P, cfg, tape, dlogits, prec, grads, "fcs.1.")[0]
     dx0 = None                     # use_source: gradient of x0 collected from layers 1..L-1
     if use_graph:
         rp_t, col_t = graph.transpose()
@@ -874,13 +871,15 @@ def difformer_backward(P: Dict[str, Tensor], cfg: dict, tape: Tape, graph: Optio
         _, _, _, s_ = _difformer_coefs(cfg, i)
         x_in, at, r = L["x_in"], L["attn"], L["r"]
         gamma, beta = P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias")
-        dg, db = (zeros(h), zeros(h)) if use_ln else (None, None)
+        dg, db = (torch.zeros(h, dtype=torch.float32, device=dev), torch.zeros(h, dtype=torch.float32, device=dev)) if use_ln \
+            else (None, None)
         if use_graph:
             gnum, gden, dr, ys, cs, pg, sg = K.ln_bwd_attn_graph(dcur, L["o"], r, x_in, L["y"], a, b, c, gamma, beta, L["st"], use_ln, p,
-                                                                 seed + 211 + i, gs, r is not None, dg, db, at["den"], graph.dinv)
+                                                                 seed + _SEED_LAYER + i, 1.0, r is not None, dg, db, at["den"],
+                                                                 graph.dinv)
         else:
             gnum, gden, dr, cs, pg, sg = K.ln_bwd_attn(dcur, L["o"], r, x_in, a, b, gamma, beta, L["st"], use_ln, False, p,
-                                                       seed + 211 + i, gs, r is not None, dg, db, at["den"])
+                                                       seed + _SEED_LAYER + i, 1.0, r is not None, dg, db, at["den"])
         if use_ln:
             grads[f"bns.{i + 1}.weight"], grads[f"bns.{i + 1}.bias"] = dg, db
         # gradient of the layer input from r
@@ -892,54 +891,13 @@ def difformer_backward(P: Dict[str, Tensor], cfg: dict, tape: Tape, graph: Optio
             dprev, acc = dr, True
         else:
             dprev, acc = K.new_like(x_in), False
-        # attention (value-sum Gram form) + graph term
-        st = at["st"]
-        d = gnum.shape[1]
-        gnum_op = K.as_operand(gnum, prec.planes)
-        pmat = torch.empty((h, d), dtype=torch.float32, device=dev)
-        K.gemm_tn(at["xop"], gnum_op, pmat)
-        dwq, dbq, dwk, dbk, dwv, dbv, bcat, a4 = K.attn_gram_prepare_bwd(st, pmat, pg, cs, sg)
-        grads[lp + "Wq.weight"], grads[lp + "Wq.bias"] = dwq, dbq
-        grads[lp + "Wk.weight"], grads[lp + "Wk.bias"] = dwk, dbk
-        A, B = [gnum_op, at["xop"]], [K.pack_operand(bcat, False, prec.planes)]
-        pairs = [(0, 0, 0, 0, d), (1, 0, 0, d, h)]
-        dv_pair = None
-        if use_graph:
-            dv = K.spmm(rp_t, col_t, graph.dinv, ys, heavy=graph.heavy_t)       # dinv (.) A^T (dinv (.) c du)
-            dv_op = K.as_operand(dv, prec.planes)
-            if use_weight:
-                K.gemm_tn(dv_op, at["xop"], dwv, beta=1.0)
-                K.colstats(dv, want_sumsq=False, sum_out=dbv)
-            wv = P[lp + "Wv.weight"] if use_weight else _identity_v(h, dev)[0]
-            A.append(dv_op)
-            B.append(K.pack_operand(wv, True, prec.planes))
-            dv_pair = (2, 0, 1, 0, d)
-            if prec.planes == 1:            # dv Wv as a third segment of the dx GEMM
-                pairs.append(dv_pair)
-                dv_pair = None
-        if use_weight:
-            grads[lp + "Wv.weight"], grads[lp + "Wv.bias"] = dwv, dbv
-        K.gemm_nt(A, B, pairs, h, dprev, bias=a4, r1_row=gden, r1_col=st.tail[0], accumulate=acc)
-        if dv_pair is not None:         # bf16x3: 3 x 6 partial products exceed the GEMM's 16 segments
-            K.gemm_nt([A[2]], [B[1]], [(0, 0, 0, 0, d)], h, dprev, accumulate=True)
+        # attention (value-sum Gram form) + graph term: dv = dinv (.) A^T (dinv (.) c du)
+        dv = K.spmm(rp_t, col_t, graph.dinv, ys, heavy=graph.heavy_t) if use_graph else None
+        attention_gram_backward(P, lp, at, x_in, gnum, gden, cs, pg, sg, use_weight, prec, dprev, acc, grads, dv=dv)
         if i == 0 and dx0 is not None:
             dprev = K.axpby(dprev, dx0, 1.0, 1.0)
-        dcur, gs = dprev, 1.0
-    dg, db = (zeros(h), zeros(h)) if use_ln else (None, None)
-    dt0, _ = K.ln_bwd(dcur, tape["t0"], None, 1.0, 0.0, P.get("bns.0.weight"), P.get("bns.0.bias"), tape["st0"], use_ln, True, p,
-                      seed + 101, gs, False, dg, db)
-    if use_ln:
-        grads["bns.0.weight"], grads["bns.0.bias"] = dg, db
-    dt0_op = K.as_operand(dt0, prec.planes)
-    dw0 = torch.empty((h, d_in), dtype=torch.float32, device=dev)
-    K.gemm_tn(dt0_op, tape["xin"], dw0)
-    grads["fcs.0.weight"] = dw0
-    grads["fcs.0.bias"], _ = K.colstats(dt0, want_sumsq=False)
-    if want_dx:
-        dx = torch.empty((n, d_in), dtype=torch.float32, device=dev)
-        K.gemm_nt([dt0_op], [_w(P, "fcs.0.weight", prec, transpose=True)], [(0, 0, 0, 0, h)], d_in, dx)
-        return dx
-    return None
+        dcur = dprev
+    return _stem_backward(P, "", tape, dcur, 1.0, use_ln, prec, grads, want_dx)
 
 
 def difformer_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precision) -> List[Tensor]:
@@ -947,14 +905,12 @@ def difformer_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: 
     q~ k~^T / (q~ . sum_l k~_l + N).  The N x N product is one tensor-core GEMM of q and k with alpha = 1/(||q|| ||k||) read from
     the device and 1/den as its row scale (trans_attentions); the layer stack runs the Gram form.  Inference only, O(N^2) memory
     like the reference: meant for small graphs."""
-    h, d_in, nl = cfg["hidden"], cfg["in_channels"], cfg["num_layers"]
+    h, nl = cfg["hidden"], cfg["num_layers"]
     check_width(h, prec, "hidden_channels")
     n = xin.rows
     dev = xin.data.device
     use_ln, use_weight = bool(cfg["use_bn"]), bool(cfg["use_weight"])
-    t0 = K.gemm_nt([xin], [_w(P, "fcs.0.weight", prec)], [(0, 0, 0, 0, d_in)], h, K.alloc_act(n, h, prec.act_dtype, dev),
-                   bias=P["fcs.0.bias"])
-    x, _ = K.ln_fwd(t0, None, 1.0, 0.0, P.get("bns.0.weight"), P.get("bns.0.bias"), use_ln, True, 0.0, 0, False)
+    _, x, _ = _stem_forward(P, "", xin, h, use_ln, prec)
     x0 = x
     out = []
     for i in range(nl):
@@ -962,19 +918,12 @@ def difformer_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: 
         a, b, _, s_ = _difformer_coefs(cfg, i)
         at = Tape()
         o = attention_gram_forward(P, lp, x, use_weight, prec, at, vsum=True)
-        wqk, bqk = torch.cat([P[lp + "Wq.weight"], P[lp + "Wk.weight"]], 0), torch.cat([P[lp + "Wq.bias"], P[lp + "Wk.bias"]], 0)
-        qk = torch.empty((n, K.ceil_to(2 * h, 8)), dtype=prec.act_dtype, device=dev)[:, :2 * h]
-        K.gemm_nt([K.as_operand(x, prec.planes)], [K.pack_operand(wqk, False, prec.planes)], [(0, 0, 0, 0, h)], 2 * h, qk, bias=bqk)
+        qk, _, _ = _project_qkv(P, lp, K.as_operand(x, prec.planes), False, prec, stats=False)
         inv_den = at["den"].reciprocal()        # [N]: the Gram denominator is the reference's normaliser / N
         att = K.alloc_act(n, n, torch.float32, dev)
         K.gemm_nt([K.as_operand(qk[:, :h], prec.planes)], [K.as_operand(qk[:, h:], prec.planes)], [(0, 0, 0, 0, h)], n, att,
                   alpha=1.0 / at["n"], alpha_dev=at["st"].sc[K.SC_ALPHA:K.SC_ALPHA + 1], row_scale=inv_den)
         out.append(att)
-        if s_ and i > 0:
-            r, b = K.axpby(x, x0, b, s_), 1.0
-        elif s_ or b:
-            r, b = x, b + s_
-        else:
-            r = None
+        r, b = _difformer_residual(x, x0, i, b, s_)
         x, _ = K.ln_fwd(o, r, a, b, P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias"), use_ln, False, 0.0, 0, False)
     return out
