@@ -493,17 +493,29 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
 // accumulators into its own fp32 workspace partial (round-to-nearest, fixed order: deterministic) and restarts them from zero.
 constexpr int FLUSH_KB = 16;
 // ws[col * mp + row] (+)= acc for the accumulator rows mrow, mrow + 8 and columns 64 j + 8c + cq + e < ncols of the chunks
-// j in [j0, 4); acc is zeroed.
+// j in [j0, 4); acc is zeroed.  The partials are loaded BATCH at a time before any of them is stored: interleaved, every
+// load would wait for the previous store (the compiler cannot tell the addresses apart), one L2 round trip per element, and the
+// flushes of a 2.45 M-row product would stall the MMA warps for longer than the products themselves take.  BATCH is the
+// largest that does not spill at the 168 registers of the caller (gemm_tn 16, gram 8).
+template <int BATCH>
 __device__ __forceinline__ void flush_acc(float (&acc)[4][32], float* ws, int mp, int mrow, int cq, int j0, int ncols, bool add) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         if (j < j0) continue;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-            const int col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
-            float* w = ws + (int64_t)col * mp + mrow + 8 * ((i >> 1) & 1);
-            if (col < ncols) *w = add ? *w + acc[j][i] : acc[j][i];
-            acc[j][i] = 0.f;
+        for (int i0 = 0; i0 < 32; i0 += BATCH) {
+            float old[BATCH];
+#pragma unroll
+            for (int q = 0; q < BATCH; ++q) {
+                const int i = i0 + q, col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
+                old[q] = (add && col < ncols) ? ws[(int64_t)col * mp + mrow + 8 * ((i >> 1) & 1)] : 0.f;
+            }
+#pragma unroll
+            for (int q = 0; q < BATCH; ++q) {
+                const int i = i0 + q, col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
+                if (col < ncols) ws[(int64_t)col * mp + mrow + 8 * ((i >> 1) & 1)] = add ? old[q] + acc[j][i] : acc[j][i];
+                acc[j][i] = 0.f;
+            }
         }
     }
 }
@@ -619,11 +631,11 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1) {
-            flush_acc(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
+            flush_acc<16>(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
             flushed = true;
         }
     }
-    flush_acc(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
+    flush_acc<16>(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
 }
 
 // out[i,j] = alpha * sum_cta ws[cta][j][i] (+ beta*out[i,j]);  i < m, j < n
@@ -732,7 +744,7 @@ __global__ void __launch_bounds__(THREADS, 1) gram_kernel(const __grid_constant_
     bool flushed = false;
     // G partial of the chunks j >= ic, then column 0 of the ones product (X^T 1) as workspace column un
     auto flush = [&]() {
-        flush_acc(acc, ws, p.mp, mrow, cq, ic, p.un, flushed);
+        flush_acc<8>(acc, ws, p.mp, mrow, cq, ic, p.un, flushed);
         if (cq == 0) {
             float* w = ws + (int64_t)p.un * p.mp + mrow;
             w[0] = flushed ? w[0] + accs[0] : accs[0];
