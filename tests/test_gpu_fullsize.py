@@ -61,6 +61,61 @@ def test_spmm_properties_products_shape(products):
     assert rel < 8e-3, f"bf16 vs fp32 SpMM: {rel:.2e}"
 
 
+def _spmm_ref_int(ei, n, xi):
+    """Exact y[r] = sum of xi[c] over the edges (c -> r) of the edge list, in int32 (edge chunks; |y| <= degree)."""
+    out = torch.zeros_like(xi)
+    for i in range(0, ei.shape[1], 1 << 19):
+        out.index_add_(0, ei[1, i:i + (1 << 19)], xi.index_select(0, ei[0, i:i + (1 << 19)]))
+    return out
+
+
+def _check_spmm_exact(K, rowptr, col, dinv, heavy, ei, n):
+    """Integer features make every row sum exact in fp32, whatever the order: the SpMM must equal the edge-list sum bit for bit
+    (bf16 outputs after round-to-nearest-even).  With the row scale dinv the kernel rounds the exact sum times dinv once (fp32),
+    which is what fp64 rounds to as well (a 24-bit integer times a 24-bit fp32 is exact in fp64)."""
+    gen = torch.Generator(device=DEV).manual_seed(5)
+    for dtype, h, lo in ((torch.bfloat16, 256, -1), (torch.float32, 64, -2)):
+        xi = torch.randint(lo, -lo + 1, (n, h), generator=gen, device=DEV, dtype=torch.int32)
+        ref = _spmm_ref_int(ei, n, xi).float()                  # exact: |sum| <= max degree < 2^24
+        x = xi.to(dtype)
+        del xi
+        y = K.spmm(rowptr, col, None, x, heavy=heavy)
+        want = ref.to(dtype)                                    # bf16: round-to-nearest-even of the exact sum
+        assert torch.equal(y, want), f"{dtype} h={h}: {int((y != want).sum())} elements differ"
+        del y, want
+        y = K.spmm(rowptr, col, dinv, x, heavy=heavy)
+        for i in range(0, n, 1 << 18):
+            want = (ref[i:i + (1 << 18)].double() * dinv[i:i + (1 << 18)].double()[:, None]).float().to(dtype)
+            got = y[i:i + (1 << 18)]
+            assert torch.equal(got, want), f"{dtype} h={h} with dinv, rows from {i}: {int((got != want).sum())} elements differ"
+        del x, y, ref
+
+
+def test_spmm_exact_products_shape(products):
+    """The products SpMM against an independent exact reference (the int32 sum over the edge list): which columns each row
+    gathers, not only how many (A.1 = degree) or that it is linear."""
+    from sgformer_b200 import kernels as K
+    n, ei, g = products
+    _check_spmm_exact(K, g.rowptr, g.col, g.dinv, g.heavy, ei, n)
+
+
+def test_spmm_heavy_rows_exact_products_size():
+    """The segmented hub-row path (heavy=) on a power-law graph of the products size, exactly; the single-warp path on the
+    same rows too."""
+    from sgformer_b200 import kernels as K
+    from sgformer_b200.graph import Graph
+    from sgformer_b200.synth import SHAPES, make_rmat_graph
+    n, _, e = SHAPES["products"][:3]
+    ei = make_rmat_graph(n, e, seed=1, device=DEV)
+    g = Graph(ei, n)
+    lens = g.rowptr[1:] - g.rowptr[:-1]
+    assert g.heavy is not None and int(lens.max()) > 8 * K.HEAVY_ROW
+    assert bool(((g.heavy.seg_len > 0) & (g.heavy.seg_len <= K.HEAVY_ROW)).all())
+    assert bool((lens[g.heavy.rows] % K.HEAVY_ROW != 0).any()), "some hub row must end in a short segment"
+    _check_spmm_exact(K, g.rowptr, g.col, g.dinv, g.heavy, ei, n)
+    _check_spmm_exact(K, g.rowptr, g.col, g.dinv, None, ei, n)
+
+
 def test_attention_conservation_laws_pokec_shape():
     """With v = 1 every output is exactly 1 (num = q~.z + N = den); in general the output stays within O(N^-1.5) of v."""
     from sgformer_b200 import engine as E

@@ -799,7 +799,7 @@ def test_gram_attention_layer_vs_fp64(K, n, h, use_weight, residual):
 
 
 @pytest.mark.parametrize("rows,h", [(1, 16), (63, 64), (64, 64), (1000, 128), (20000, 256), (5000, 100), (4097, 200), (300000, 256),
-                                    (777, 8)])
+                                    (777, 8), (300000, 64), (300000, 100), (300000, 128)])
 @pytest.mark.parametrize("planes", [1, 3])
 def test_gram_kernel(K, monkeypatch, rows, h, planes):
     """sgf_gram (X^T X with one operand load, upper block triangle mirrored, X^T 1 as an MMA column) against fp64, and against
