@@ -137,6 +137,36 @@ int sgf_spmm_heavy(const int32_t* col, const float* row_scale, const void* x, in
                    int dtype, const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg, float* partial,
                    const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * K12 — GAT edge softmax (replaces PyG GATConv's message passing as medium/models.py:116-155 uses it: per-edge logits, softmax
+ * over the in-edges of each target, attention dropout, weighted aggregation).  rowptr/col: the CSR of sgf_csr_build with
+ * self_loop_mode 1 (existing self loops dropped, one per node added: remove_self_loops + add_self_loops); rowptr_t/col_t: the
+ * same pattern built by_source.  xp = x W^T [n, heads*c] (activation dtype, 16-byte aligned rows); a_src, a_dst, lse, r_ws:
+ * fp32 [n, heads]; da_src, da_dst: fp32 [heads, n].  c must be a multiple of 4 (fp32) / 8 (bf16), heads*c at most 512 (fp32) /
+ * 1024 (bf16), heads <= SGF_GAT_MAX_HEADS.
+ *   e_ij = leaky_relu(a_src[j] + a_dst[i], 0.2);  alpha_ij = exp(e_ij - lse_i);  y_i = sum_j alpha_ij d_ij xp_j
+ *   out_i = (mean ? mean over heads of y_i : y_i) + bias  (bias nullable; out [n, c] or [n, heads*c] in the activation dtype)
+ * d_ij = attention dropout (p, seed + the dropout epoch): 0 or 1/(1-p) from a hash of (target, source, duplicate rank, head), so the
+ * forward and both backward traversals draw the same mask.  No float atomics: every launch is bit-identical run to run.
+ * sgf_gat_logits: a_src[n,h] = <xp[n,h,:], att_src[h,:]>, a_dst likewise (att_* fp32 [heads*c]).
+ * sgf_gat_bwd, given g = dL/dout: pass 1 over the CSR writes r_i = <g_i, y_i> per head and da_dst; pass 2 over the transposed CSR
+ * rebuilds alpha_ij from a_src, a_dst and lse and writes dxp_j = sum_i alpha_ij d_ij g_i + da_src_j att_src + da_dst_j att_dst
+ * (the full gradient of xp, logits included) and da_src.
+ * sgf_dense_dropout: y = dropout(x) for an fp32 matrix (GAT's input dropout), one hash of (seed + epoch, r*cols + c) per element.
+ * ------------------------------------------------------------------------------------------------ */
+#define SGF_GAT_MAX_HEADS 8
+int sgf_gat_logits(const void* xp, int64_t ldx, int64_t n, int heads, int c, int dtype, const float* att_src, const float* att_dst,
+                   float* a_src, float* a_dst, void* stream);
+int sgf_gat_fwd(const int64_t* rowptr, const int32_t* col, const void* xp, int64_t ldx, const float* a_src, const float* a_dst,
+                int64_t n, int heads, int c, int dtype, int mean, const float* bias, void* out, int64_t ldo, float* lse, float p,
+                uint64_t seed, void* stream);
+int sgf_gat_bwd(const int64_t* rowptr, const int32_t* col, const int64_t* rowptr_t, const int32_t* col_t, const void* xp, int64_t ldx,
+                const float* a_src, const float* a_dst, const float* lse, const void* g, int64_t ldg, const float* att_src,
+                const float* att_dst, int64_t n, int heads, int c, int dtype, int mean, float p, uint64_t seed, float* r_ws,
+                float* da_src, float* da_dst, void* dxp, int64_t ldd, void* stream);
+int sgf_dense_dropout(const float* x, int64_t ldx, int64_t rows, int64_t cols, float p, uint64_t seed, float* y, int64_t ldy,
+                      void* stream);
+
 /* Row-sharded SpMM fused with the halo exchange (SURVEY.md §8e C4): as sgf_spmm, but x is the gathered operand
  * [n_slots*slot_rows, h] of which only slot 0 (this rank's own rows) is present at launch; slot s > 0 (the rows of rank
  * (rank + s) mod world) is being written by that rank over NVLink (copy-engine peer copy into this buffer) and is complete once
@@ -278,7 +308,9 @@ int sgf_ln_bwd(const void* dy, const void* x, const void* r, int64_t ld, int64_t
  * sgf_bn_finalize: batch statistics from column sums of z (training; sum/sumsq non-NULL; updates the running buffers
  * with momentum and the unbiased variance when they are non-NULL) or the running statistics (sum == NULL).  zbias
  * (nullable) is a per-column bias added to z before normalisation (GCNConv's bias): it only shifts the mean.
- * sgf_bn_fwd:  t = use_bn ? gamma*((z+zbias)-mean)*rstd+beta : z+zbias;  t = relu?(t);  t = dropout(t);  t += res?;
+ * use_relu of the BatchNorm entry points is an activation code: 0 none, 1 ReLU, 2 ELU (alpha 1; GAT's F.elu, backward exp(t) for
+ * t <= 0).
+ * sgf_bn_fwd:  t = use_bn ? gamma*((z+zbias)-mean)*rstd+beta : z+zbias;  t = act(t);  t = dropout(t);  t += res?;
  *   y_scaled (nullable) = row_scale[r]*t;   if mix: t = gw*t + (1-gw)*mix[r,:];   y (nullable) = t. */
 int sgf_bn_finalize(const float* sum, const float* sumsq, int64_t rows, int h, float eps, float momentum,
                     const float* zbias, float* mean, float* rstd, float* running_mean, float* running_var, void* stream);
@@ -287,7 +319,7 @@ int sgf_bn_fwd(const void* z, const void* res, const void* mix, int64_t ld, int6
                int use_bn, int use_relu, float p, uint64_t seed, float gw, const float* row_scale, void* y,
                void* y_scaled, void* stream);
 /* backward.  Upstream gradient g_raw = gscale*(dy + row_scale2[r]*dy2) (dy or dy2 nullable, not both);
- * g = g_raw * dropout mask * relu mask.
+ * g = g_raw * dropout mask * act'(pre-activation).
  * phase 1 (training BN only): sums[0:h] += g, sums[h:2h] += g*xhat   (caller-zeroed fp32 [2h]; == dbeta, dgamma)
  * phase 2: dz = gamma*rstd*(g - sums_g/rows - xhat*sums_gx/rows) (training BN) | gamma*rstd*g (eval BN) | g (no BN);
  *   dz is written times out_row_scale[r] (nullable); dz_colsum[c] += dz (unscaled; bias gradient; nullable);

@@ -152,6 +152,12 @@ _SIGS = {
                                        _i64, _vp, _vp]),
     "sgf_attn_bwd_prep": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.c_int, C.c_int, _f32, _vp, _i64, _vp, _vp]),
     "sgf_attn_combine_scal": (C.c_int, [_vp, C.c_int, C.c_int, _vp, _vp]),
+    "sgf_gat_logits": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "sgf_gat_fwd": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _i64, _vp, _f32,
+                              _u64, _vp]),
+    "sgf_gat_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int,
+                              C.c_int, _f32, _u64, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "sgf_dense_dropout": (C.c_int, [_vp, _i64, _i64, _i64, _f32, _u64, _vp, _i64, _vp]),
     "sgf_attn_prepare_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _i64, _vp, _i64, _vp, _i64, _i64,
                                        _i64, _vp, _vp, _vp, _vp]),
 }

@@ -276,6 +276,12 @@ __device__ __forceinline__ void dropout_chunk(uint64_t seed, uint64_t chunk_id, 
         }
     }
 }
+// The device epoch word registered by sgf_set_dropout_epoch (rowops.cu), or null.
+const uint64_t* dropout_epoch_word();
+
+// Activation codes of the BatchNorm kernels' `use_relu` argument: 0 none, 1 ReLU, kActElu ELU (alpha 1; GAT's F.elu).
+constexpr int kActElu = 2;
+
 __host__ __device__ __forceinline__ uint32_t dropout_thr16(float p) { return static_cast<uint32_t>(p * 65536.f + 0.5f); }
 __host__ __device__ __forceinline__ float dropout_inv_keep(uint32_t thr16) { return 65536.f / (65536.f - static_cast<float>(thr16)); }
 

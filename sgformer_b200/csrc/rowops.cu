@@ -23,6 +23,7 @@ constexpr float kLnEps = 1e-5f;
 // (sgf_set_dropout_epoch).  A step captured in a CUDA graph bakes the host seed into the graph; the epoch, advanced by a
 // node of the same graph, is what makes every replay draw fresh masks (forward and backward of one step read the same value).
 static const uint64_t* g_dropout_epoch = nullptr;
+const uint64_t* dropout_epoch_word() { return g_dropout_epoch; }
 struct SeedArg {
     uint64_t base;
     const uint64_t* epoch;
@@ -661,7 +662,8 @@ __global__ void __launch_bounds__(kRowBlock, 3) bn_fwd_kernel(const T* __restric
             if (mix) L.load_raw(mix, ld, rn, nm);
         }
         SGF_FOR_ELEMS v[c][i] = v[c][i] * sc[c][i] + sh[c][i];
-        if (use_relu) SGF_FOR_ELEMS v[c][i] = fmaxf(v[c][i], 0.f);
+        if (use_relu == kActElu) SGF_FOR_ELEMS v[c][i] = v[c][i] > 0.f ? v[c][i] : expm1f(v[c][i]);
+        else if (use_relu) SGF_FOR_ELEMS v[c][i] = fmaxf(v[c][i], 0.f);
         if (DROP) L.dropout(v, seed, r, chunks, thr16, inv_keep);
         if (res) SGF_FOR_ELEMS v[c][i] += tr[c][i];
         if (y_scaled) {
@@ -827,7 +829,12 @@ __global__ void __launch_bounds__(kRowBlock, 2) bn_bwd_kernel(const T* __restric
         SGF_FOR_ELEMS {
             const float zv = zz[c][i];
             float gg = gy[c][i];
-            if (use_relu && zv * sc[c][i] + sh[c][i] <= 0.f) gg = 0.f;
+            if (use_relu == kActElu) {
+                const float pre = zv * sc[c][i] + sh[c][i];
+                if (pre <= 0.f) gg *= expf(pre);
+            } else if (use_relu && zv * sc[c][i] + sh[c][i] <= 0.f) {
+                gg = 0.f;
+            }
             if (APPLY) {
                 const float d = sc[c][i] * gg - q0[c][i] - q1[c][i] * zv;
                 a1[c][i] += L.cval[c] ? d : 0.f;

@@ -69,6 +69,9 @@ _SEED_LAYER = 211           # + i: TransConv / DIFFormer layer i
 _SEED_GCONV_STEM = 307      # GraphConv input layer
 _SEED_GCONV_LAYER = 401     # + i: GraphConv layer i
 _SEED_GCN_LAYER = 503       # + i: GCN layer i
+_SEED_GAT_INPUT = 601       # GAT input dropout
+_SEED_GAT_ACT = 611         # + i: dropout after GAT layer i's ELU
+_SEED_GAT_ATT = 653         # + i: attention dropout of GAT layer i
 
 
 def check_width(h: int, prec: Precision, what: str):
@@ -737,6 +740,147 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         elif want_dx:
             dx = torch.empty((n, L["cur_k"]), dtype=torch.float32, device=dev)
             K.gemm_nt([u_op], [_w(P, wname, prec, transpose=True)], [(0, 0, 0, 0, hout)], L["cur_k"], dx)
+    return dx
+
+
+# =================================================================================================
+# GAT backbone (medium): PyG GATConv stack
+# =================================================================================================
+# Layer i:  xp = x W^T [N, H*C] (GEMM),  a_src / a_dst = per-head dots of xp with att_src / att_dst (sgf_gat_logits, one row pass:
+# the logits come from the same rounded xp the aggregation gathers, in either precision),  z = edge softmax aggregation + bias
+# (sgf_gat_fwd; concat for the hidden layers, head mean for the last), then BatchNorm?/ELU/dropout in one bn_fwd pass whose
+# statistics come from one colstats pass.  Backward: bn_bwd (ELU code), sgf_gat_bwd (two gathers: forward CSR, then transposed
+# CSR) -> dxp incl. the logits' share, d att_* by per-head weighted column sums, dW and dx by the GEMMs.
+def _gat_dims(P, pfx: str, i: int):
+    att = P[f"{pfx}convs.{i}.att_src"]
+    return int(att.shape[-2]), int(att.shape[-1])
+
+
+def _gat_layer(P, lp: str, heads: int, c: int, mean: bool, prec: Precision, i: int):
+    """-> (cp, weight [heads*cp, in], att_src [heads*cp], att_dst [heads*cp], bias) of layer i.  The kernels move rows in 16-byte
+    chunks per head, so a head-mean layer (the last conv: out_channels = classes in `--method gat`) whose width is not a multiple of
+    4 (fp32) / 8 (bf16) runs on zero-padded heads: the padded channels have zero weights and attention vectors, so they change
+    neither the logits nor the real channels, and the output is the real columns of the padded one."""
+    vn = 8 if prec.name == "bf16" else 4
+    cp = K.ceil_to(c, vn)
+    hc_max = 1024 if prec.name == "bf16" else 512
+    if heads > K.GAT_MAX_HEADS or (cp != c and not mean) or heads * cp > hc_max:
+        raise ValueError(f"sgformer_b200 GAT layer {i}: heads={heads}, out_channels={c} is not supported in precision '{prec.name}': "
+                         f"heads must be at most {K.GAT_MAX_HEADS}, the out_channels of a concatenating layer a multiple of {vn} and "
+                         f"heads*out_channels at most {hc_max}")
+    w, a_s, a_d, b = P[lp + "lin_src.weight"], P[lp + "att_src"].reshape(-1), P[lp + "att_dst"].reshape(-1), P[lp + "bias"]
+    if cp == c:
+        return cp, w, a_s, a_d, b
+    dev = w.device
+
+    def pad(t, rows):      # [heads*c, ...] -> [heads*cp, ...], zeros in each head's padding
+        out = torch.zeros((heads, cp) + tuple(t.shape[1:]), dtype=torch.float32, device=dev)
+        out[:, :c] = t.detach().reshape((heads, c) + tuple(t.shape[1:]))
+        return out.reshape((heads * cp,) + tuple(t.shape[1:]))
+    bp = torch.zeros(cp, dtype=torch.float32, device=dev)
+    bp[:c] = b.detach()
+    return cp, pad(w, True), pad(a_s, False), pad(a_d, False), bp
+
+
+def gat_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, training: bool, seed: int,
+                tape: Optional[Tape], mix: Optional[Tensor] = None, gw: float = 1.0, pfx: str = "gnn.",
+                comm: Comm = SINGLE, x_raw: Optional[Tensor] = None) -> Tensor:
+    """models.GAT.forward (medium/models.py:145-155).  `graph`: self_loop_mode 1 (remove_self_loops + add_self_loops); x_raw: the
+    fp32 node features xin was packed from (input dropout)."""
+    if comm.active:
+        raise NotImplementedError("sgformer_b200: row sharding of the GAT branch is not supported")
+    nl = cfg["gcn_num_layers"]
+    n = xin.rows
+    dev = xin.data.device
+    p = float(cfg["gcn_dropout"]) if training else 0.0
+    use_bn = bool(cfg["gcn_use_bn"])
+    cur_op = xin
+    if p > 0.0:
+        xr = x_raw if x_raw.dtype == torch.float32 and x_raw.stride(-1) == 1 else x_raw.float().contiguous()
+        cur_op = K.pack_operand(K.dense_dropout(xr, p, seed + _SEED_GAT_INPUT), False, prec.planes)
+    layers = []
+    out = None
+    for i in range(nl):
+        last = i == nl - 1
+        H, C = _gat_dims(P, pfx, i)
+        lp = f"{pfx}convs.{i}."
+        cp, w, att_s, att_d, bias = _gat_layer(P, lp, H, C, last, prec, i)
+        xp = K.gemm_nt([cur_op], [K.pack_operand(w, False, prec.planes)], [(0, 0, 0, 0, cur_op.k)], H * cp,
+                       K.alloc_act(n, H * cp, prec.act_dtype, dev))
+        a_s, a_d = K.gat_logits(xp, H, cp, att_s, att_d)
+        z, lse = K.gat_fwd(graph.rowptr, graph.col, xp, a_s, a_d, H, cp, last, bias, p, seed + _SEED_GAT_ATT + i)
+        if cp != C:
+            z = z[:, :C]
+        L = dict(cur_op=cur_op, xp=xp, a_s=a_s, a_d=a_d, lse=lse, H=H, C=C, cp=cp, w=w, att=(att_s, att_d))
+        if last:
+            out = K.axpby(z, mix, gw, 1.0 - gw) if mix is not None else z
+        else:
+            name = f"{pfx}bns.{i}."
+            mean, rstd = _bn_stats(z, P, name, use_bn, training)
+            y, _ = K.bn_fwd(z, None, None, mean, rstd, P.get(name + "weight"), P.get(name + "bias"), None, use_bn, K.ACT_ELU, p,
+                            seed + _SEED_GAT_ACT + i, 1.0, None, True, False)
+            L.update(z=z, mean=mean, rstd=rstd)
+            cur_op = K.as_operand(y, prec.planes)
+        layers.append(L)
+    if tape is not None:
+        tape.update(layers=layers, p=p, seed=seed, n=n, training=training, mixed=mix is not None, gw=gw)
+    return out
+
+
+def gat_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Precision, grads: Dict[str, Tensor],
+                 pfx: str = "gnn.", want_dx: bool = False, comm: Comm = SINGLE) -> Optional[Tensor]:
+    nl = cfg["gcn_num_layers"]
+    n, p, seed, training = tape["n"], tape["p"], tape["seed"], tape["training"]
+    dev = dout.device
+    use_bn = bool(cfg["gcn_use_bn"])
+    rp_t, col_t = graph.transpose()
+    gs = tape["gw"] if tape["mixed"] else 1.0
+    dcur = dout
+    dx = None
+    for i in reversed(range(nl)):
+        L = tape["layers"][i]
+        last = i == nl - 1
+        lp = f"{pfx}convs.{i}."
+        H, C, cp = L["H"], L["C"], L["cp"]
+        if last:
+            g = K.axpby(dcur, None, gs, 0.0) if gs != 1.0 else dcur
+        else:
+            name = f"{pfx}bns.{i}."
+            g, sums, _ = K.bn_bwd(dcur, None, None, L["z"], L["mean"], L["rstd"], P.get(name + "weight"), P.get(name + "bias"), None,
+                                  use_bn, K.ACT_ELU, training, p, seed + _SEED_GAT_ACT + i, 1.0)
+            if use_bn and training:
+                _bn_param_grads(grads, comm, P, name, sums, dcur, None, None, L["z"], L["mean"], L["rstd"], K.ACT_ELU)
+        if cp != C:            # zero-padded heads (see _gat_layer): the gradient of the padding columns is zero
+            gp = torch.zeros((n, cp), dtype=g.dtype, device=dev)
+            K.axpby(g, None, 1.0, 0.0, out=gp[:, :C])
+            g = gp
+        db, _ = K.colstats(g, want_sumsq=False)
+        grads[lp + "bias"] = db if cp == C else db[:C]
+        att_s, att_d = L["att"]
+        xp = L["xp"]
+        dxp, da_s, da_d = K.gat_bwd(graph.rowptr, graph.col, rp_t, col_t, xp, L["a_s"], L["a_d"], L["lse"], g, att_s, att_d, H, cp,
+                                    last, p, seed + _SEED_GAT_ATT + i)
+        datt_s = torch.zeros((H, cp), dtype=torch.float32, device=dev)
+        datt_d = torch.zeros((H, cp), dtype=torch.float32, device=dev)
+        for hd in range(H):
+            xh = xp[:, hd * cp:(hd + 1) * cp]
+            K.colstats(xh, w=da_s[hd], want_sumsq=False, sum_out=datt_s[hd])
+            K.colstats(xh, w=da_d[hd], want_sumsq=False, sum_out=datt_d[hd])
+        grads[lp + "att_src"], grads[lp + "att_dst"] = datt_s[:, :C], datt_d[:, :C]
+        dxp_op = K.as_operand(dxp, prec.planes)
+        cur_op = L["cur_op"]
+        dw = torch.empty((H * cp, cur_op.k), dtype=torch.float32, device=dev)
+        K.gemm_tn(dxp_op, cur_op, dw)
+        grads[lp + "lin_src.weight"] = dw if cp == C else dw.view(H, cp, -1)[:, :C].reshape(H * C, -1)
+        wt = K.pack_operand(L["w"], True, prec.planes)
+        if i > 0:
+            dcur = K.alloc_act(n, cur_op.k, prec.act_dtype, dev)
+            K.gemm_nt([dxp_op], [wt], [(0, 0, 0, 0, H * cp)], cur_op.k, dcur)
+        elif want_dx:
+            dx = torch.empty((n, cur_op.k), dtype=torch.float32, device=dev)
+            K.gemm_nt([dxp_op], [wt], [(0, 0, 0, 0, H * cp)], cur_op.k, dx)
+            if p > 0.0:
+                dx = K.dense_dropout(dx, p, seed + _SEED_GAT_INPUT)
     return dx
 
 

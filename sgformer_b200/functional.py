@@ -5,6 +5,7 @@ the others back the standalone modules/functions of the reference surface (Trans
 full_attention_conv, GraphConvLayer's SpMM, nn.Linear on the tensor-core GEMM)."""
 from __future__ import annotations
 
+import functools
 import threading
 from typing import Dict, Optional, Sequence
 
@@ -98,7 +99,12 @@ class SGFormerFn(_TapeFunction):
         gw = float(cfg["graph_weight"])
         if cfg["use_graph"]:
             add = cfg["aggregate"] == "add"
-            fwd = E.gcn_forward if cfg["variant"] == "medium" else E.gconv_forward
+            if cfg["variant"] != "medium":
+                fwd = E.gconv_forward
+            elif cfg["gnn_kind"] == "gat":
+                fwd = functools.partial(E.gat_forward, x_raw=x)
+            else:
+                fwd = E.gcn_forward
             x2 = fwd(P, cfg, xin, graph, prec, training, seed, tg, mix=x1 if add else None, gw=gw, comm=comm)
             feats = [x2] if add else [x1, x2]
         else:
@@ -119,7 +125,7 @@ class SGFormerFn(_TapeFunction):
         gw = float(cfg["graph_weight"])
         dx = None
         if cfg["use_graph"]:
-            bwd = E.gcn_backward if cfg["variant"] == "medium" else E.gconv_backward
+            bwd = E.gconv_backward if cfg["variant"] != "medium" else E.gat_backward if cfg["gnn_kind"] == "gat" else E.gcn_backward
             if cfg["aggregate"] == "add":
                 dm = dfeats[0]
                 dxg = bwd(P, cfg, tg, graph, dm, prec, grads, want_dx=want_dx, comm=comm)
@@ -190,14 +196,18 @@ class TransConvFn(_TapeFunction):
 
 
 class GraphBranchFn(_TapeFunction):
-    """Standalone GNN branch: GraphConv (large/100M) or the PyG-GCN backbone (medium).  Returns [N, h] in x's dtype."""
+    """Standalone GNN branch: GraphConv (large/100M), the PyG-GCN or the PyG-GAT backbone (medium).  Returns [N, h] in x's
+    dtype."""
 
     @staticmethod
     def forward(ctx, x, graph, cfg, prec, training, kind, pfx, names, *params):
         P = _pdict(names, params)
         need_tape = _want_tape(ctx)
         tape = E.Tape() if need_tape else None
-        fwd = E.gcn_forward if kind == "gcn" else E.gconv_forward
+        if kind == "gat":
+            fwd = functools.partial(E.gat_forward, x_raw=x)
+        else:
+            fwd = E.gcn_forward if kind == "gcn" else E.gconv_forward
         out = fwd(P, cfg, E.input_operand(x, prec), graph, prec, training, E.next_seed(), tape, pfx=pfx)
         if need_tape:
             ctx.state = (cfg, prec, graph, kind, pfx, names, params, tape, x.requires_grad)
@@ -207,7 +217,7 @@ class GraphBranchFn(_TapeFunction):
     def backward(ctx, dout):
         cfg, prec, graph, kind, pfx, names, params, tape, want_dx = ctx.state
         grads: Dict[str, Tensor] = {}
-        bwd = E.gcn_backward if kind == "gcn" else E.gconv_backward
+        bwd = E.gat_backward if kind == "gat" else E.gcn_backward if kind == "gcn" else E.gconv_backward
         dx = bwd(_pdict(names, params), cfg, tape, graph, _to_act(dout, prec), prec, grads, pfx=pfx, want_dx=want_dx)
         ctx.state = None
         return (dx, None, None, None, None, None, None, None, *_grad_list(names, params, grads))

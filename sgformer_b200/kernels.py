@@ -811,6 +811,68 @@ def head_mean(x: Tensor, heads: int, d: int) -> Tensor:
 
 
 # ------------------------------------------------------------------------------------------------
+# GAT edge softmax (csrc/gat.cu)
+# ------------------------------------------------------------------------------------------------
+ACT_ELU = 2          # `use_relu` code of bn_fwd / bn_bwd for ELU (GAT's F.elu)
+GAT_MAX_HEADS = 8    # SGF_GAT_MAX_HEADS
+
+
+def gat_logits(xp: Tensor, heads: int, c: int, att_src: Tensor, att_dst: Tensor) -> Tuple[Tensor, Tensor]:
+    """xp [N, heads*c] -> (a_src, a_dst) fp32 [N, heads]."""
+    _use(xp)
+    n, _, ld = _mat(xp, "xp")
+    a_src = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
+    a_dst = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
+    check(lib().sgf_gat_logits(_p(xp), ld, n, heads, c, dcode(xp), _p(_f32vec(att_src, heads * c, "att_src")),
+                               _p(_f32vec(att_dst, heads * c, "att_dst")), _p(a_src), _p(a_dst), _stream()), "sgf_gat_logits")
+    return a_src, a_dst
+
+
+def gat_fwd(rowptr: Tensor, col: Tensor, xp: Tensor, a_src: Tensor, a_dst: Tensor, heads: int, c: int, mean: bool,
+            bias: Optional[Tensor], p: float, seed: int) -> Tuple[Tensor, Tensor]:
+    """-> (out [N, c] if mean else [N, heads*c] in xp's dtype, lse fp32 [N, heads]).  See sgf_gat_fwd."""
+    _use(xp)
+    n, _, ld = _mat(xp, "xp")
+    out = alloc_act(n, c if mean else heads * c, xp.dtype, xp.device)
+    lse = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
+    check(lib().sgf_gat_fwd(_p(rowptr), _p(col), _p(xp), ld, _p(a_src), _p(a_dst), n, heads, c, dcode(xp), int(mean),
+                            _p(_f32vec(bias, out.shape[1], "bias")), _p(out), out.stride(0), _p(lse), p, seed, _stream()),
+          "sgf_gat_fwd")
+    return out, lse
+
+
+def gat_bwd(rowptr: Tensor, col: Tensor, rowptr_t: Tensor, col_t: Tensor, xp: Tensor, a_src: Tensor, a_dst: Tensor, lse: Tensor,
+            g: Tensor, att_src: Tensor, att_dst: Tensor, heads: int, c: int, mean: bool, p: float, seed: int):
+    """g = dL/dout -> (dxp [N, heads*c] in xp's dtype, da_src fp32 [heads, N], da_dst fp32 [heads, N]).  See sgf_gat_bwd."""
+    _use(xp)
+    n, _, ld = _mat(xp, "xp")
+    _, _, ldg = _mat(g, "g")
+    if g.dtype != xp.dtype:
+        raise TypeError("gat_bwd: g and xp must share the activation dtype")
+    dev = xp.device
+    r_ws = torch.empty((n, heads), dtype=torch.float32, device=dev)
+    da_src = torch.empty((heads, n), dtype=torch.float32, device=dev)
+    da_dst = torch.empty((heads, n), dtype=torch.float32, device=dev)
+    dxp = new_like(xp)
+    check(lib().sgf_gat_bwd(_p(rowptr), _p(col), _p(rowptr_t), _p(col_t), _p(xp), ld, _p(a_src), _p(a_dst), _p(lse), _p(g), ldg,
+                            _p(_f32vec(att_src, heads * c, "att_src")), _p(_f32vec(att_dst, heads * c, "att_dst")), n, heads, c,
+                            dcode(xp), int(mean), p, seed, _p(r_ws), _p(da_src), _p(da_dst), _p(dxp), dxp.stride(0), _stream()),
+          "sgf_gat_bwd")
+    return dxp, da_src, da_dst
+
+
+def dense_dropout(x: Tensor, p: float, seed: int) -> Tensor:
+    """fp32 [rows, cols] -> dropout(x) (sgf_dense_dropout; the same (p, seed) applied to a gradient is its backward)."""
+    _use(x)
+    rows, cols, ld = _mat(x, "x")
+    if x.dtype != torch.float32:
+        raise TypeError("dense_dropout expects fp32")
+    y = alloc_act(rows, cols, torch.float32, x.device)
+    check(lib().sgf_dense_dropout(_p(x), ld, rows, cols, p, seed, _p(y), y.stride(0), _stream()), "sgf_dense_dropout")
+    return y
+
+
+# ------------------------------------------------------------------------------------------------
 # attention glue
 # ------------------------------------------------------------------------------------------------
 def attn_prepare_fwd(s_raw: Tensor, z_raw: Tensor, nq2v: Tensor, nk2v: Tensor, planes: int):

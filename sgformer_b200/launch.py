@@ -16,6 +16,10 @@ def main(argv=None):
     ap = argparse.ArgumentParser(prog="python -m sgformer_b200.launch")
     ap.add_argument("--variant", required=True, choices=["large", "medium", "100M"])
     ap.add_argument("--precision", choices=["bf16", "fp32"], default=None)
+    ap.add_argument("--native-backbones", action="store_true",
+                    help="medium: make the GAT and GCN that the reference's parse.py builds backbones from resolve to "
+                         "sgformer_b200.medium.GAT / GCN, so that --backbone gat|gcn (and --method gat|gcn) run on the kernels "
+                         "(models.py still imports torch_geometric)")
     ap.add_argument("script")
     ap.add_argument("script_args", nargs=argparse.REMAINDER)
     a = ap.parse_args(argv)
@@ -26,6 +30,16 @@ def main(argv=None):
     sys.path[:0] = [os.path.join(HERE, "dropin", a.variant), sdir]
     sys.argv = [script] + a.script_args
     os.chdir(sdir)
+    if a.native_backbones:
+        if a.variant != "medium":
+            ap.error("--native-backbones applies to --variant medium")
+        # parse.py star-imports models, ours, ..., graphtrans (whose own GCN shadows models.GCN); parse_method looks the classes up
+        # in parse's namespace, so that is where they are replaced (main.py's `from parse import ...` then reuses this module)
+        import models
+        import parse
+        from . import medium
+        for mod in (models, parse):
+            mod.GAT, mod.GCN = medium.GAT, medium.GCN
     runpy.run_path(script, run_name="__main__")
 
 

@@ -1,5 +1,6 @@
-"""Drop-in for the reference's medium/ours.py (`--method ours`, medium/parse.py:97-104) plus a native `GCN` backbone
-with the semantics of medium/models.py:14-63 (PyG GCNConv stack) for users without torch_geometric."""
+"""Drop-in for the reference's medium/ours.py (`--method ours`, medium/parse.py:97-104) plus native `GCN` and `GAT` backbones
+with the semantics of medium/models.py:14-63 (PyG GCNConv stack) and :116-155 (PyG GATConv stack) for users without
+torch_geometric."""
 import math
 
 import torch
@@ -13,6 +14,9 @@ from .dist import SINGLE
 from .graph import get_graph
 from .modules import SGFormerBase, TransConvBase, TransConvLayerBase, _Base, full_attention_conv
 
+# GAT / GATConv stay out of __all__: the medium drop-in star-imports this module after the reference's `models`, and a star export
+# would replace the reference's GAT in its parse.py (`--method gat`, `--backbone gat`) without being asked to
+# (`launch --native-backbones` opts in)
 __all__ = ["full_attention_conv", "TransConvLayer", "TransConv", "SGFormer", "GCN", "GCNConv"]
 
 
@@ -143,6 +147,115 @@ def _gcn_flat(gnn, prefix):
     return tuple(names), tensors
 
 
+# PyG GATConv parameter names of other generations -> the 2.0-2.3 names used here (lin_src is lin_dst: one shared Linear)
+_GAT_ALIASES = {"lin_l.weight": ("lin_src.weight", "lin_dst.weight"), "lin_r.weight": ("lin_src.weight", "lin_dst.weight"),
+                "lin.weight": ("lin_src.weight", "lin_dst.weight"), "att_l": ("att_src",), "att_r": ("att_dst",)}
+
+
+class GATConv(nn.Module):
+    """Parameter container with PyG 2.0-2.3 GATConv's names and inits for `in_channels: int`: `lin_src` (= `lin_dst`, one shared
+    bias-free Linear, weight [heads*out, in], glorot), `att_src` / `att_dst` [1, heads, out] (glorot), `bias` [heads*out] with
+    concat else [out] (zeros).  load_state_dict also accepts PyG 1.7.2's `lin_l` / `lin_r` / `att_l` / `att_r` and PyG >= 2.4's
+    `lin`.  It runs inside `GAT` (one schedule for the whole stack); calling a conv on its own is not supported."""
+
+    def __init__(self, in_channels, out_channels, heads=1, concat=True, negative_slope=0.2, dropout=0.0, add_self_loops=True,
+                 edge_dim=None, fill_value='mean', bias=True, **kw):
+        super().__init__()
+        if not isinstance(in_channels, int):
+            raise NotImplementedError("sgformer_b200.GATConv: bipartite (tuple) in_channels are not supported")
+        if edge_dim is not None:
+            raise NotImplementedError("sgformer_b200.GATConv: edge_attr / edge_dim is not supported")
+        if negative_slope != 0.2 or not add_self_loops or not bias:
+            raise NotImplementedError("sgformer_b200.GATConv: only negative_slope=0.2, add_self_loops=True and bias=True are "
+                                      "supported (PyG's defaults, as models.GAT uses them)")
+        self.in_channels, self.out_channels, self.heads, self.concat = in_channels, out_channels, heads, concat
+        self.negative_slope, self.dropout, self.add_self_loops = negative_slope, dropout, add_self_loops
+        self.lin_src = _Lin(in_channels, heads * out_channels)
+        self.lin_dst = self.lin_src
+        self.att_src = nn.Parameter(torch.empty(1, heads, out_channels))
+        self.att_dst = nn.Parameter(torch.empty(1, heads, out_channels))
+        self.bias = nn.Parameter(torch.empty(heads * out_channels if concat else out_channels))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        w = self.lin_src.weight
+        a = math.sqrt(6.0 / (w.size(-2) + w.size(-1)))
+        nn.init.uniform_(w, -a, a)
+        for att in (self.att_src, self.att_dst):
+            a = math.sqrt(6.0 / (att.size(-2) + att.size(-1)))
+            nn.init.uniform_(att, -a, a)
+        nn.init.zeros_(self.bias)
+
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kw):
+        for old, new in _GAT_ALIASES.items():
+            if prefix + old in state_dict:
+                t = state_dict.pop(prefix + old)
+                for nm in new:
+                    state_dict.setdefault(prefix + nm, t)
+        super()._load_from_state_dict(state_dict, prefix, *args, **kw)
+
+    def forward(self, x, edge_index, edge_attr=None, size=None, return_attention_weights=None):
+        if return_attention_weights:
+            raise NotImplementedError("sgformer_b200.GATConv: return_attention_weights is not supported")
+        raise NotImplementedError("sgformer_b200.GATConv runs inside sgformer_b200.medium.GAT (one schedule for the whole stack)")
+
+
+class GAT(_Base):
+    """models.GAT (medium/models.py:116-155): input dropout, GATConv(heads, concat) layers with BatchNorm?/ELU/dropout between them,
+    a last GATConv(out_heads, concat=False)."""
+
+    def __init__(self, in_channels, hidden_channels, out_channels, num_layers=2, dropout=0.5, use_bn=False, heads=2, out_heads=1):
+        super().__init__()
+        self.convs = nn.ModuleList()
+        self.convs.append(GATConv(in_channels, hidden_channels, dropout=dropout, heads=heads, concat=True))
+        self.bns = nn.ModuleList()
+        self.bns.append(nn.BatchNorm1d(hidden_channels * heads))
+        for _ in range(num_layers - 2):
+            self.convs.append(GATConv(hidden_channels * heads, hidden_channels, dropout=dropout, heads=heads, concat=True))
+            self.bns.append(nn.BatchNorm1d(hidden_channels * heads))
+        self.convs.append(GATConv(hidden_channels * heads, out_channels, dropout=dropout, heads=out_heads, concat=False))
+        self.dropout = dropout
+        self.activation = F.elu
+        self.use_bn = use_bn
+
+    def reset_parameters(self):
+        for conv in self.convs:
+            conv.reset_parameters()
+        for bn in self.bns:
+            bn.reset_parameters()
+
+    def _cfg_kw(self):
+        return dict(gcn_num_layers=len(self.convs), gcn_dropout=float(self.dropout), gcn_use_bn=bool(self.use_bn), gnn_kind="gat")
+
+    def forward(self, data):
+        x, edge_index = data.graph['node_feat'], data.graph['edge_index']
+        _check_gat_data(data)
+        if not x.is_cuda:
+            raise RuntimeError("sgformer_b200.GAT needs CUDA tensors (no CPU fallback)")
+        names, tensors = _gat_flat(self, "gnn.")
+        cfg = make_config("medium", x.shape[1], self.convs[0].lin_src.weight.shape[0], self.convs[-1].out_channels, **self._cfg_kw())
+        graph = get_graph(edge_index, x.shape[0], 1)
+        return Fn.GraphBranchFn.apply(x, graph, cfg, E.precision(self.precision), self.training, "gat", "gnn.", names, *tensors)
+
+
+def _check_gat_data(data):
+    for k in ('edge_weight', 'edge_attr'):
+        if data.graph.get(k, None) is not None:
+            raise NotImplementedError(f"sgformer_b200.GAT: {k} is not supported")
+
+
+def _gat_flat(gnn, prefix):
+    """(names, tensors) of a GAT with PyG 2.0-2.3 GATConv naming."""
+    names, tensors = [], []
+    for i, c in enumerate(gnn.convs):
+        for nm, t in (("lin_src.weight", c.lin_src.weight), ("att_src", c.att_src), ("att_dst", c.att_dst), ("bias", c.bias)):
+            names.append(f"{prefix}convs.{i}.{nm}"); tensors.append(t)
+    for i, bn in enumerate(gnn.bns[:len(gnn.convs) - 1]):
+        for nm in ("weight", "bias", "running_mean", "running_var", "num_batches_tracked"):
+            names.append(f"{prefix}bns.{i}.{nm}"); tensors.append(getattr(bn, nm))
+    return tuple(names), tensors
+
+
 class SGFormer(SGFormerBase):
     """medium/ours.py:179-223: attention branch + an injected GNN (`gnn=`)."""
     variant = "medium"
@@ -166,7 +279,7 @@ class SGFormer(SGFormerBase):
         self.params2.extend(list(self.fc.parameters()))
         self._io = (in_channels, hidden_channels, out_channels)
 
-    def _cfg(self, gcn_layers=2, gcn_dropout=0.5, gcn_use_bn=True) -> dict:
+    def _cfg(self, gcn_layers=2, gcn_dropout=0.5, gcn_use_bn=True, gnn_kind="gcn") -> dict:
         d, h, c = self._io
         t = self.trans_conv
         _, _, tnl, tnh = t._dims
@@ -175,7 +288,7 @@ class SGFormer(SGFormerBase):
                            trans_use_weight=t.convs[0].use_weight if tnl else True, trans_use_act=False, alpha=t.alpha,
                            use_graph=bool(self.use_graph), graph_weight=float(self.graph_weight),
                            aggregate=self.aggregate, gcn_num_layers=gcn_layers, gcn_dropout=gcn_dropout,
-                           gcn_use_bn=gcn_use_bn)
+                           gcn_use_bn=gcn_use_bn, gnn_kind=gnn_kind)
 
     def forward(self, data):
         x, edge_index = data.graph['node_feat'], data.graph['edge_index']
@@ -190,6 +303,14 @@ class SGFormer(SGFormerBase):
         tensors = list(tt) + ft
         if not self.use_graph:
             return Fn.SGFormerFn.apply(x, None, self._cfg(), prec, self.training, self._comm, tuple(names), *tensors)
+        if bool(self.use_graph) and isinstance(self.gnn, GAT) and self.gnn.convs[-1].out_channels == self._io[1]:
+            _check_gat_data(data)
+            if self._comm.active:
+                raise NotImplementedError("sgformer_b200: row sharding of the GAT branch is not supported")
+            gn, gt = _gat_flat(self.gnn, "gnn.")
+            cfg = self._cfg(len(self.gnn.convs), float(self.gnn.dropout), bool(self.gnn.use_bn), "gat")
+            graph = get_graph(edge_index, x.shape[0], 1)
+            return Fn.SGFormerFn.apply(x, graph, cfg, prec, self.training, self._comm, tuple(names) + tuple(gn), *tensors, *gt)
         if fused:
             gn, gt = _gcn_flat(self.gnn, "gnn.")
             cfg = self._cfg(len(self.gnn.convs), float(self.gnn.dropout), bool(self.gnn.use_bn))
