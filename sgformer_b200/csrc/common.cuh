@@ -173,6 +173,10 @@ __device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  :: "l"(tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
 }
+// L2 prefetch of `bytes` (a multiple of 16) contiguous bytes from a 16-byte aligned global address: a hint, nothing waits on it
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gsrc, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(gsrc), "r"(bytes) : "memory");
+}
 // cp.async (LDGSTS): 16-byte global -> shared copies that need no destination register; a thread that reads back only what it copied
 // itself needs no barrier, just wait_group.
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {

@@ -80,11 +80,15 @@ constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + MMA_WARPS * 2 * WSTG_BYTES + B
 // Resident-B mode (p.b_res): the whole B operand of one n-block (all k-blocks) stays in shared memory across the row tiles
 // of a CTA, so that only A streams through the ring.  Without it every 128-row tile re-fetches K x n_block of weights from
 // L2, and at short K the few k-blocks of a tile cannot cover that latency.
+// The A-only ring takes whatever shared memory the resident B leaves (p.ring_stages, at least RES_MIN_STAGES): the ring is
+// all the loads a CTA has in flight, and a 256-wide B leaves room for 4 stages, a narrow one (the 47-class head) for 8.
 constexpr int RES_BYTES = (256 + 16) * 256 * 2;   // 136 KB: K = 256 x (256 + 16-column tail)
 constexpr int RES_MAX_KB = 16;                    // one full/empty mbarrier pair per resident k-block
-constexpr int RES_STAGES = 3;                     // A-only ring
-constexpr int SMEM_BYTES_RES = RES_BYTES + RES_STAGES * A_BYTES + MMA_WARPS * WSTG_BYTES + BAR_BYTES + STAT_BYTES + 1024;
-static_assert(SMEM_BYTES <= 232448 && SMEM_BYTES_RES <= 232448, "exceeds the 227 KB of dynamic shared memory per CTA");
+constexpr int RES_MIN_STAGES = 3, RING_MAX = 8;   // A-only ring
+constexpr int SMEM_LIMIT = 232448;                // 227 KB of dynamic shared memory per CTA
+constexpr int RES_FIXED_BYTES = MMA_WARPS * WSTG_BYTES + BAR_BYTES + STAT_BYTES + 1024;
+constexpr int SMEM_BYTES_RES = RES_BYTES + RES_MIN_STAGES * A_BYTES + RES_FIXED_BYTES;
+static_assert(SMEM_BYTES <= SMEM_LIMIT && SMEM_BYTES_RES <= SMEM_LIMIT, "exceeds the 227 KB of dynamic shared memory per CTA");
 
 struct Seg {
     int a_idx, a_koff, b_idx, b_koff, k_blocks;
@@ -94,6 +98,7 @@ struct Params {
     int n_out, bn_main, bn_pad, has_tail, n_blocks;   // bn_pad: bn_main rounded up to the 64-column MMA chunk
     int64_t num_tiles;
     int b_res;          // 1: resident-B schedule (see RES_BYTES)
+    int res_bytes, ring_stages;   // b_res: shared memory of the resident B (all k-blocks), stages of the A-only ring
     int64_t chunk;      // b_res: row tiles per CTA between two reloads of B (only matters when n_blocks > 1)
     int n_seg, total_kb;
     Seg seg[SGF_MAX_SEG];
@@ -212,21 +217,21 @@ template <int F>
 __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_constant__ Tmaps tm, const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    // streaming: [ring: STAGES x (A | B)] [staging];  resident: [B: RES_BYTES] [ring: RES_STAGES x A] [staging]
+    // streaming: [ring: STAGES x (A | B)] [staging];  resident: [B: p.res_bytes] [ring: p.ring_stages x A] [staging]
     const bool res = p.b_res != 0;
     uint8_t* bres = smem;
-    uint8_t* ring = res ? smem + RES_BYTES : smem;
-    const int ring_stages = res ? RES_STAGES : STAGES;
+    uint8_t* ring = res ? smem + p.res_bytes : smem;
+    const int ring_stages = res ? p.ring_stages : STAGES;
     const int ring_stride = res ? A_BYTES : STAGE_BYTES;
     const int stg_per_warp = res ? 1 : 2;                 // warp-private [16 rows x 128 B] staging tiles
     uint8_t* staging = ring + ring_stages * ring_stride;
     uint64_t* full = reinterpret_cast<uint64_t*>(staging + MMA_WARPS * stg_per_warp * WSTG_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* bres_full = empty + STAGES;
+    uint64_t* empty = full + RING_MAX;
+    uint64_t* bres_full = empty + RING_MAX;
     uint64_t* bres_empty = bres_full + RES_MAX_KB;
     float* stat_sm = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + BAR_BYTES);   // [2][STAT_COLS]: sum, sumsq
-    static_assert((2 * STAGES + 2 * RES_MAX_KB) * 8 <= BAR_BYTES, "barrier area");
-    static_assert(RES_STAGES <= STAGES, "ring barriers");
+    static_assert((2 * RING_MAX + 2 * RES_MAX_KB) * 8 <= BAR_BYTES, "barrier area");
+    static_assert(STAGES <= RING_MAX, "ring barriers");
     const bool want_stats = p.col_sum != nullptr || p.col_sumsq != nullptr;
 
     const int warp = threadIdx.x >> 5;
@@ -242,7 +247,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
         }
         if (p.has_tail) tma_prefetch_desc(&tm.tail);
         if (p.tma_store) tma_prefetch_desc(&tm.out);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
+        for (int s = 0; s < ring_stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
         for (int s = 0; s < RES_MAX_KB; ++s) { mbar_init(&bres_full[s], 1); mbar_init(&bres_empty[s], MMA_WARPS); }
         fence_barrier_init();
     }
@@ -322,6 +327,16 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
     int stage = 0; uint32_t phase = 0;
     TileIter ti(p);
     while (ti.next()) {
+        const int m_blk = ti.m_blk, n_blk = ti.n_blk;
+        const int64_t row_w = (int64_t)m_blk * BM + wg * 64 + wq * 16;     // first row of this warp's 16
+        const int col_base = n_blk * p.bn_main;
+        if (!GEN && (f_acc || f_aux) && lane < 16 && row_w + lane < p.rows) {
+            // the epilogue's addend rows go to L2 while the MMAs run (the specialised epilogue's rows are whole, aligned
+            // 64-byte multiples): its loads then wait for L2 rather than for HBM
+            if (f_acc) bulk_prefetch_l2(static_cast<const __nv_bfloat16*>(p.out) + (row_w + lane) * p.ldo + col_base, p.bn_main * 2);
+            if (f_aux) bulk_prefetch_l2(static_cast<const __nv_bfloat16*>(p.aux) + (row_w + lane) * p.ld_aux + col_base, p.bn_main * 2);
+        }
+        int prev = 0;     // the stage of the previous k-block: its MMAs may still run, it is released one k-block later
         for (int kbg = 0; kbg < p.total_kb; ++kbg) {
             if (res && ti.first) mbar_wait(&bres_full[kbg], (uint32_t)(ti.group & 1));
             mbar_wait(&full[stage], phase);
@@ -338,24 +353,31 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
                 if (p.has_tail) wgmma_n16<0, 0>(acct, da, make_smem_desc_sw128(sb + p.bn_pad * BK * 2 + k * 32, 16, 1024), sc);
             }
             wgmma_commit();
-            wgmma_wait<0>();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) fence_regs(acc[j]);
-            fence_regs(acct);
+            // resident-B (a ring of 4-8 A stages): this k-block's MMAs stay in flight and the previous block's stage is released.
+            // Streaming (3 stages of A and B): holding a stage one block longer would leave the producer two, so wait and release.
+            if (res) wgmma_wait<1>();
+            else wgmma_wait<0>();
             __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&empty[stage]);
-                if (res && ti.last) mbar_arrive(&bres_empty[kbg]);
+            if (lane == 0 && (kbg > 0 || !res)) {
+                mbar_arrive(&empty[res ? prev : stage]);
+                if (res && ti.last) mbar_arrive(&bres_empty[kbg - 1]);
             }
+            prev = stage;
             if (++stage == ring_stages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fence_regs(acc[j]);
+        fence_regs(acct);
+        __syncwarp();
+        if (lane == 0 && res) {
+            mbar_arrive(&empty[prev]);
+            if (ti.last) mbar_arrive(&bres_empty[p.total_kb - 1]);
         }
 
         // -------- epilogue --------
-        const int m_blk = ti.m_blk, n_blk = ti.n_blk;
-        const int64_t row_w = (int64_t)m_blk * BM + wg * 64 + wq * 16;     // first row of this warp's 16
         const int64_t rows[2] = {row_w + rr, row_w + rr + 8};
         const bool row_ok[2] = {rows[0] < p.rows, rows[1] < p.rows};
-        const int col_base = n_blk * p.bn_main;
         float rs[2] = {1.f, 1.f}, r1r[2] = {0.f, 0.f}, inv_den[2] = {1.f, 1.f};
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
@@ -490,32 +512,40 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
 // The error of one wgmma accumulator grows with the number of nodes it sums: measured on an H100, sgf_gram over 300 k rows of
 // bf16x3 operands (about 4500 rows per accumulator) missed fp64 by 2.7e-5 relative, beyond the 2e-5 that tests/test_gpu_kernels.py
 // allows (a bias consistent with truncating fp32 accumulation).  Every FLUSH_KB node blocks (1024 rows) a thread adds its
-// accumulators into its own fp32 workspace partial (round-to-nearest, fixed order: deterministic) and restarts them from zero.
+// accumulators into its own fp32 partial (round-to-nearest, fixed order: deterministic) and restarts them from zero; gemm_tn
+// keeps that partial in shared memory, gram in the workspace.
 constexpr int FLUSH_KB = 16;
+// Diagnostic builds (-DSGF_TN_DIAG=n, scripts/bench_gemm_tn.py; never in the shipped library, results are wrong):
+// 1 = no mid-loop flush, 2 = no MMAs (loads only), 3 = no loads (the producer arrives without TMA; MMAs on stale tiles).
+#ifndef SGF_TN_DIAG
+#define SGF_TN_DIAG 0
+#endif
+
+// ws += v as one fire-and-forget L2 reduction.  red.add.f32 rounds to nearest even like the fp32 add it replaces; unlike it,
+// it flushes subnormal operands and results to zero, so a partial below 2^-126 in magnitude can differ from old + acc.  The
+// issuing thread does not wait for it: the flush costs the MMA warps only the issue of the instructions.
+__device__ __forceinline__ void red_add_f32(float* p, float v) {
+    asm volatile("red.global.add.f32 [%0], %1;" :: "l"(p), "f"(v) : "memory");
+}
 // ws[col * mp + row] (+)= acc for the accumulator rows mrow, mrow + 8 and columns 64 j + 8c + cq + e < ncols of the chunks
-// j in [j0, 4); acc is zeroed.  The partials are loaded BATCH at a time before any of them is stored: interleaved, every
-// load would wait for the previous store (the compiler cannot tell the addresses apart), one L2 round trip per element, and the
-// flushes of a 2.45 M-row product would stall the MMA warps for longer than the products themselves take.  BATCH is the
-// largest that does not spill at the 168 registers of the caller (gemm_tn 16, gram 8).
-template <int BATCH>
-__device__ __forceinline__ void flush_acc(float (&acc)[4][32], float* ws, int mp, int mrow, int cq, int j0, int ncols, bool add) {
+// j in [j0, 4); acc is zeroed (gram).  The first flush of a slice stores, every later one adds with red.add: no load of the old
+// partial, so nothing on the MMA warps' path waits for an L2 round trip (loading it 8 elements at a time cost a flush 16 round
+// trips).  Each partial element belongs to one thread, and one thread's operations on an address stay in program order, so
+// the adds happen in flush order.  (gemm_tn keeps its partial in shared memory instead, see tn::PART_CHUNK_BYTES: there the
+// reductions, twice as many per CTA, competed with the TMA loads in L2 and measured slower than loading the partial.)
+__device__ __forceinline__ void flush_acc_red(float (&acc)[4][32], float* ws, int mp, int mrow, int cq, int j0, int ncols, bool add) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         if (j < j0) continue;
 #pragma unroll
-        for (int i0 = 0; i0 < 32; i0 += BATCH) {
-            float old[BATCH];
-#pragma unroll
-            for (int q = 0; q < BATCH; ++q) {
-                const int i = i0 + q, col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
-                old[q] = (add && col < ncols) ? ws[(int64_t)col * mp + mrow + 8 * ((i >> 1) & 1)] : 0.f;
+        for (int i = 0; i < 32; ++i) {
+            const int col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
+            float* w = ws + (int64_t)col * mp + mrow + 8 * ((i >> 1) & 1);
+            if (col < ncols) {
+                if (add) red_add_f32(w, acc[j][i]);
+                else *w = acc[j][i];
             }
-#pragma unroll
-            for (int q = 0; q < BATCH; ++q) {
-                const int i = i0 + q, col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
-                if (col < ncols) ws[(int64_t)col * mp + mrow + 8 * ((i >> 1) & 1)] = add ? old[q] + acc[j][i] : acc[j][i];
-                acc[j][i] = 0.f;
-            }
+            acc[j][i] = 0.f;
         }
     }
 }
@@ -526,13 +556,17 @@ __device__ __forceinline__ void flush_acc(float (&acc)[4][32], float* ws, int mp
 // CTA (x, y): features [128 x, 128 x + 128) of A (one warpgroup per 64) against all n of B, over the y-th slice of the
 // node blocks.  CTAs that share a node slice run side by side, so the second read of B hits L2.
 namespace tn {
-constexpr int BKN = 64, STAGES = 4, MMA_WARPS = 8, THREADS = 32 * (MMA_WARPS + 4);   // + the producer warpgroup
+constexpr int BKN = 64, MAX_STAGES = 8, MMA_WARPS = 8, THREADS = 32 * (MMA_WARPS + 4);   // + the producer warpgroup
 constexpr int CHUNK_BYTES = 64 * BKN * 2;   // one [64 feat x 64 node] box = 8 KB
-constexpr int A_BYTES = 2 * CHUNK_BYTES;    // the CTA's 128 features of A
-constexpr int B_BYTES = 4 * CHUNK_BYTES;    // up to 256 features of B
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // 48 KB
+constexpr int A_BYTES = 2 * CHUNK_BYTES;    // the CTA's 128 features of A; a stage is A_BYTES + n_chunks boxes of B
+// The running flush partial of a CTA stays in shared memory, [n_chunks][32][256 MMA threads] fp32 (thread-private, conflict-free):
+// a flush is then an add in shared memory (the same fp32 round-to-nearest old + acc as before) and only the last one of a slice
+// writes the workspace.  Reading the partial back from L2 cost every flush several dependent round trips, during which the
+// producer could run only a ring ahead and then starved the loads (products step, 256 x 256: 1.63 ms with mid-loop flushes,
+// 0.98 ms without).  The ring takes the shared memory the partial leaves (2 stages at n = 256, more for narrower B).
+constexpr int PART_CHUNK_BYTES = 32 * 32 * MMA_WARPS * 4;   // 32 KB per 64 columns of B
 constexpr int BAR_BYTES = 256;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;
+constexpr int SMEM_LIMIT = 232448;          // 227 KB of dynamic shared memory per CTA
 
 struct Params {
     int64_t rows;
@@ -540,6 +574,7 @@ struct Params {
     int64_t kb_total;
     float* ws;  // [gridDim.y][un][mp]
     int n_pairs;                                  // partial products accumulated per node block (1, or the 6 of bf16x3)
+    int stages, stage_bytes;                      // ring depth and stride (A_BYTES + n_chunks boxes)
     int a_off[SGF_TN_MAX_PAIRS], b_off[SGF_TN_MAX_PAIRS];   // column offset (elements) of the plane each product reads
 };
 struct Tmaps {
@@ -549,8 +584,11 @@ struct Tmaps {
 __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_constant__ Tmaps tm, const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
+    // [ring: stages x (A | B)] [flush partial: n_chunks x PART_CHUNK_BYTES] [barriers]
+    uint8_t* part_base = smem + p.stages * p.stage_bytes;
+    uint64_t* full = reinterpret_cast<uint64_t*>(part_base + p.n_chunks * PART_CHUNK_BYTES);
+    uint64_t* empty = full + MAX_STAGES;
+    static_assert(2 * MAX_STAGES * 8 <= BAR_BYTES, "barrier area");
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -564,7 +602,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tm.a);
         tma_prefetch_desc(&tm.b);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], MMA_WARPS); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -578,14 +616,19 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
             for (int64_t kb = kb0; kb < kb1; ++kb) {
                 for (int pr = 0; pr < p.n_pairs; ++pr) {
                     mbar_wait(&empty[stage], phase ^ 1);
-                    uint8_t* sa = smem + stage * STAGE_BYTES;
+                    uint8_t* sa = smem + stage * p.stage_bytes;
                     uint8_t* sb = sa + A_BYTES;
+#if SGF_TN_DIAG == 3
+                    mbar_arrive(&full[stage]);
+                    (void)sb; (void)stage_tx;
+#else
                     mbar_arrive_expect_tx(&full[stage], stage_tx);
                     for (int c = 0; c < a_chunks; ++c)
                         tma_load_2d(sa + c * CHUNK_BYTES, &tm.a, &full[stage], p.a_off[pr] + m0 + c * 64, (int32_t)(kb * BKN));
                     for (int c = 0; c < p.n_chunks; ++c)
                         tma_load_2d(sb + c * CHUNK_BYTES, &tm.b, &full[stage], p.b_off[pr] + c * 64, (int32_t)(kb * BKN));
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+#endif
+                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
                 }
             }
         }
@@ -604,14 +647,15 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
     float* ws = p.ws + (int64_t)blockIdx.y * p.un * p.mp;
     const int mrow = m0 + wg * 64 + wq * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3);
+    float* part = reinterpret_cast<float*>(part_base) + threadIdx.x;     // element (j, i) at part[(32 j + i) * 256]
     bool flushed = false;
     int stage = 0; uint32_t phase = 0;
     for (int64_t kb = kb0; kb < kb1; ++kb) {
         for (int pr = 0; pr < p.n_pairs; ++pr) {
             mbar_wait(&full[stage], phase);
-            if (active) {
-                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * CHUNK_BYTES;
-                const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
+            if (active && SGF_TN_DIAG != 2) {
+                const uint32_t sa = smem_u32(smem + stage * p.stage_bytes) + wg * CHUNK_BYTES;
+                const uint32_t sb = smem_u32(smem + stage * p.stage_bytes) + A_BYTES;
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < BKN / 16; ++k) {
@@ -628,14 +672,33 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tn_kernel(const __grid_consta
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[stage]);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
         }
-        if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1) {
-            flush_acc<16>(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
+        if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1 && SGF_TN_DIAG != 1) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (j >= p.n_chunks) continue;
+#pragma unroll
+                for (int i = 0; i < 32; ++i) {
+                    float& q = part[(32 * j + i) * (32 * MMA_WARPS)];
+                    q = flushed ? q + acc[j][i] : acc[j][i];
+                    acc[j][i] = 0.f;
+                }
+            }
             flushed = true;
         }
     }
-    flush_acc<16>(acc, ws, p.mp, mrow, cq, 0, p.un, flushed);
+    // the last flush: ws[col * mp + row] = partial + acc (acc alone if the slice never flushed)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const int col = 64 * j + 8 * (i >> 2) + cq + (i & 1);
+            if (col < p.un) {
+                const float v = acc[j][i];
+                ws[(int64_t)col * p.mp + mrow + 8 * ((i >> 1) & 1)] = flushed ? part[(32 * j + i) * (32 * MMA_WARPS)] + v : v;
+            }
+        }
 }
 
 // out[i,j] = alpha * sum_cta ws[cta][j][i] (+ beta*out[i,j]);  i < m, j < n
@@ -716,10 +779,15 @@ __global__ void __launch_bounds__(THREADS, 1) gram_kernel(const __grid_constant_
             for (int64_t kb = kb0; kb < kb1; ++kb) {
                 mbar_wait(&empty[stage], phase ^ 1);
                 uint8_t* sa = smem + stage * stage_stride;
+#if SGF_TN_DIAG == 3
+                mbar_arrive(&full[stage]);
+                (void)sa;
+#else
                 mbar_arrive_expect_tx(&full[stage], (uint32_t)(p.n_planes * plane_bytes));
                 for (int pl = 0; pl < p.n_planes; ++pl)
                     for (int c = 0; c < nld; ++c)
                         tma_load_2d(sa + pl * plane_bytes + c * CHUNK_BYTES, &tm, &full[stage], p.plane_off[pl] + (c0 + c) * 64, (int32_t)(kb * BKN));
+#endif
                 if (++stage == p.stages) { stage = 0; phase ^= 1; }
             }
         }
@@ -744,11 +812,11 @@ __global__ void __launch_bounds__(THREADS, 1) gram_kernel(const __grid_constant_
     bool flushed = false;
     // G partial of the chunks j >= ic, then column 0 of the ones product (X^T 1) as workspace column un
     auto flush = [&]() {
-        flush_acc<8>(acc, ws, p.mp, mrow, cq, ic, p.un, flushed);
+        flush_acc_red(acc, ws, p.mp, mrow, cq, ic, p.un, flushed);
         if (cq == 0) {
             float* w = ws + (int64_t)p.un * p.mp + mrow;
-            w[0] = flushed ? w[0] + accs[0] : accs[0];
-            w[8] = flushed ? w[8] + accs[2] : accs[2];
+            if (flushed) { red_add_f32(w, accs[0]); red_add_f32(w + 8, accs[2]); }
+            else { w[0] = accs[0]; w[8] = accs[2]; }
         }
 #pragma unroll
         for (int i = 0; i < 8; ++i) accs[i] = 0.f;
@@ -757,7 +825,7 @@ __global__ void __launch_bounds__(THREADS, 1) gram_kernel(const __grid_constant_
     int stage = 0; uint32_t phase = 0;
     for (int64_t kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
-        if (active) {
+        if (active && SGF_TN_DIAG != 2) {
             const uint32_t sa = smem_u32(smem + stage * stage_stride);
             wgmma_fence();
             for (int pr = 0; pr < p.n_pairs; ++pr) {
@@ -788,7 +856,7 @@ __global__ void __launch_bounds__(THREADS, 1) gram_kernel(const __grid_constant_
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[stage]);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1) flush();
+        if (active && (kb - kb0 + 1) % FLUSH_KB == 0 && kb + 1 < kb1 && SGF_TN_DIAG != 1) flush();
     }
     if (active) flush();
 }
@@ -920,11 +988,16 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
         // several n-blocks: B is re-loaded per (chunk, n-block); a chunk of 4 row tiles per CTA keeps the A tiles that are
         // re-read for the following n-blocks inside the 50 MB L2 (132 CTAs x 4 x 128 rows x K x 2 B = 35 MB at K = 256)
         p.chunk = p.n_blocks == 1 ? (int64_t)1 << 40 : 4;
+        // the A ring of the resident schedule takes the shared memory B leaves
+        p.res_bytes = (int)(b_tx * p.total_kb);
+        const int st = (nt::SMEM_LIMIT - p.res_bytes - nt::RES_FIXED_BYTES) / nt::A_BYTES;
+        p.ring_stages = st < nt::RING_MAX ? st : nt::RING_MAX;
+        if (p.b_res && p.ring_stages < nt::RES_MIN_STAGES) return SGF_ERR_UNSUPPORTED;
     }
     // resident-B: one CTA per SM over ROW tiles (every CTA visits all n-blocks of its rows)
     const int64_t work = p.b_res ? m_blocks : p.num_tiles;
     const int64_t grid = work < num_sms() ? work : num_sms();
-    const int smem_bytes = p.b_res ? nt::SMEM_BYTES_RES : nt::SMEM_BYTES;
+    const int smem_bytes = p.b_res ? p.res_bytes + p.ring_stages * nt::A_BYTES + nt::RES_FIXED_BYTES : nt::SMEM_BYTES;
 
     // epilogue specialisation: the exact feature set of this call if it has a compiled instantiation, else the generic kernel
     int feat = (a->bias ? nt::F_BIAS : 0) | (a->aux ? nt::F_AUX : 0) | (a->relu ? nt::F_RELU : 0) |
@@ -937,7 +1010,7 @@ extern "C" int sgf_gemm_nt(const sgf_gemm_nt_args* a, void* stream) {
                          p.n_blocks * p.bn_main == a->n_out;     // every 32-column piece of every n-block is complete
     static const bool no_special = [] { const char* e = getenv("SGF_GEMM_NT_GENERIC"); return e && e[0] == '1'; }();
     if (!fast_ok || no_special) feat = nt::F_GENERIC;
-    const int smem_max = nt::SMEM_BYTES > nt::SMEM_BYTES_RES ? nt::SMEM_BYTES : nt::SMEM_BYTES_RES;
+    const int smem_max = nt::SMEM_LIMIT;
 #define SGF_NT_CASE(FEAT)                                                                                                   \
     case (FEAT): {                                                                                                         \
         static bool attr_set = false;                                                                                      \
@@ -1025,11 +1098,17 @@ extern "C" int sgf_gemm_tn(const sgf_gemm_tn_args* a, void* stream) {
         if ((rc = make_tmap_bf16(&tm.b, a->b, a->rows, b_span, a->ldb, tn::BKN))) return rc;
         static bool attr_set = false;
         if (!attr_set) {
-            SGF_CUDA_TRY(cudaFuncSetAttribute(tn::gemm_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tn::SMEM_BYTES));
+            SGF_CUDA_TRY(cudaFuncSetAttribute(tn::gemm_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tn::SMEM_LIMIT));
             attr_set = true;
         }
+        // the ring takes what the flush partial leaves
+        p.stage_bytes = tn::A_BYTES + p.n_chunks * tn::CHUNK_BYTES;
+        const int fixed = p.n_chunks * tn::PART_CHUNK_BYTES + tn::BAR_BYTES + 1024;
+        const int stages = (tn::SMEM_LIMIT - fixed) / p.stage_bytes;
+        p.stages = stages < tn::MAX_STAGES ? stages : tn::MAX_STAGES;
+        if (p.stages < 2) return SGF_ERR_UNSUPPORTED;
         grid = tn_splits(p.kb_total, m_blocks);
-        tn::gemm_tn_kernel<<<dim3(m_blocks, grid), tn::THREADS, tn::SMEM_BYTES, st>>>(tm, p);
+        tn::gemm_tn_kernel<<<dim3(m_blocks, grid), tn::THREADS, p.stages * p.stage_bytes + fixed, st>>>(tm, p);
         SGF_LAUNCH_CHECK(); count_launch();
     }
     int64_t total = (int64_t)a->n * mp;
