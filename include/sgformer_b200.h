@@ -106,6 +106,29 @@ int sgf_add_self_loops(const int64_t* edge_index, int64_t nnz, int64_t n, int64_
  * the two multisets; equal sums <=> symmetric (2^-64 collision odds).  One pass over edge_index.  Decides whether the backward
  * SpMM (A^T, autograd of torch_sparse.matmul, large/ours.py:33) can reuse the forward CSR. */
 int sgf_edge_symmetry(const int64_t* edge_index, int64_t nnz, int64_t n, uint64_t* out2, void* stream);
+/* Weighted graphs (edge_weight of the medium GCN / DIFFormer, DESIGN.md §4.10).  The CSR of sgf_csr_build (n x n, by_source,
+ * self_loop_mode as there) plus, per entry j: eid[j] (int64) = position of the source edge in edge_index, val[j] = weight[eid[j]]
+ * (fp32).  Rows are sorted by (col, eid).  self_loop_mode 1 (PyG gcn_norm(add_self_loops=True)): existing self loops are
+ * dropped and node i's added loop takes the weight of i's LAST self loop in edge order (eid = its position), or 1 when i has none
+ * (eid = -1).  dinv (nullable): mode 1 -> deg[i]^-1/2 with deg[i] = sum of row i's values (summed in fp64 in CSR order, inf -> 0,
+ * negative -> NaN); mode 0 -> the count-based dinv of sgf_csr_build (DIFFormer's gcn_conv normalises by the unweighted degree).
+ * col / eid / val hold nnz (+ n in mode 1) entries.  nnz < 2^32 - 1.  ws sized by sgf_csr_build_weighted_ws_bytes(nnz, n). */
+int sgf_csr_build_weighted_ws_bytes(int64_t nnz, int64_t n, size_t* bytes /* host out */);
+int sgf_csr_build_weighted(const int64_t* edge_index, const float* weight /* [nnz] */, int64_t nnz, int64_t n, int by_source,
+                           int self_loop_mode, int64_t* rowptr, int32_t* col, int64_t* eid, float* val, float* dinv /* or NULL */,
+                           void* ws, size_t ws_bytes, void* stream);
+/* sgf_edge_symmetry over the weighted multisets {(r, c, w)} and {(c, r, w)} (the weight's bit pattern is hashed along): equal
+ * sums <=> the transposed weighted CSR equals the forward one and can share its storage. */
+int sgf_edge_symmetry_weighted(const int64_t* edge_index, const float* weight, int64_t nnz, int64_t n, uint64_t* out2, void* stream);
+/* Gradient of a weighted layer y = Â t (Â[c,r] = dinv[c] val[j] dinv[r], CSR of sgf_csr_build_weighted by_source = 0) w.r.t. the
+ * edge weights, ADDED into out[nnz] (fp32, one entry per edge of edge_index):  out[eid[j]] += <a_c, b_r> + q_c  for entry
+ * j = (c, r), where a = dinv (.) dL/dy and b = dinv (.) t are [n_rows, h] activations (dtype 0 fp32 / 1 bf16, h <= 512), and
+ * q_c = -1/2 dinv[c] (<a_c, y_c> + <b_c, u_c>) with u = Â^T dL/dy when y is non-NULL (the degree term of self_loop_mode 1; NULL
+ * for DIFFormer's unweighted normalisation).  loop_grad (fp32 [n_rows], nullable): self_loop_mode 1 - the added self loop's
+ * gradient is added to EVERY self-loop edge (i, i) of edge_index instead.  No atomics: deterministic. */
+int sgf_edge_weight_grad(const int64_t* rowptr, const int32_t* col, const int64_t* eid, int64_t n_rows, int h, int dtype,
+                         const void* a, int64_t lda, const void* b, int64_t ldb, const void* y, int64_t ldy, const void* u, int64_t ldu,
+                         const float* dinv, const int64_t* edge_index, int64_t nnz, float* loop_grad, float* out, void* stream);
 /* K9 on the CSR: the induced subgraph of `subset` emitted directly as the subset's own CSR (rows = subset order, columns
  * = positions in subset, sorted; dinv from the induced in-degrees) — the structure GraphConv needs for a mini-batch, in
  * O(sum of the subset rows' lengths) instead of PyG subgraph's O(E) mask per batch + a CSR rebuild.
@@ -136,6 +159,13 @@ int sgf_spmm(const int64_t* rowptr, const int32_t* col, const float* row_scale, 
 int sgf_spmm_heavy(const int32_t* col, const float* row_scale, const void* x, int64_t ldx, void* y, int64_t ldy, int h,
                    int dtype, const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg, float* partial,
                    const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, void* stream);
+/* Weighted SpMM (CSR of sgf_csr_build_weighted):  y[r,:] = row_scale[r] * sum_{j in row r} val[j] * x[col[j], :]  (fp32
+ * accumulation), and its hub-row segment path; otherwise as sgf_spmm / sgf_spmm_heavy. */
+int sgf_spmm_weighted(const int64_t* rowptr, const int32_t* col, const float* val, const float* row_scale, const void* x, int64_t ldx,
+                      void* y, int64_t ldy, int64_t n_rows, int h, int dtype, int64_t max_row_len, void* stream);
+int sgf_spmm_heavy_weighted(const int32_t* col, const float* val, const float* row_scale, const void* x, int64_t ldx, void* y,
+                            int64_t ldy, int h, int dtype, const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg,
+                            float* partial, const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K12 — GAT edge softmax (replaces PyG GATConv's message passing as medium/models.py:116-155 uses it: per-edge logits, softmax

@@ -158,6 +158,14 @@ _SIGS = {
     "sgf_gat_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int,
                               C.c_int, _f32, _u64, _vp, _vp, _vp, _vp, _i64, _vp]),
     "sgf_dense_dropout": (C.c_int, [_vp, _i64, _i64, _i64, _f32, _u64, _vp, _i64, _vp]),
+    "sgf_csr_build_weighted_ws_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
+    "sgf_csr_build_weighted": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "sgf_edge_symmetry_weighted": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
+    "sgf_spmm_weighted": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, C.c_int, C.c_int, _i64, _vp]),
+    "sgf_spmm_heavy_weighted": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, C.c_int, C.c_int, _vp, _vp, _i64, _vp, _vp, _vp,
+                                          _i64, _vp]),
+    "sgf_edge_weight_grad": (C.c_int, [_vp, _vp, _vp, _i64, C.c_int, C.c_int, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp,
+                                       _vp, _i64, _vp, _vp, _vp]),
     "sgf_attn_prepare_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _i64, _vp, _i64, _vp, _i64, _i64,
                                        _i64, _vp, _vp, _vp, _vp]),
 }

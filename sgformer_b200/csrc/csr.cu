@@ -12,6 +12,10 @@
 //             in global memory above) so the arrays are deterministic and bit-exact with the reference's
 //             (target, source)-sorted storage
 //   dinv    : dinv[i] = sqrt(1/len_i) (0 for empty rows)
+//
+// Weighted build (sgf_csr_build_weighted, edge_weight of the medium GCN / DIFFormer, DESIGN.md §4.10): the fill writes 64-bit keys
+// (col << 32 | eid + 1) instead of column ids, so the same sort tiers order every row by (col, eid) and carry the source edge's
+// position along; an unpack pass then splits the keys into col / eid and gathers val[j] = w[eid[j]].
 #include <cstdlib>
 
 #include "common.cuh"
@@ -190,13 +194,23 @@ __global__ void csr_add_loops_kernel(int64_t n, int64_t row_begin, const int64_t
 // ---- per-row sort ---------------------------------------------------------------------------------
 constexpr int kSortSmemMax = 2048;
 
-__device__ __forceinline__ void bitonic_block(int32_t* a, int npow2, int tid, int nthreads) {
+// Sort keys: int32 column ids, or the int64 (col << 32 | eid + 1) keys of the weighted build.  key_pad sorts after every key.
+template <typename T> __device__ __forceinline__ T key_pad();
+template <> __device__ __forceinline__ int32_t key_pad<int32_t>() { return INT32_MAX; }
+template <> __device__ __forceinline__ int64_t key_pad<int64_t>() { return INT64_MAX; }
+__device__ __forceinline__ int32_t key_min(int32_t a, int32_t b) { return min(a, b); }
+__device__ __forceinline__ int32_t key_max(int32_t a, int32_t b) { return max(a, b); }
+__device__ __forceinline__ int64_t key_min(int64_t a, int64_t b) { return a < b ? a : b; }
+__device__ __forceinline__ int64_t key_max(int64_t a, int64_t b) { return a < b ? b : a; }
+
+template <typename T>
+__device__ __forceinline__ void bitonic_block(T* a, int npow2, int tid, int nthreads) {
     for (int k = 2; k <= npow2; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
             for (int i = tid; i < npow2; i += nthreads) {
                 int ixj = i ^ j;
                 if (ixj > i) {
-                    int32_t x = a[i], y = a[ixj];
+                    T x = a[i], y = a[ixj];
                     bool up = (i & k) == 0;
                     if ((x > y) == up) { a[i] = y; a[ixj] = x; }
                 }
@@ -211,37 +225,38 @@ __device__ __forceinline__ void bitonic_block(int32_t* a, int npow2, int tid, in
 constexpr int kWarpSortMax = 256;
 // bitonic network over 32 * NREG entries held NREG per lane (entry i = lane + 32 * reg): compare-exchange partners at distance
 // j < 32 by shfl.xor, at distance 32 inside the lane.  ~8 instructions per stage and register instead of the ~9 per ENTRY of a rank sort.
-template <int NREG>
-__device__ __forceinline__ void warp_bitonic(int32_t (&v)[NREG], int lane) {
+template <int NREG, typename T>
+__device__ __forceinline__ void warp_bitonic(T (&v)[NREG], int lane) {
 #pragma unroll
     for (int k = 2; k <= 32 * NREG; k <<= 1) {
 #pragma unroll
         for (int j = k >> 1; j > 0; j >>= 1) {
             if (j == 32) {                      // NREG == 2, k == 64: ascending everywhere
-                const int32_t lo = min(v[0], v[NREG - 1]), hi = max(v[0], v[NREG - 1]);
+                const T lo = key_min(v[0], v[NREG - 1]), hi = key_max(v[0], v[NREG - 1]);
                 v[0] = lo; v[NREG - 1] = hi;
             } else {
                 const bool lower = (lane & j) == 0;
 #pragma unroll
                 for (int r = 0; r < NREG; ++r) {
-                    const int32_t o = __shfl_xor_sync(0xffffffffu, v[r], j);
+                    const T o = __shfl_xor_sync(0xffffffffu, v[r], j);
                     const bool up = ((lane + 32 * r) & k) == 0;
-                    v[r] = (lower == up) ? min(v[r], o) : max(v[r], o);
+                    v[r] = (lower == up) ? key_min(v[r], o) : key_max(v[r], o);
                 }
             }
         }
     }
 }
 
-__device__ __forceinline__ void warp_sort_row(int32_t* __restrict__ col, int64_t s, int len, int32_t* sm, int lane) {
+template <typename T>
+__device__ __forceinline__ void warp_sort_row(T* __restrict__ col, int64_t s, int len, T* sm, int lane) {
     if (len <= 32) {
-        int32_t v[1] = {lane < len ? col[s + lane] : INT32_MAX};      // padding sorts to the end (column ids are < INT32_MAX)
+        T v[1] = {lane < len ? col[s + lane] : key_pad<T>()};      // padding sorts to the end (column ids are < INT32_MAX)
         warp_bitonic<1>(v, lane);
         if (lane < len) col[s + lane] = v[0];
         return;
     }
     if (len <= 64) {
-        int32_t v[2] = {col[s + lane], lane + 32 < len ? col[s + lane + 32] : INT32_MAX};
+        T v[2] = {col[s + lane], lane + 32 < len ? col[s + lane + 32] : key_pad<T>()};
         warp_bitonic<2>(v, lane);
         col[s + lane] = v[0];
         if (lane + 32 < len) col[s + lane + 32] = v[1];
@@ -249,14 +264,14 @@ __device__ __forceinline__ void warp_sort_row(int32_t* __restrict__ col, int64_t
     }
     int p2 = 128;
     while (p2 < len) p2 <<= 1;
-    for (int i = lane; i < p2; i += 32) sm[i] = i < len ? col[s + i] : INT32_MAX;
+    for (int i = lane; i < p2; i += 32) sm[i] = i < len ? col[s + i] : key_pad<T>();
     __syncwarp();
     for (int k = 2; k <= p2; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
             for (int i = lane; i < p2; i += 32) {
                 int ixj = i ^ j;
                 if (ixj > i) {
-                    int32_t x = sm[i], y = sm[ixj];
+                    T x = sm[i], y = sm[ixj];
                     bool up = (i & k) == 0;
                     if ((x > y) == up) { sm[i] = y; sm[ixj] = x; }
                 }
@@ -269,12 +284,13 @@ __device__ __forceinline__ void warp_sort_row(int32_t* __restrict__ col, int64_t
 }
 
 // one warp per row; rows longer than kWarpSortMax are queued for the block kernels
+template <typename T>
 __global__ void __launch_bounds__(256) csr_sort_rows_warp_kernel(const int64_t* __restrict__ rowptr, int64_t n,
-                                                                  int32_t* __restrict__ col, int64_t* __restrict__ long_rows,
+                                                                  T* __restrict__ col, int64_t* __restrict__ long_rows,
                                                                   int* __restrict__ n_long) {
-    __shared__ int32_t sm_all[8][kWarpSortMax];
+    __shared__ T sm_all[8][kWarpSortMax];
     const int lane = threadIdx.x & 31;
-    int32_t* sm = sm_all[threadIdx.x >> 5];
+    T* sm = sm_all[threadIdx.x >> 5];
     int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = warp; r < n; r += nwarps) {
@@ -290,11 +306,12 @@ __global__ void __launch_bounds__(256) csr_sort_rows_warp_kernel(const int64_t* 
 }
 
 // one block per queued long row whose padded length p2 satisfies min_p2 < p2 <= max_p2
-__global__ void csr_sort_rows_block_kernel(const int64_t* __restrict__ rowptr, int32_t* __restrict__ col,
+template <typename T>
+__global__ void csr_sort_rows_block_kernel(const int64_t* __restrict__ rowptr, T* __restrict__ col,
                                            const int64_t* __restrict__ long_rows, const int* __restrict__ n_long,
-                                           int32_t* __restrict__ scratch, int64_t scratch_per_block, int64_t min_p2,
+                                           T* __restrict__ scratch, int64_t scratch_per_block, int64_t min_p2,
                                            int64_t max_p2) {
-    __shared__ int32_t sm[kSortSmemMax];
+    __shared__ T sm[kSortSmemMax];
     const int tid = threadIdx.x, nt = blockDim.x;
     const int nq = *n_long;
     for (int q = blockIdx.x; q < nq; q += gridDim.x) {
@@ -305,22 +322,22 @@ __global__ void csr_sort_rows_block_kernel(const int64_t* __restrict__ rowptr, i
         while (p2 < len) p2 <<= 1;
         if (p2 <= min_p2 || p2 > max_p2) continue;  // block-uniform
         if (p2 <= kSortSmemMax) {
-            for (int i = tid; i < p2; i += nt) sm[i] = i < len ? col[s + i] : INT32_MAX;
+            for (int i = tid; i < p2; i += nt) sm[i] = i < len ? col[s + i] : key_pad<T>();
             __syncthreads();
             bitonic_block(sm, (int)p2, tid, nt);
             for (int i = tid; i < len; i += nt) col[s + i] = sm[i];
             __syncthreads();
         } else {
             // hub rows: bitonic network in global scratch (padded to a power of two)
-            int32_t* g = scratch + (int64_t)blockIdx.x * scratch_per_block;
-            for (int64_t i = tid; i < p2; i += nt) g[i] = i < len ? col[s + i] : INT32_MAX;
+            T* g = scratch + (int64_t)blockIdx.x * scratch_per_block;
+            for (int64_t i = tid; i < p2; i += nt) g[i] = i < len ? col[s + i] : key_pad<T>();
             __syncthreads();
             for (int64_t k = 2; k <= p2; k <<= 1) {
                 for (int64_t j = k >> 1; j > 0; j >>= 1) {
                     for (int64_t i = tid; i < p2; i += nt) {
                         int64_t ixj = i ^ j;
                         if (ixj > i) {
-                            int32_t x = g[i], y = g[ixj];
+                            T x = g[i], y = g[ixj];
                             bool up = (i & k) == 0;
                             if ((x > y) == up) { g[i] = y; g[ixj] = x; }
                         }
@@ -340,6 +357,71 @@ __global__ void csr_dinv_kernel(const int64_t* __restrict__ rowptr, int64_t n, f
         float d = (float)(rowptr[i + 1] - rowptr[i]);
         // same operation order as the reference: (1/d).sqrt(), inf -> 0   (large/ours.py:29-32)
         dinv[i] = d > 0.f ? sqrtf(1.0f / d) : 0.0f;
+    }
+}
+
+// ---- weighted build ----------------------------------------------------------------------------------
+// last[i] = position of node i's last self loop in edge order (-1: none); an atomicMax, so the result does not depend on the
+// order in which the threads run (PyG's GPU scatter leaves that choice undefined).
+__global__ void csr_last_loop_kernel(const int64_t* __restrict__ src, const int64_t* __restrict__ dst, int64_t nnz, int64_t n,
+                                     long long* __restrict__ last) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
+        const int64_t r = src[e];
+        if (r == dst[e] && r >= 0 && r < n) atomicMax(&last[r], (long long)e);
+    }
+}
+
+// csr_fill_kernel writing the 64-bit key (col << 32 | e + 1) of edge e
+__global__ void csr_fill_keyed_kernel(const int64_t* __restrict__ key, const int64_t* __restrict__ val, int64_t nnz,
+                                      int64_t row_begin, int64_t row_end, int64_t n_cols, int drop_self_loops,
+                                      const int64_t* __restrict__ rowptr, int* __restrict__ cursor, int64_t* __restrict__ keys) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
+        int64_t k = key[e];
+        if (k < row_begin || k >= row_end) continue;
+        int64_t v = val[e];
+        if (v < 0 || v >= n_cols) continue;
+        if (drop_self_loops && k == v) continue;
+        int pos = atomicAdd(&cursor[k], 1);
+        keys[rowptr[k] + pos] = (v << 32) | (e + 1);
+    }
+}
+
+// the added self loop of node i takes the weight of i's last existing self loop (eid = last[i], -1 -> weight 1)
+__global__ void csr_add_loops_keyed_kernel(int64_t n, const long long* __restrict__ last, const int64_t* __restrict__ rowptr,
+                                           int* __restrict__ cursor, int64_t* __restrict__ keys) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        int pos = atomicAdd(&cursor[i], 1);
+        keys[rowptr[i] + pos] = (i << 32) | (int64_t)(last[i] + 1);
+    }
+}
+
+__global__ void csr_unpack_weighted_kernel(const int64_t* __restrict__ keys, const int64_t* __restrict__ rowptr, int64_t n,
+                                           const float* __restrict__ w, int32_t* __restrict__ col, int64_t* __restrict__ eid,
+                                           float* __restrict__ val) {
+    const int64_t total = rowptr[n];
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < total; j += stride) {
+        const int64_t k = keys[j];
+        const int64_t e = (k & 0xffffffffLL) - 1;
+        col[j] = (int32_t)(k >> 32);
+        eid[j] = e;
+        val[j] = e >= 0 ? w[e] : 1.0f;
+    }
+}
+
+// weighted gcn_norm: deg[i] = sum of row i's values in CSR order (fp64, fixed order: bit-identical run to run),
+// dinv = deg^-1/2 with inf -> 0 (a negative degree gives NaN, as PyG's pow does)
+__global__ void csr_weighted_dinv_kernel(const int64_t* __restrict__ rowptr, const float* __restrict__ val, int64_t n,
+                                         float* __restrict__ dinv) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        double d = 0.0;
+        for (int64_t j = rowptr[i]; j < rowptr[i + 1]; ++j) d += (double)val[j];
+        const float df = (float)d;
+        dinv[i] = df == 0.f ? 0.f : (float)(1.0 / sqrt((double)df));
     }
 }
 
@@ -544,6 +626,35 @@ __global__ void __launch_bounds__(256) edge_symmetry_kernel(const int64_t* __res
     }
 }
 
+// as edge_symmetry_kernel over {(r, c, w)} and {(c, r, w)}: the weight's bit pattern is mixed into every term, so a symmetric
+// pattern whose weights are not symmetric hashes differently
+__global__ void __launch_bounds__(256) edge_symmetry_weighted_kernel(const int64_t* __restrict__ src, const int64_t* __restrict__ dst,
+                                                                     const float* __restrict__ w, int64_t nnz, uint64_t n,
+                                                                     unsigned long long* __restrict__ out) {
+    uint64_t h1 = 0, h2 = 0;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
+        const uint64_t r = (uint64_t)src[e], c = (uint64_t)dst[e];
+        const uint64_t wb = mix64((uint64_t)__float_as_uint(w[e]) + 0x632BE59BD9B4E019ULL);
+        h1 += mix64(mix64(r * n + c) ^ wb);
+        h2 += mix64(mix64(c * n + r) ^ wb);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        h1 += __shfl_xor_sync(0xffffffffu, h1, o);
+        h2 += __shfl_xor_sync(0xffffffffu, h2, o);
+    }
+    __shared__ uint64_t sm[2][8];
+    const int lane = threadIdx.x & 31, wi = threadIdx.x >> 5;
+    if (lane == 0) { sm[0][wi] = h1; sm[1][wi] = h2; }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+        uint64_t t = 0;
+        for (int i = 0; i < 8; ++i) t += sm[threadIdx.x][i];
+        atomicAdd(&out[threadIdx.x], (unsigned long long)t);
+    }
+}
+
 static inline int grid_for(int64_t work, int block, int per_sm = 8) {
     int64_t g = (work + block - 1) / block;
     int64_t cap = (int64_t)num_sms() * per_sm;
@@ -563,6 +674,24 @@ static inline int64_t fill_window_bytes() {
         return (int64_t)(e ? std::atoi(e) : 128) << 20;
     }();
     return v;
+}
+
+// Row windows [lo, hi) of the fill, each written by one launch (sizes: fill_window_bytes of entry_bytes-sized entries)
+template <typename Launch>
+static int for_fill_windows(int64_t nnz, int64_t row_begin, int64_t row_end, int64_t entry_bytes, Launch launch) {
+    const int64_t n = row_end - row_begin;
+    const int64_t win_bytes = fill_window_bytes();
+    int64_t nwin = win_bytes > 0 ? ((nnz + n) * entry_bytes + win_bytes - 1) / win_bytes : 1;
+    if (nwin > kMaxFillWindows) nwin = kMaxFillWindows;
+    if (nwin < 1 || n == 0) nwin = 1;
+    const int64_t rows_per = (n + nwin - 1) / nwin;
+    for (int64_t wi = 0; wi < nwin; ++wi) {
+        const int64_t lo = row_begin + wi * rows_per, hi = lo + rows_per < row_end ? lo + rows_per : row_end;
+        if (nwin > 1 && lo >= hi) break;
+        launch(nwin > 1 ? lo : row_begin, nwin > 1 ? hi : row_end);
+        SGF_LAUNCH_CHECK(); count_launch();
+    }
+    return SGF_OK;
 }
 
 // exclusive scan of int counts (+add) into int64 out[0..n], using block_sums scratch
@@ -596,7 +725,7 @@ static constexpr int kHubBlocks = 16;
 // in fill order — still a valid CSR for the SpMM, but not bit-comparable.
 static constexpr int64_t kHubScratchMax = (int64_t)1 << 26;
 
-static CsrWs carve_ws(void* ws, int64_t nnz, int64_t n) {
+static CsrWs carve_ws(void* ws, int64_t nnz, int64_t n, size_t key_bytes = 4) {
     CsrWs w;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
@@ -611,7 +740,7 @@ static CsrWs carve_ws(void* ws, int64_t nnz, int64_t n) {
     int64_t tot = nnz + n;
     int64_t p2 = kSortSmemMax * kHubBlocks;
     while (p2 < tot && p2 < kHubScratchMax) p2 <<= 1;
-    size_t o_scr = take((size_t)p2 * 4);
+    size_t o_scr = take((size_t)p2 * key_bytes);
     w.counts = (int*)(base + o_counts); w.cursor = (int*)(base + o_cursor); w.block_sums = (int64_t*)(base + o_bs);
     w.total = (int64_t*)(base + o_misc); w.err = (int*)(base + o_misc + 8); w.n_long = (int*)(base + o_misc + 12);
     w.maxlen = (unsigned long long*)(base + o_misc + 16);
@@ -621,22 +750,25 @@ static CsrWs carve_ws(void* ws, int64_t nnz, int64_t n) {
 }
 
 // per-row ascending sort of col (tiers by row length; see the kernels)
-static int sort_long_rows(const int64_t* rowptr, int32_t* col, const CsrWs& w, cudaStream_t st);
-static int sort_rows(const int64_t* rowptr, int32_t* col, int64_t n, const CsrWs& w, cudaStream_t st) {
+template <typename T> static int sort_long_rows(const int64_t* rowptr, T* col, const CsrWs& w, cudaStream_t st);
+template <typename T>
+static int sort_rows(const int64_t* rowptr, T* col, int64_t n, const CsrWs& w, cudaStream_t st) {
     csr_sort_rows_warp_kernel<<<grid_for(n * 32, 256), 256, 0, st>>>(rowptr, n, col, w.long_rows, w.n_long);
     SGF_LAUNCH_CHECK(); count_launch();
     return sort_long_rows(rowptr, col, w, st);
 }
 // the rows queued in w.long_rows (longer than kWarpSortMax)
-static int sort_long_rows(const int64_t* rowptr, int32_t* col, const CsrWs& w, cudaStream_t st) {
+template <typename T>
+static int sort_long_rows(const int64_t* rowptr, T* col, const CsrWs& w, cudaStream_t st) {
+    T* scratch = reinterpret_cast<T*>(w.scratch);
     int64_t share = w.scratch_elems / kHubBlocks;
     // queued rows: (256, 2048] in shared memory across the whole chip; (2048, share] in global scratch by kHubBlocks
     // blocks; (share, scratch] by a single block.
-    csr_sort_rows_block_kernel<<<num_sms() * 4, 256, 0, st>>>(rowptr, col, w.long_rows, w.n_long, w.scratch, 0, 0, kSortSmemMax);
+    csr_sort_rows_block_kernel<<<num_sms() * 4, 256, 0, st>>>(rowptr, col, w.long_rows, w.n_long, scratch, 0, 0, kSortSmemMax);
     SGF_LAUNCH_CHECK(); count_launch();
-    csr_sort_rows_block_kernel<<<kHubBlocks, 1024, 0, st>>>(rowptr, col, w.long_rows, w.n_long, w.scratch, share, kSortSmemMax, share);
+    csr_sort_rows_block_kernel<<<kHubBlocks, 1024, 0, st>>>(rowptr, col, w.long_rows, w.n_long, scratch, share, kSortSmemMax, share);
     SGF_LAUNCH_CHECK(); count_launch();
-    csr_sort_rows_block_kernel<<<1, 1024, 0, st>>>(rowptr, col, w.long_rows, w.n_long, w.scratch, w.scratch_elems, share, w.scratch_elems);
+    csr_sort_rows_block_kernel<<<1, 1024, 0, st>>>(rowptr, col, w.long_rows, w.n_long, scratch, w.scratch_elems, share, w.scratch_elems);
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -683,18 +815,11 @@ extern "C" int sgf_csr_build_rot(const int64_t* edge_index, int64_t nnz, int64_t
         // already in L2 and are written back whole, at the price of re-reading the keys once per window.  The 128 MB window
         // exceeds the 50 MB L2 of an H100 yet builds the products-shaped CSR faster than a 40 MB one (13.9 vs 16.0 ms,
         // scripts/bench_csr.py on an H100 at a 400 W power limit): fewer windows re-read the keys fewer times.
-        const int64_t win_bytes = fill_window_bytes();
-        int64_t nwin = win_bytes > 0 ? ((nnz + n) * 4 + win_bytes - 1) / win_bytes : 1;
-        if (nwin > kMaxFillWindows) nwin = kMaxFillWindows;
-        if (nwin < 1 || n == 0) nwin = 1;
-        const int64_t rows_per = (n + nwin - 1) / nwin;
-        for (int64_t wi = 0; wi < nwin; ++wi) {
-            const int64_t lo = row_begin + wi * rows_per, hi = lo + rows_per < row_end ? lo + rows_per : row_end;
-            if (nwin > 1 && lo >= hi) break;
-            csr_fill_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(key, val, nnz, row_begin, nwin > 1 ? lo : row_begin, nwin > 1 ? hi : row_end,
-                                                               n_cols, self_loop_mode, rowptr, w.cursor, col);
-            SGF_LAUNCH_CHECK(); count_launch();
-        }
+        const int rcf = for_fill_windows(nnz, row_begin, row_end, 4, [&](int64_t lo, int64_t hi) {
+            csr_fill_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(key, val, nnz, row_begin, lo, hi, n_cols, self_loop_mode, rowptr,
+                                                               w.cursor, col);
+        });
+        if (rcf) return rcf;
     }
     if (self_loop_mode == 1 && n > 0) {
         csr_add_loops_kernel<<<grid_for(n, 256), 256, 0, st>>>(n, row_begin, rowptr, w.cursor, col);
@@ -939,6 +1064,87 @@ extern "C" int sgf_edge_symmetry(const int64_t* edge_index, int64_t nnz, int64_t
     if (nnz == 0) return SGF_OK;
     edge_symmetry_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(edge_index, edge_index + nnz, nnz, (uint64_t)n,
                                                             reinterpret_cast<unsigned long long*>(out2));
+    SGF_LAUNCH_CHECK(); count_launch();
+    return SGF_OK;
+}
+
+// ---- weighted build ----------------------------------------------------------------------------------------------------------
+// workspace: CsrWs with 8-byte sort scratch | keys int64[nnz + n] | last int64[n]
+struct WCsrWs { CsrWs csr; int64_t* keys; long long* last; size_t bytes; };
+static WCsrWs carve_wws(void* ws, int64_t nnz, int64_t n) {
+    WCsrWs u;
+    u.csr = carve_ws(ws, nnz, n, 8);
+    size_t off = align_up(u.csr.bytes, 256);
+    char* base = (char*)ws;
+    u.keys = (int64_t*)(base + off); off = align_up(off + (size_t)(nnz + n + 1) * 8, 256);
+    u.last = (long long*)(base + off); off = align_up(off + (size_t)(n + 1) * 8, 256);
+    u.bytes = off;
+    return u;
+}
+
+extern "C" int sgf_csr_build_weighted_ws_bytes(int64_t nnz, int64_t n, size_t* bytes) {
+    if (!bytes || nnz < 0 || n < 0) return SGF_ERR_ARG;
+    *bytes = carve_wws(nullptr, nnz, n).bytes;
+    return SGF_OK;
+}
+
+extern "C" int sgf_csr_build_weighted(const int64_t* edge_index, const float* weight, int64_t nnz, int64_t n, int by_source,
+                                      int self_loop_mode, int64_t* rowptr, int32_t* col, int64_t* eid, float* val, float* dinv,
+                                      void* ws, size_t ws_bytes, void* stream) {
+    if (nnz < 0 || n < 0 || n >= (int64_t)INT32_MAX || nnz >= (int64_t)UINT32_MAX || !rowptr || !ws) return SGF_ERR_ARG;
+    if (nnz + n > 0 && (!col || !eid || !val)) return SGF_ERR_ARG;
+    if (nnz > 0 && (!edge_index || !weight)) return SGF_ERR_ARG;
+    if (self_loop_mode != 0 && self_loop_mode != 1) return SGF_ERR_ARG;
+    WCsrWs u = carve_wws(ws, nnz, n);
+    if (ws_bytes < u.bytes) return SGF_ERR_ARG;
+    const CsrWs& w = u.csr;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t* key = by_source ? edge_index : edge_index + nnz;
+    const int64_t* other = by_source ? edge_index + nnz : edge_index;
+    SGF_CUDA_TRY(cudaMemsetAsync(w.total, 0, 64, st));
+    SGF_CUDA_TRY(cudaMemsetAsync(w.counts, 0, (size_t)(n + 1) * 4, st));
+    if (n == 0) return cudaMemsetAsync(rowptr, 0, 8, st) == cudaSuccess ? SGF_OK : SGF_ERR_ARG;
+    if (nnz > 0) {
+        csr_count_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(key, other, nnz, 0, n, n, self_loop_mode, w.counts, w.err);
+        SGF_LAUNCH_CHECK(); count_launch();
+    }
+    int rc = launch_scan(w.counts, n, self_loop_mode, rowptr, w.block_sums, w.total, w.cursor, st);
+    if (rc) return rc;
+    if (nnz > 0) {
+        rc = for_fill_windows(nnz, 0, n, 8, [&](int64_t lo, int64_t hi) {
+            csr_fill_keyed_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(key, other, nnz, lo, hi, n, self_loop_mode, rowptr, w.cursor,
+                                                                     u.keys);
+        });
+        if (rc) return rc;
+    }
+    if (self_loop_mode == 1) {
+        SGF_CUDA_TRY(cudaMemsetAsync(u.last, 0xff, (size_t)n * 8, st));      // -1: no self loop
+        if (nnz > 0) {
+            csr_last_loop_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(edge_index, edge_index + nnz, nnz, n, u.last);
+            SGF_LAUNCH_CHECK(); count_launch();
+        }
+        csr_add_loops_keyed_kernel<<<grid_for(n, 256), 256, 0, st>>>(n, u.last, rowptr, w.cursor, u.keys);
+        SGF_LAUNCH_CHECK(); count_launch();
+    }
+    if ((rc = sort_rows(rowptr, u.keys, n, w, st))) return rc;
+    csr_unpack_weighted_kernel<<<grid_for(nnz + n, 256), 256, 0, st>>>(u.keys, rowptr, n, weight, col, eid, val);
+    SGF_LAUNCH_CHECK(); count_launch();
+    if (dinv) {
+        if (self_loop_mode == 1) csr_weighted_dinv_kernel<<<grid_for(n, 256), 256, 0, st>>>(rowptr, val, n, dinv);
+        else csr_dinv_kernel<<<grid_for(n, 256), 256, 0, st>>>(rowptr, n, dinv);
+        SGF_LAUNCH_CHECK(); count_launch();
+    }
+    return SGF_OK;
+}
+
+extern "C" int sgf_edge_symmetry_weighted(const int64_t* edge_index, const float* weight, int64_t nnz, int64_t n, uint64_t* out2,
+                                          void* stream) {
+    if (nnz < 0 || n < 0 || !out2 || (nnz > 0 && (!edge_index || !weight))) return SGF_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    SGF_CUDA_TRY(cudaMemsetAsync(out2, 0, 16, st));
+    if (nnz == 0) return SGF_OK;
+    edge_symmetry_weighted_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(edge_index, edge_index + nnz, weight, nnz, (uint64_t)n,
+                                                                     reinterpret_cast<unsigned long long*>(out2));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }

@@ -14,6 +14,11 @@
 //   * kUnroll neighbour rows are in flight per lane group before the fp32 accumulation (memory-level parallelism:
 //     >= 64 KB in flight per SM at 32 resident warps, above the ~44 KB latency-bandwidth product of one SM's HBM share).
 // Algorithmic bytes per launch: nnz*4 + (n+1)*8 + nnz*h*b + n*h*b (DESIGN.md §SpMM).
+//
+// Weighted graphs (edge_weight, DESIGN.md §4.10): the WEIGHTED instantiations also read the fp32 value array `val` next to `col`
+// (32 at a time, broadcast by shuffle like the column ids) and FMA it into the fp32 accumulation: nnz*8 index + value bytes
+// instead of nnz*4.  The dinv pre-scale by the producer and the row_scale post-scale stay as they are.  The value pointer is the
+// kernels' last parameter, so the unweighted instantiations compile to the same code as before.
 #include "common.cuh"
 #include "launch_count.h"
 #include "../../include/sgformer_b200.h"
@@ -37,18 +42,21 @@ constexpr int kUnroll = SGF_SPMM_UNROLL;
 constexpr int kMinBlocks = SGF_SPMM_MIN_BLOCKS;
 
 // gather-accumulate up to 32 neighbour rows whose ids sit one per lane in my_idx (cnt valid), all lane groups cooperating
-template <typename T, int CPL, bool COH = false>
+template <typename T, int CPL, bool COH = false, bool WEIGHTED = false>
 __device__ __forceinline__ void gather_item(int my_idx, int cnt, const T* __restrict__ x, int64_t ldx, int groups, int grp,
-                                            const int (&coff)[CPL], const bool (&cval)[CPL], float (&acc)[CPL][Vec16<T>::N]) {
+                                            const int (&coff)[CPL], const bool (&cval)[CPL], float (&acc)[CPL][Vec16<T>::N],
+                                            float my_w = 0.f) {
     constexpr int VN = Vec16<T>::N;
     for (int j0 = 0; j0 < cnt; j0 += groups * kUnroll) {
         uint4 v[kUnroll][CPL];
         int nb[kUnroll];
+        float wt[kUnroll];
 #pragma unroll
         for (int u = 0; u < kUnroll; ++u) {
             int j = j0 + u * groups + grp;
             int t = __shfl_sync(0xffffffffu, my_idx, j & 31);
             nb[u] = j < cnt ? t : -1;
+            if constexpr (WEIGHTED) wt[u] = __shfl_sync(0xffffffffu, my_w, j & 31);
         }
 #pragma unroll
         for (int u = 0; u < kUnroll; ++u) {
@@ -65,21 +73,32 @@ __device__ __forceinline__ void gather_item(int my_idx, int cnt, const T* __rest
             for (int c = 0; c < CPL; ++c) {
                 float f[VN];
                 Vec16<T>::unpack(v[u][c], f);
+                if constexpr (WEIGHTED) {
 #pragma unroll
-                for (int i = 0; i < VN; ++i) acc[c][i] += f[i];
+                    for (int i = 0; i < VN; ++i) acc[c][i] = fmaf(wt[u], f[i], acc[c][i]);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < VN; ++i) acc[c][i] += f[i];
+                }
             }
     }
 }
 
 // gather-accumulate the neighbour rows col[s..e) of x into acc (fp32)
-template <typename T, int CPL>
+// (WEIGHTED: entry j contributes val[j] * x[col[j], :])
+template <typename T, int CPL, bool WEIGHTED = false>
 __device__ __forceinline__ void gather_range(const int32_t* __restrict__ col, const T* __restrict__ x, int64_t ldx, int64_t s, int64_t e,
                                              int lane, int groups, int grp, const int (&coff)[CPL], const bool (&cval)[CPL],
-                                             float (&acc)[CPL][Vec16<T>::N]) {
+                                             float (&acc)[CPL][Vec16<T>::N], const float* __restrict__ val = nullptr) {
     for (int64_t base = s; base < e; base += 32) {
         const int cnt = (int)((e - base) < 32 ? (e - base) : 32);
         const int my_idx = lane < cnt ? ldg_nc_na_s32(col + base + lane) : -1;
-        gather_item<T, CPL>(my_idx, cnt, x, ldx, groups, grp, coff, cval, acc);
+        if constexpr (WEIGHTED) {
+            const float my_w = lane < cnt ? __ldg(val + base + lane) : 0.f;
+            gather_item<T, CPL, false, true>(my_idx, cnt, x, ldx, groups, grp, coff, cval, acc, my_w);
+        } else {
+            gather_item<T, CPL>(my_idx, cnt, x, ldx, groups, grp, coff, cval, acc);
+        }
     }
 }
 
@@ -211,11 +230,11 @@ spmm_range_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict_
     }
 }
 
-template <typename T, int CPL, bool FLAGS = false>
+template <typename T, int CPL, bool FLAGS = false, bool WEIGHTED = false>
 __global__ void __launch_bounds__(kSpmmBlock, kMinBlocks)
 spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col, const float* __restrict__ row_scale,
                  const T* __restrict__ x, int64_t ldx, T* __restrict__ y, int64_t ldy, int64_t n_rows, int chunks, int lpr_log2,
-                 int64_t max_len, SlotWait sw) {
+                 int64_t max_len, SlotWait sw, const float* __restrict__ val = nullptr) {
     constexpr int VN = Vec16<T>::N;
     __shared__ int s_ready, s_lock;
     int ready = 0;
@@ -239,7 +258,7 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
         coff[c] = ch * VN;
     }
 #if SGF_SPMM_PIPELINE
-    static_assert(!FLAGS, "the flagged variant uses the simple loop");
+    static_assert(!FLAGS && !WEIGHTED, "the flagged and weighted variants use the simple loop");
     int64_t r = warp0;
     if (r >= n_rows) return;
     // current row [s, e) (a skipped hub row behaves like an empty row that is not stored), next row [sn, en)
@@ -316,7 +335,7 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
 #pragma unroll
             for (int i = 0; i < VN; ++i) acc[c][i] = 0.f;
         if (FLAGS) gather_range_flagged<T, CPL>(col, x, ldx, s, e, lane, groups, grp, coff, cval, acc, sw, ready, &s_ready, &s_lock);
-        else gather_range<T, CPL>(col, x, ldx, s, e, lane, groups, grp, coff, cval, acc);
+        else gather_range<T, CPL, WEIGHTED>(col, x, ldx, s, e, lane, groups, grp, coff, cval, acc, val);
         for (int o = lpr; o < 32; o <<= 1) {
 #pragma unroll
             for (int c = 0; c < CPL; ++c)
@@ -341,11 +360,11 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
 
 // hub rows (power-law graphs): a row longer than the threshold is cut into segments, one warp per segment writes an fp32
 // partial sum, and a second kernel adds a row's partials in fixed order (deterministic), scales and stores the row.
-template <typename T, int CPL>
+template <typename T, int CPL, bool WEIGHTED = false>
 __global__ void __launch_bounds__(kSpmmBlock, kMinBlocks)
 spmm_segments_kernel(const int32_t* __restrict__ col, const T* __restrict__ x, int64_t ldx, const int64_t* __restrict__ seg_start,
                      const int32_t* __restrict__ seg_len, int64_t n_seg, float* __restrict__ partial, int h, int chunks,
-                     int lpr_log2) {
+                     int lpr_log2, const float* __restrict__ val = nullptr) {
     constexpr int VN = Vec16<T>::N;
     const int lane = threadIdx.x & 31;
     const int lpr = 1 << lpr_log2;
@@ -369,7 +388,7 @@ spmm_segments_kernel(const int32_t* __restrict__ col, const T* __restrict__ x, i
         for (int c = 0; c < CPL; ++c)
 #pragma unroll
             for (int i = 0; i < VN; ++i) acc[c][i] = 0.f;
-        gather_range<T, CPL>(col, x, ldx, s, s + seg_len[sg], lane, groups, grp, coff, cval, acc);
+        gather_range<T, CPL, WEIGHTED>(col, x, ldx, s, s + seg_len[sg], lane, groups, grp, coff, cval, acc, val);
         for (int o = lpr; o < 32; o <<= 1) {
 #pragma unroll
             for (int c = 0; c < CPL; ++c)
@@ -404,7 +423,8 @@ __global__ void spmm_heavy_finalize_kernel(const float* __restrict__ partial, co
 
 template <typename T>
 static int launch_spmm(const int64_t* rowptr, const int32_t* col, const float* row_scale, const void* x, int64_t ldx,
-                       void* y, int64_t ldy, int64_t n_rows, int h, int64_t max_len, cudaStream_t st, const SlotWait* slots = nullptr) {
+                       void* y, int64_t ldy, int64_t n_rows, int h, int64_t max_len, cudaStream_t st, const SlotWait* slots = nullptr,
+                       const float* val = nullptr) {
     constexpr int VN = Vec16<T>::N;
     if (h % VN != 0 || ldx % VN != 0 || ldy % VN != 0) return SGF_ERR_ARG;
     if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15)) return SGF_ERR_ARG;
@@ -430,6 +450,9 @@ static int launch_spmm(const int64_t* rowptr, const int32_t* col, const float* r
         if (slots)                                                                                                    \
             spmm_rows_kernel<T, N, true><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(rowptr, col, row_scale, xp, ldx, yp, ldy, \
                                                                                   n_rows, chunks, lpr_log2, max_len, sw);   \
+        else if (val)                                                                                                 \
+            spmm_rows_kernel<T, N, false, true><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(rowptr, col, row_scale, xp, ldx, yp, \
+                                                                                   ldy, n_rows, chunks, lpr_log2, max_len, sw, val); \
         else                                                                                                          \
             spmm_rows_kernel<T, N><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(rowptr, col, row_scale, xp, ldx, yp, ldy,  \
                                                                             n_rows, chunks, lpr_log2, max_len, sw);    \
@@ -487,7 +510,8 @@ static int launch_range(const int64_t* rowptr, const int32_t* col, const float* 
 template <typename T>
 static int launch_heavy(const int32_t* col, const float* row_scale, const void* x, int64_t ldx, void* y, int64_t ldy, int h,
                         const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg, float* partial,
-                        const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, cudaStream_t st) {
+                        const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, cudaStream_t st,
+                        const float* val = nullptr) {
     constexpr int VN = Vec16<T>::N;
     if (h % VN != 0 || ldx % VN != 0) return SGF_ERR_ARG;
     const int chunks = h / VN;
@@ -501,8 +525,12 @@ static int launch_heavy(const int32_t* col, const float* row_scale, const void* 
     const T* xp = static_cast<const T*>(x);
 #define SGF_SEG_CASE(N)                                                                                                 \
     case N:                                                                                                             \
-        spmm_segments_kernel<T, N><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(col, xp, ldx, seg_start, seg_len, n_seg, partial, \
-                                                                            h, chunks, lpr_log2);                       \
+        if (val)                                                                                                        \
+            spmm_segments_kernel<T, N, true><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(col, xp, ldx, seg_start, seg_len, n_seg, \
+                                                                                      partial, h, chunks, lpr_log2, val); \
+        else                                                                                                            \
+            spmm_segments_kernel<T, N><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(col, xp, ldx, seg_start, seg_len, n_seg, \
+                                                                                partial, h, chunks, lpr_log2);          \
         break;
     switch (cpl) {
         SGF_SEG_CASE(1)
@@ -603,5 +631,34 @@ extern "C" int sgf_spmm_heavy(const int32_t* col, const float* row_scale, const 
     if (dtype == 1)
         return sgf::launch_heavy<__nv_bfloat16>(col, row_scale, x, ldx, y, ldy, h, seg_start, seg_len, n_seg, partial, heavy_rows,
                                                 heavy_seg_ptr, n_heavy, st);
+    return SGF_ERR_ARG;
+}
+
+extern "C" int sgf_spmm_weighted(const int64_t* rowptr, const int32_t* col, const float* val, const float* row_scale, const void* x,
+                                 int64_t ldx, void* y, int64_t ldy, int64_t n_rows, int h, int dtype, int64_t max_row_len,
+                                 void* stream) {
+    if (!rowptr || n_rows < 0 || h <= 0 || (n_rows > 0 && (!x || !y || !val)) || max_row_len < 0) return SGF_ERR_ARG;
+    if (n_rows == 0) return SGF_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == 0) return sgf::launch_spmm<float>(rowptr, col, row_scale, x, ldx, y, ldy, n_rows, h, max_row_len, st, nullptr, val);
+    if (dtype == 1)
+        return sgf::launch_spmm<__nv_bfloat16>(rowptr, col, row_scale, x, ldx, y, ldy, n_rows, h, max_row_len, st, nullptr, val);
+    return SGF_ERR_ARG;
+}
+
+extern "C" int sgf_spmm_heavy_weighted(const int32_t* col, const float* val, const float* row_scale, const void* x, int64_t ldx,
+                                       void* y, int64_t ldy, int h, int dtype, const int64_t* seg_start, const int32_t* seg_len,
+                                       int64_t n_seg, float* partial, const int64_t* heavy_rows, const int64_t* heavy_seg_ptr,
+                                       int64_t n_heavy, void* stream) {
+    if (!col || !val || !x || !y || h <= 0 || n_seg < 0 || n_heavy < 0) return SGF_ERR_ARG;
+    if (n_seg == 0 || n_heavy == 0) return SGF_OK;
+    if (!seg_start || !seg_len || !partial || !heavy_rows || !heavy_seg_ptr) return SGF_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == 0)
+        return sgf::launch_heavy<float>(col, row_scale, x, ldx, y, ldy, h, seg_start, seg_len, n_seg, partial, heavy_rows,
+                                        heavy_seg_ptr, n_heavy, st, val);
+    if (dtype == 1)
+        return sgf::launch_heavy<__nv_bfloat16>(col, row_scale, x, ldx, y, ldy, h, seg_start, seg_len, n_seg, partial, heavy_rows,
+                                                heavy_seg_ptr, n_heavy, st, val);
     return SGF_ERR_ARG;
 }

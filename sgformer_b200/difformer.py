@@ -2,7 +2,9 @@
 
 `DIFFormer` keeps the reference's attribute tree (state_dict keys, `Wk` before `Wq`, inits, `reset_parameters` of convs, bns and
 fcs), so `.to()`, `copy.deepcopy` and `load_state_dict` behave as there; its forward and backward run as one schedule on the CUDA
-kernels (functional.DIFFormerFn).  Out of scope, each with an error: num_heads > 1, kernel='sigmoid' (O(N^2)), edge weights."""
+kernels (functional.DIFFormerFn).  `DIFFormer.forward(data, edge_weight)` runs its graph term on the weighted CSR build and SpMM.
+Out of scope, each with an error: num_heads > 1, kernel='sigmoid' (O(N^2)), multi-dimensional edge attributes, and edge weights in
+the standalone `gcn_conv`."""
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -31,9 +33,10 @@ def full_attention_conv(qs, ks, vs, kernel, output_attn=False):
 
 def gcn_conv(x, edge_index, edge_weight):
     """medium/difformer.py:63-79: y[:, h] = D^-1/2 A D^-1/2 x[:, h] (in-degree over edge targets, no self loops) on the CSR
-    SpMM kernel.  x: [N, H, D]."""
+    SpMM kernel.  x: [N, H, D].  Edge weights run inside DIFFormer.forward (the fused schedule), not through this function."""
     if edge_weight is not None:
-        raise NotImplementedError("sgformer_b200.gcn_conv: edge_weight is not supported")
+        raise NotImplementedError("sgformer_b200.gcn_conv: edge_weight is not supported by the standalone function; "
+                                  "DIFFormer.forward(data, edge_weight) runs weighted graphs")
     if not x.is_cuda:
         _require_cuda("gcn_conv")
         raise RuntimeError("sgformer_b200.gcn_conv needs CUDA tensors (no CPU fallback)")
@@ -117,14 +120,16 @@ class DIFFormer(_Base):
 
     def forward(self, data, edge_weight=None):
         x, edge_index = data.graph['node_feat'], data.graph['edge_index']
-        if edge_weight is not None:
-            raise NotImplementedError("sgformer_b200.DIFFormer: edge_weight is not supported")
         if not x.is_cuda:
             _require_cuda("DIFFormer")
             raise RuntimeError("sgformer_b200.DIFFormer needs the dataset on a CUDA device (no CPU fallback)")
         cfg = self._cfg()
-        graph = get_graph(edge_index, x.shape[0], 0) if cfg["use_graph"] else None
         names, tensors = self._flat()
+        graph = None
+        if cfg["use_graph"]:       # edge_weight only reaches gcn_conv, which runs only with use_graph (medium/difformer.py:129)
+            graph = get_graph(edge_index, x.shape[0], 0, edge_weight=edge_weight)
+            if edge_weight is not None:
+                names, tensors = tuple(names) + (E.EDGE_WEIGHT,), list(tensors) + [edge_weight]
         return Fn.DIFFormerFn.apply(x, graph, cfg, E.precision(self.precision), self.training, names, *tensors)
 
     def get_attentions(self, x):

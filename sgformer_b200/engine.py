@@ -661,6 +661,33 @@ def _slice_rows(op: K.Operand, r0: int, r1: int) -> K.Operand:
 # =================================================================================================
 # GCN backbone (medium): PyG GCNConv stack
 # =================================================================================================
+# Weighted graphs (edge_weight, DESIGN.md §4.10): `graph` is the weighted Graph; layers < L-1 run on it (its weighted dinv is their
+# pre / post scale, the SpMMs read its values), the last one on the unweighted pattern (graph.pattern()), as models.GCN passes
+# edge_weight to every conv but the last (medium/models.py:53-62).  The edge-weight gradient (P[EDGE_WEIGHT] requiring grad) is
+# summed over the weighted layers by sgf_edge_weight_grad, which needs each layer's t = dinv (.) x W^T from the forward.
+EDGE_WEIGHT = "edge_weight"
+
+
+def _is_weighted(graph) -> bool:
+    return getattr(graph, "val", None) is not None
+
+
+def _layer_graph(graph: Graph, last: bool) -> Graph:
+    return graph.pattern() if _is_weighted(graph) and last else graph
+
+
+def _weighted_spmm(g: Graph, transposed: bool, row_scale: Tensor, x: Tensor) -> Tensor:
+    if transposed:
+        rp, cl = g.transpose()
+        return K.spmm(rp, cl, row_scale, x, heavy=g.heavy_t, val=g.val_t)
+    return K.spmm(g.rowptr, g.col, row_scale, x, heavy=g.heavy, val=g.val)
+
+
+def _want_edge_grad(P) -> bool:
+    w = P.get(EDGE_WEIGHT)
+    return w is not None and w.requires_grad
+
+
 def gcn_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, training: bool, seed: int,
                 tape: Optional[Tape], mix: Optional[Tensor] = None, gw: float = 1.0, pfx: str = "gnn.",
                 comm: Comm = SINGLE) -> Tensor:
@@ -670,18 +697,22 @@ def gcn_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, tra
     dev = xin.data.device
     p = float(cfg["gcn_dropout"]) if training else 0.0
     use_bn = bool(cfg["gcn_use_bn"])
-    dinv = graph.dinv
+    if _is_weighted(graph) and comm.active:
+        raise NotImplementedError("sgformer_b200: row sharding of a weighted graph is not supported")
+    keep_t = tape is not None and _is_weighted(graph) and _want_edge_grad(P)
     cur_op, cur_k = xin, cfg["in_channels"]
     layers = []
     out = None
     for i in range(nl):
         last = i == nl - 1
+        g = _layer_graph(graph, last)
+        dinv = g.dinv
         wname = f"{pfx}convs.{i}.lin.weight"
         hout = P[wname].shape[0]
         check_width(hout, prec, f"GCN layer {i} out_channels")
         t = K.gemm_nt([cur_op], [_w(P, wname, prec)], [(0, 0, 0, 0, cur_k)], hout, K.alloc_act(n, hout, prec.act_dtype, dev),
                       row_scale=dinv)
-        s = comm.spmm_gathered(K, graph, False, dinv, t)
+        s = _weighted_spmm(g, False, dinv, t) if _is_weighted(g) else comm.spmm_gathered(K, g, False, dinv, t)
         zb = P.get(f"{pfx}convs.{i}.bias")
         if last:
             out, _ = K.bn_fwd(s, None, mix, None, None, None, None, zb, False, False, 0.0, 0, gw, None, True, False)
@@ -691,7 +722,7 @@ def gcn_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, tra
             mean, rstd = _bn_stats(s, P, name, use_bn, training, zbias=zb, comm=comm)
             y, _ = K.bn_fwd(s, None, None, mean, rstd, P.get(name + "weight"), P.get(name + "bias"), zb, use_bn, True, p,
                             seed + _SEED_GCN_LAYER + i, 1.0, None, True, False)
-            layers.append(dict(s=s, cur_op=cur_op, cur_k=cur_k, hout=hout, mean=mean, rstd=rstd))
+            layers.append(dict(s=s, cur_op=cur_op, cur_k=cur_k, hout=hout, mean=mean, rstd=rstd, t=t if keep_t else None))
             cur_op, cur_k = K.as_operand(y, prec.planes), hout
     if tape is not None:
         tape.update(layers=layers, p=p, seed=seed, n=n, training=training, mixed=mix is not None, gw=gw)
@@ -704,15 +735,20 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
     n, p, seed, training = tape["n"], tape["p"], tape["seed"], tape["training"]
     dev = dout.device
     use_bn = bool(cfg["gcn_use_bn"])
-    dinv = graph.dinv
     red = comm.allreduce_ if comm.active else None
     nstat = comm.n_global if comm.active else 0
     gs = tape["gw"] if tape["mixed"] else 1.0
     dcur = dout
     dx = None
+    dew = None
+    if _is_weighted(graph) and _want_edge_grad(P):
+        dew = torch.zeros(graph.edge_index.shape[1], dtype=torch.float32, device=dev)
+        grads[EDGE_WEIGHT] = dew
     for i in reversed(range(nl)):
         L = tape["layers"][i]
         last = i == nl - 1
+        g = _layer_graph(graph, last)
+        dinv = g.dinv
         zb = P.get(f"{pfx}convs.{i}.bias")
         hout = L["hout"]
         if last:
@@ -728,7 +764,13 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         gs = 1.0
         if zb is not None:
             grads[f"{pfx}convs.{i}.bias"] = colsum
-        u = comm.spmm_gathered(K, graph, True, dinv, dzs)        # = Â^T dz = gradient of (x W^T)
+        if _is_weighted(g):
+            u = _weighted_spmm(g, True, dinv, dzs)
+            if dew is not None:     # dL/dw of this layer: <dzs_c, t_r> + the degree term of row c
+                K.edge_weight_grad(g.rowptr, g.col, g.eid, dzs, L["t"], dew, y=L["s"], u=u, dinv=dinv, edge_index=g.edge_index,
+                                   loops=True)
+        else:
+            u = comm.spmm_gathered(K, g, True, dinv, dzs)        # = Â^T dz = gradient of (x W^T)
         u_op = K.as_operand(u, prec.planes)
         wname = f"{pfx}convs.{i}.lin.weight"
         dw = torch.empty((hout, L["cur_k"]), dtype=torch.float32, device=dev)
@@ -977,6 +1019,8 @@ def difformer_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, graph: Op
     t0, x, st0 = _stem_forward(P, "", xin, h, use_ln, prec, p, seed + _SEED_STEM, tape is not None)
     x0 = x
     layers = []
+    # weighted graph (gcn_conv's edge_weight): value = w dinv[c] dinv[r] with the unweighted dinv; dL/dw needs dinv (.) v
+    keep_v = tape is not None and use_graph and _is_weighted(graph) and _want_edge_grad(P)
     for i in range(nl):
         lp = f"convs.{i}."
         a, b, c, s_ = _difformer_coefs(cfg, i)
@@ -984,13 +1028,16 @@ def difformer_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, graph: Op
         o = attention_gram_forward(P, lp, x, use_weight, prec, at, vsum=True)
         r, b = _difformer_residual(x, x0, i, b, s_)
         gamma, beta = P.get(f"bns.{i + 1}.weight"), P.get(f"bns.{i + 1}.bias")
+        vs = None
         if use_graph:
-            y = K.spmm(graph.rowptr, graph.col, graph.dinv, _difformer_v_scaled(P, lp, x, use_weight, prec, graph.dinv),
-                       heavy=graph.heavy)
+            vs = _difformer_v_scaled(P, lp, x, use_weight, prec, graph.dinv)
+            y = _weighted_spmm(graph, False, graph.dinv, vs) if _is_weighted(graph) else \
+                K.spmm(graph.rowptr, graph.col, graph.dinv, vs, heavy=graph.heavy)
             xn, st = K.ln_fwd_graph(o, r, y, a, b, c, gamma, beta, use_ln, False, p, seed + _SEED_LAYER + i, tape is not None)
         else:
             xn, st = K.ln_fwd(o, r, a, b, gamma, beta, use_ln, False, p, seed + _SEED_LAYER + i, tape is not None)
-        layers.append(dict(x_in=x, attn=at, o=o, r=r, y=y if use_graph else None, st=st, coef=(a, b, c)))
+        layers.append(dict(x_in=x, attn=at, o=o, r=r, y=y if use_graph else None, st=st, coef=(a, b, c),
+                           vs=vs if keep_v else None))
         x = xn
     logits = head_forward(P, cfg, [x], prec, tape, "fcs.1.")
     if tape is not None:
@@ -1006,8 +1053,12 @@ def difformer_backward(P: Dict[str, Tensor], cfg: dict, tape: Tape, graph: Optio
     use_ln, use_weight, use_graph = bool(cfg["use_bn"]), bool(cfg["use_weight"]), bool(cfg["use_graph"])
     dcur = head_backward(P, cfg, tape, dlogits, prec, grads, "fcs.1.")[0]
     dx0 = None                     # use_source: gradient of x0 collected from layers 1..L-1
+    dew = None
     if use_graph:
         rp_t, col_t = graph.transpose()
+        if _is_weighted(graph) and _want_edge_grad(P):
+            dew = torch.zeros(graph.edge_index.shape[1], dtype=torch.float32, device=dev)
+            grads[EDGE_WEIGHT] = dew
     for i in reversed(range(nl)):
         L = tape["layers"][i]
         lp = f"convs.{i}."
@@ -1036,7 +1087,12 @@ def difformer_backward(P: Dict[str, Tensor], cfg: dict, tape: Tape, graph: Optio
         else:
             dprev, acc = K.new_like(x_in), False
         # attention (value-sum Gram form) + graph term: dv = dinv (.) A^T (dinv (.) c du)
-        dv = K.spmm(rp_t, col_t, graph.dinv, ys, heavy=graph.heavy_t) if use_graph else None
+        dv = None
+        if use_graph:
+            dv = _weighted_spmm(graph, True, graph.dinv, ys) if _is_weighted(graph) else \
+                K.spmm(rp_t, col_t, graph.dinv, ys, heavy=graph.heavy_t)
+        if dew is not None:        # dL/dw = dinv_c dinv_r <c du_c, v_r> = <ys_c, vs_r>
+            K.edge_weight_grad(graph.rowptr, graph.col, graph.eid, ys, L["vs"], dew)
         attention_gram_backward(P, lp, at, x_in, gnum, gden, cs, pg, sg, use_weight, prec, dprev, acc, grads, dv=dv)
         if i == 0 and dx0 is not None:
             dprev = K.axpby(dprev, dx0, 1.0, 1.0)

@@ -118,6 +118,77 @@ def csr_build(edge_index: Tensor, n: int, by_source: bool = False, self_loop_mod
     return rowptr, col, (dinv[:n] if dinv is not None else None)
 
 
+def edge_weight_vec(edge_weight: Tensor, nnz: int) -> Tensor:
+    """edge_weight as contiguous fp32 [nnz] (other floating dtypes are cast, as the drivers pass fp32)."""
+    _use(edge_weight)
+    if edge_weight.dim() != 1 or edge_weight.numel() != nnz or not edge_weight.dtype.is_floating_point:
+        raise ValueError(f"edge_weight must be a floating [nnz={nnz}] vector (multi-dimensional edge_attr is not supported); "
+                         f"got {edge_weight.dtype} {tuple(edge_weight.shape)}")
+    return edge_weight.detach().to(torch.float32).contiguous()
+
+
+def csr_build_weighted(edge_index: Tensor, edge_weight: Tensor, n: int, by_source: bool = False, self_loop_mode: int = 0,
+                       want_dinv: bool = True):
+    """-> (rowptr int64 [n+1], col int32 [nnz'], eid int64 [nnz'], val fp32 [nnz'], dinv fp32 [n] | None): the weighted CSR of
+    sgf_csr_build_weighted (rows sorted by (col, eid); self_loop_mode 1: the added loop carries the weight of the node's last self
+    loop; dinv = weighted deg^-1/2 in mode 1, the count-based one in mode 0)."""
+    _use(edge_index)
+    if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
+        raise ValueError("edge_index must be int64 [2, nnz]")
+    ei = edge_index.contiguous()
+    nnz = ei.shape[1]
+    w = edge_weight_vec(edge_weight, nnz)
+    dev = ei.device
+    cap = max(nnz + (n if self_loop_mode == 1 else 0), 1)
+    rowptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    col = torch.empty(cap, dtype=torch.int32, device=dev)
+    eid = torch.empty(cap, dtype=torch.int64, device=dev)
+    val = torch.empty(cap, dtype=torch.float32, device=dev)
+    dinv = torch.empty(max(n, 1), dtype=torch.float32, device=dev) if want_dinv else None
+    nbytes = C.c_size_t(0)
+    check(lib().sgf_csr_build_weighted_ws_bytes(nnz, n, C.byref(nbytes)), "sgf_csr_build_weighted_ws_bytes")
+    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+    check(lib().sgf_csr_build_weighted(_p(ei), _p(w), nnz, n, int(by_source), self_loop_mode, _p(rowptr), _p(col), _p(eid), _p(val),
+                                       _p(dinv), _p(ws), nbytes.value, _stream()), "sgf_csr_build_weighted")
+    total = int(rowptr[n].item()) if self_loop_mode == 1 else nnz      # mode 1: existing self loops dropped (one device sync)
+    return rowptr, col[:total], eid[:total], val[:total], (dinv[:n] if dinv is not None else None)
+
+
+def edge_symmetry_weighted(edge_index: Tensor, edge_weight: Tensor, n: int) -> bool:
+    """Multiset equality of {(r,c,w)} and {(c,r,w)} (edge_symmetry with the weights' bit patterns hashed along)."""
+    ei = _edge_index(edge_index)
+    w = edge_weight_vec(edge_weight, ei.shape[1])
+    out = torch.empty(2, dtype=torch.int64, device=ei.device)
+    check(lib().sgf_edge_symmetry_weighted(_p(ei), _p(w), ei.shape[1], n, _p(out), _stream()), "sgf_edge_symmetry_weighted")
+    a, b = out.tolist()
+    return a == b
+
+
+def edge_weight_grad(rowptr: Tensor, col: Tensor, eid: Tensor, a: Tensor, b: Tensor, out: Tensor, y: Optional[Tensor] = None,
+                     u: Optional[Tensor] = None, dinv: Optional[Tensor] = None, edge_index: Optional[Tensor] = None,
+                     loops: bool = False):
+    """out[eid[j]] += <a_c, b_r> (+ the degree term -1/2 dinv_c (<a_c, y_c> + <b_c, u_c>) when y is given) for every CSR entry
+    j = (c, r); `loops` (self_loop_mode 1): the added loop's share goes to every self-loop edge of edge_index (sgf_edge_weight_grad)."""
+    _use(a)
+    n = rowptr.numel() - 1
+    _, h, lda = _mat(a, "a")
+    _, hb, ldb = _mat(b, "b")
+    if hb != h or b.dtype != a.dtype or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError("edge_weight_grad: operand shape/dtype mismatch")
+    ldy = ldu = 0
+    if y is not None:
+        _, _, ldy = _mat(y, "y")
+        _, _, ldu = _mat(u, "u")
+        if y.dtype != a.dtype or u.dtype != a.dtype:
+            raise ValueError("edge_weight_grad: y / u dtype mismatch")
+    loop_grad = torch.empty(max(n, 1), dtype=torch.float32, device=a.device) if loops else None
+    ei = _edge_index(edge_index) if loops else None
+    check(lib().sgf_edge_weight_grad(_p(rowptr), _p(col), _p(eid), n, h, dcode(a), _p(a), lda, _p(b), ldb, _p(y), ldy, _p(u), ldu,
+                                     _p(_f32vec(dinv, n, "dinv")), _p(ei), out.numel(), _p(loop_grad), _p(out), _stream()),
+          "sgf_edge_weight_grad")
+    return out
+
+
 def subgraph(edge_index: Tensor, n: int, subset: Tensor) -> Tensor:
     """Induced subgraph with relabelling; returns int64 [2, nnz_sub] in input edge order (PyG `subgraph` semantics)."""
     _use(edge_index)
@@ -247,7 +318,10 @@ def heavy_rows(rowptr: Tensor) -> Optional[HeavyRows]:
 
 
 def spmm(rowptr: Tensor, col: Tensor, row_scale: Optional[Tensor], x: Tensor, out: Optional[Tensor] = None,
-         heavy: Optional[HeavyRows] = None) -> Tensor:
+         heavy: Optional[HeavyRows] = None, val: Optional[Tensor] = None) -> Tensor:
+    """y = row_scale (.) A x over the CSR (rowptr, col); `val` (fp32 [nnz]): the weighted CSR's values (sgf_spmm_weighted)."""
+    if val is not None:
+        return _spmm_weighted(rowptr, col, val, row_scale, x, out, heavy)
     _use(x)
     n = rowptr.numel() - 1
     rows, h, ldx = _mat(x, "x")
@@ -269,6 +343,37 @@ def spmm(rowptr: Tensor, col: Tensor, row_scale: Optional[Tensor], x: Tensor, ou
         check(lib().sgf_spmm_heavy(_p(col), _p(rs), _p(x), ldx, _p(out), ldy, h, dcode(x), _p(heavy.seg_start),
                                    _p(heavy.seg_len), ns, _p(partial), _p(heavy.rows), _p(heavy.seg_ptr), heavy.rows.numel(),
                                    _stream()), "sgf_spmm_heavy")
+    if ev is not None:
+        e1.record()
+        ev.append((e0, e1))
+    return out
+
+
+def _spmm_weighted(rowptr: Tensor, col: Tensor, val: Tensor, row_scale: Optional[Tensor], x: Tensor, out: Optional[Tensor],
+                   heavy: Optional[HeavyRows]) -> Tensor:
+    _use(x)
+    n = rowptr.numel() - 1
+    rows, h, ldx = _mat(x, "x")
+    if val.dtype != torch.float32 or not val.is_contiguous() or val.numel() != col.numel():
+        raise ValueError("spmm: val must be contiguous fp32 with one value per column id")
+    if out is None:
+        out = alloc_act(n, h, x.dtype, x.device)
+    _, ho, ldy = _mat(out, "out")
+    if ho != h or out.dtype != x.dtype:
+        raise ValueError("spmm: out shape/dtype mismatch")
+    ev = spmm_events
+    if ev is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    rs = _f32vec(row_scale, n, "row_scale")
+    check(lib().sgf_spmm_weighted(_p(rowptr), _p(col), _p(val), _p(rs), _p(x), ldx, _p(out), ldy, n, h, dcode(x),
+                                  HEAVY_ROW if heavy is not None else 0, _stream()), "sgf_spmm_weighted")
+    if heavy is not None:
+        ns = heavy.seg_start.numel()
+        partial = torch.empty((ns, h), dtype=torch.float32, device=x.device)
+        check(lib().sgf_spmm_heavy_weighted(_p(col), _p(val), _p(rs), _p(x), ldx, _p(out), ldy, h, dcode(x), _p(heavy.seg_start),
+                                            _p(heavy.seg_len), ns, _p(partial), _p(heavy.rows), _p(heavy.seg_ptr),
+                                            heavy.rows.numel(), _stream()), "sgf_spmm_heavy_weighted")
     if ev is not None:
         e1.record()
         ev.append((e0, e1))

@@ -96,16 +96,23 @@ class GCN(_Base):
 
     def forward(self, data):
         x, edge_index = data.graph['node_feat'], data.graph['edge_index']
-        if 'edge_weight' in data.graph and data.graph['edge_weight'] is not None:
-            raise NotImplementedError("sgformer_b200.GCN: edge_weight is not supported")
         if not x.is_cuda:
             raise RuntimeError("sgformer_b200.GCN needs CUDA tensors (no CPU fallback)")
         names, tensors = _gcn_flat(self, "gnn.")
         cfg = make_config("medium", x.shape[1], self.convs[0].out_channels, self.convs[-1].out_channels,
                           gcn_num_layers=len(self.convs), gcn_dropout=self.dropout, gcn_use_bn=self.use_bn)
-        graph = get_graph(edge_index, x.shape[0], 1)
+        graph, names, tensors = _gcn_graph(data, x.shape[0], names, tensors)
         return Fn.GraphBranchFn.apply(x, graph, cfg, E.precision(self.precision), self.training, "gcn", "gnn.", names,
                                       *tensors)
+
+
+def _gcn_graph(data, n, names, tensors):
+    """The mode-1 Graph of data.graph: weighted when data.graph['edge_weight'] is set (models.GCN passes it to every conv but the
+    last, medium/models.py:53-62); the weight then joins the autograd inputs under engine.EDGE_WEIGHT."""
+    w = data.graph.get('edge_weight', None)
+    if w is None:
+        return get_graph(data.graph['edge_index'], n, 1), names, tensors
+    return get_graph(data.graph['edge_index'], n, 1, edge_weight=w), tuple(names) + (E.EDGE_WEIGHT,), list(tensors) + [w]
 
 
 def _is_gcn_like(gnn) -> bool:
@@ -239,9 +246,9 @@ class GAT(_Base):
 
 
 def _check_gat_data(data):
-    for k in ('edge_weight', 'edge_attr'):
-        if data.graph.get(k, None) is not None:
-            raise NotImplementedError(f"sgformer_b200.GAT: {k} is not supported")
+    # models.GAT never reads edge_weight (medium/models.py:145-155): it is ignored here as well
+    if data.graph.get('edge_attr', None) is not None:
+        raise NotImplementedError("sgformer_b200.GAT: edge_attr is not supported")
 
 
 def _gat_flat(gnn, prefix):
@@ -296,7 +303,7 @@ class SGFormer(SGFormerBase):
             raise RuntimeError("sgformer_b200.SGFormer (medium) needs the dataset on a CUDA device (no CPU fallback)")
         prec = E.precision(self.precision)
         fused = bool(self.use_graph) and self.gnn is not None and _is_gcn_like(self.gnn) and \
-            data.graph.get('edge_weight', None) is None and _gcn_out_dim(self.gnn) == self._io[1]
+            _gcn_out_dim(self.gnn) == self._io[1]
         tn, tt = self.trans_conv._flat("trans_conv.")
         fn, ft = self.fc._parameters.keys(), list(self.fc._parameters.values())
         names = list(tn) + ["fc." + k for k in fn]
@@ -315,7 +322,12 @@ class SGFormer(SGFormerBase):
             gn, gt = _gcn_flat(self.gnn, "gnn.")
             cfg = self._cfg(len(self.gnn.convs), float(self.gnn.dropout), bool(self.gnn.use_bn))
             comm = self._comm
-            graph = get_graph(edge_index, comm.n_global, 1, rows=comm.rows, col_rot=comm.col_rot) if comm.active else get_graph(edge_index, x.shape[0], 1)
+            if comm.active:
+                if data.graph.get('edge_weight', None) is not None:
+                    raise NotImplementedError("sgformer_b200: row sharding of a weighted graph (edge_weight) is not supported")
+                graph = get_graph(edge_index, comm.n_global, 1, rows=comm.rows, col_rot=comm.col_rot)
+            else:
+                graph, gn, gt = _gcn_graph(data, x.shape[0], gn, gt)
             return Fn.SGFormerFn.apply(x, graph, cfg, prec, self.training, comm, tuple(names) + tuple(gn), *tensors, *gt)
         # foreign GNN module: run it as given, mix + fc on the GPU kernels
         x1 = Fn.TransConvFn.apply(x, self.trans_conv._cfg(), prec, self.training, tn, *tt)
