@@ -262,22 +262,23 @@ def graph_conv(x: Tensor, edge_index: Tensor, sd: Dict[str, Tensor], cfg: dict, 
 # GCN backbone, medium  (medium/models.py:14-63 on top of PyG GCNConv / gcn_norm)
 # --------------------------------------------------------------------------------------------
 
-def pyg_gcn_adjacency(edge_index: Tensor, n: int, edge_weight: Optional[Tensor] = None) -> Tensor:
+def pyg_gcn_adjacency(edge_index: Tensor, n: int, edge_weight: Optional[Tensor] = None, dtype=torch.float32) -> Tensor:
     """PyG gcn_norm(add_self_loops=True, improved=False): drop existing self loops, add one unit
     self loop per node (existing self-loop weights are kept when edge_weight is given),
     deg = scatter-add of weights at `col`, w_e = deg^-1/2[row] w_e deg^-1/2[col] (inf -> 0).
-    Aggregation is out[col] += w_e x[row]  ->  CSR with row index = col."""
+    Aggregation is out[col] += w_e x[row]  ->  CSR with row index = col.
+    PyG computes in fp32; `dtype` = fp64 only for accuracy studies in tests."""
     row, col = edge_index[0], edge_index[1]
-    w = torch.ones(row.numel(), dtype=torch.float32) if edge_weight is None else edge_weight.to(torch.float32)
+    w = torch.ones(row.numel(), dtype=dtype) if edge_weight is None else edge_weight.to(dtype)
     keep = row != col
-    loop_w = torch.ones(n, dtype=torch.float32)
+    loop_w = torch.ones(n, dtype=dtype)
     if edge_weight is not None:
         loop_w[row[~keep]] = w[~keep]
     ar = torch.arange(n, dtype=row.dtype)
     row = torch.cat([row[keep], ar])
     col = torch.cat([col[keep], ar])
     w = torch.cat([w[keep], loop_w])
-    deg = torch.zeros(n, dtype=torch.float32).scatter_add_(0, col, w)
+    deg = torch.zeros(n, dtype=dtype).scatter_add_(0, col, w)
     dis = deg.pow(-0.5)
     dis = torch.where(torch.isinf(dis), torch.zeros_like(dis), dis)
     w = dis[row] * w * dis[col]
@@ -290,9 +291,9 @@ def gcn_medium(x: Tensor, edge_index: Tensor, sd: Dict[str, Tensor], cfg: dict, 
     """models.GCN.forward (medium/models.py:49-63): GCNConv = (x W^T) then Â·, + bias; BN/ReLU/dropout
     between layers, none after the last."""
     n = x.shape[0]
-    adj = pyg_gcn_adjacency(edge_index, n, edge_weight)
+    adj = pyg_gcn_adjacency(edge_index, n, edge_weight, x.dtype)
     # quirk kept: the last conv is called without edge_weight (medium/models.py:62)
-    adj_last = adj if edge_weight is None else pyg_gcn_adjacency(edge_index, n, None)
+    adj_last = adj if edge_weight is None else pyg_gcn_adjacency(edge_index, n, None, x.dtype)
     nl = cfg["gcn_num_layers"]
     for i in range(nl):
         a = adj_last if i == nl - 1 else adj

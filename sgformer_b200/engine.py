@@ -92,6 +92,17 @@ def _w(P: Dict[str, Tensor], name: str, prec: Precision, transpose: bool = False
     return K.pack_operand(P[name], transpose, prec.planes)
 
 
+def _b_blocks(w: Tensor, widths, prec: Precision):
+    """B side of a GEMM that contracts each column block (of `widths`) of w [n_out, sum(widths)] with an A source of its own
+    -> (operands, [(operand index, K offset)] per block).  A TMA load starts on a 16-byte boundary, so a block must start at a
+    multiple of 8 bf16 columns of its operand (K.gemm_nt refuses anything else).  Where one does not (fp32 widths such as
+    h = 100), every block is packed as an operand of its own and read from offset 0."""
+    offs = [sum(widths[:j]) for j in range(len(widths))]
+    if all(o % 8 == 0 for o in offs):
+        return [K.pack_operand(w, False, prec.planes)], [(0, o) for o in offs]
+    return [K.pack_operand(w[:, o:o + k], False, prec.planes) for o, k in zip(offs, widths)], [(j, 0) for j in range(len(widths))]
+
+
 _xin_cache: "OrderedDict[tuple, tuple]" = OrderedDict()
 
 
@@ -256,8 +267,9 @@ def attention_gram_backward(P: Dict[str, Tensor], lp: str, tape: Tape, x: Tensor
     K.gemm_tn(xop, gnum_op, pmat)
     comm.allreduce_(pmat, pg, cs, sg)                         # C2
     dwq, dbq, dwk, dbk, dwv, dbv, bcat, a4 = K.attn_gram_prepare_bwd(st, pmat, pg, cs, sg)
-    A, B = [gnum_op, xop], [K.pack_operand(bcat, False, prec.planes)]
-    pairs = [(0, 0, 0, 0, d), (1, 0, 0, d, h)]
+    B, at = _b_blocks(bcat, [d, h], prec)
+    A = [gnum_op, xop]
+    pairs = [(0, 0, at[0][0], at[0][1], d), (1, 0, at[1][0], at[1][1], h)]
     if dv is not None:
         dv_op = K.as_operand(dv, prec.planes)
         if use_weight:
@@ -266,7 +278,7 @@ def attention_gram_backward(P: Dict[str, Tensor], lp: str, tape: Tape, x: Tensor
         A.append(dv_op)
         B.append(K.pack_operand(P[lp + "Wv.weight"] if use_weight else _identity_v(h, dev)[0], True, prec.planes))
         if prec.planes == 1:            # dv Wv as a third segment of the dx GEMM
-            pairs.append((2, 0, 1, 0, d))
+            pairs.append((2, 0, len(B) - 1, 0, d))
     grads[lp + "Wq.weight"], grads[lp + "Wq.bias"] = dwq, dbq
     grads[lp + "Wk.weight"], grads[lp + "Wk.bias"] = dwk, dbk
     names = [lp + "Wq.weight", lp + "Wq.bias", lp + "Wk.weight", lp + "Wk.bias"]
@@ -276,7 +288,7 @@ def attention_gram_backward(P: Dict[str, Tensor], lp: str, tape: Tape, x: Tensor
     _mark_global(grads, comm, *names)          # built from all-reduced contractions: already global sums
     K.gemm_nt(A, B, pairs, h, dprev, bias=a4, r1_row=gden, r1_col=st.tail[0], accumulate=accumulate)
     if dv is not None and prec.planes != 1:     # bf16x3: 3 x 6 partial products exceed the GEMM's 16 segments
-        K.gemm_nt([A[2]], [B[1]], [(0, 0, 0, 0, d)], h, dprev, accumulate=True)
+        K.gemm_nt([A[2]], [B[-1]], [(0, 0, 0, 0, d)], h, dprev, accumulate=True)
 
 
 # =================================================================================================
@@ -531,9 +543,9 @@ def gconv_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, t
         y = comm.spmm_gathered(K, graph, False, dinv, cur_s)    # C4: operand rows of every shard
         st = _stat_bufs(use_bn, training, h, dev)      # BatchNorm sums come out of the GEMM epilogue
         if use_init:
-            w = _w(P, f"{pfx}convs.{i}.W.weight", prec)
-            z = K.gemm_nt([K.as_operand(y, prec.planes, memo=True), K.as_operand(x0, prec.planes, memo=True)], [w],
-                          [(0, 0, 0, 0, h), (1, 0, 0, h, h)], h, K.new_like(y), bias=P[f"{pfx}convs.{i}.W.bias"],
+            w, at = _b_blocks(P[f"{pfx}convs.{i}.W.weight"], [h, h], prec)
+            z = K.gemm_nt([K.as_operand(y, prec.planes, memo=True), K.as_operand(x0, prec.planes, memo=True)], w,
+                          [(0, 0, at[0][0], at[0][1], h), (1, 0, at[1][0], at[1][1], h)], h, K.new_like(y), bias=P[f"{pfx}convs.{i}.W.bias"],
                           col_sum=st[0], col_sumsq=st[1])
         elif use_weight:
             w = _w(P, f"{pfx}convs.{i}.W.weight", prec)
@@ -583,9 +595,9 @@ def gconv_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: P
                                     L["rstd"], P.get(name + "weight"), P.get(name + "bias"), None, use_bn, use_act, training,
                                     p, seed + _SEED_GCONV_LAYER + i, gs, dres=dx0 if use_res else None, dres_accumulate=res_acc,
                                     want_dz_colsum=use_init or use_weight, reduce_fn=red, stat_rows=nstat)
-        gs = 1.0
         if use_bn:
-            _bn_param_grads(grads, comm, P, name, sums, dy_plain, dy_scaled, dinv, L["z"], L["mean"], L["rstd"], use_act)
+            _bn_param_grads(grads, comm, P, name, sums, dy_plain, dy_scaled, dinv, L["z"], L["mean"], L["rstd"], use_act, gs)
+        gs = 1.0
         if use_init or use_weight:
             wname = f"{pfx}convs.{i}.W.weight"
             dz_op = K.as_operand(dz, prec.planes)
@@ -621,7 +633,8 @@ def gconv_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: P
                                  tape["rstd0"], P.get(pfx + "bns.0.weight"), P.get(pfx + "bns.0.bias"), None, use_bn, True,
                                  training, p, seed + _SEED_GCONV_STEM, gs, want_dz_colsum=True, reduce_fn=red, stat_rows=nstat)
     if use_bn:
-        _bn_param_grads(grads, comm, P, pfx + "bns.0.", sums, g_plain, g_scaled, dinv, tape["z0"], tape["mean0"], tape["rstd0"], True)
+        _bn_param_grads(grads, comm, P, pfx + "bns.0.", sums, g_plain, g_scaled, dinv, tape["z0"], tape["mean0"], tape["rstd0"], True,
+                        gs)
     dz0_op = K.as_operand(dz0, prec.planes)
     dw0 = torch.empty((h, d_in), dtype=torch.float32, device=dev)
     K.gemm_tn(dz0_op, tape["xin"], dw0)
@@ -641,13 +654,13 @@ def _mark_global(grads: dict, comm: Comm, *names: str):
 
 
 def _bn_param_grads(grads: dict, comm: Comm, P, name: str, sums: Optional[Tensor], dy, dy2, dinv, z: Tensor, mean, rstd,
-                    use_relu: bool):
+                    use_relu: bool, gscale: float = 1.0, zbias: Optional[Tensor] = None):
     """Stores the affine gradients of the BatchNorm `name`.  Training: `sums` = (sum g, sum g*xhat) from bn_bwd, which
     all-reduced them between its phases.  Eval (sums is None; rare: eval-mode backward): computed here from the running
-    statistics and the gradient (dy, dy2) that entered bn_bwd."""
+    statistics and the gradient gscale * (dy, dy2) that entered bn_bwd; `zbias` = the bias bn_fwd added to z (GCN layers)."""
     if sums is None:
-        sums = K.bn_bwd_sums(dy, dy2, dinv if dy2 is not None else None, z, mean, rstd, P[name + "weight"], P[name + "bias"], None,
-                             True, use_relu, 0.0, 0, 1.0)
+        sums = K.bn_bwd_sums(dy, dy2, dinv if dy2 is not None else None, z, mean, rstd, P[name + "weight"], P[name + "bias"], zbias,
+                             True, use_relu, 0.0, 0, gscale)
     else:
         _mark_global(grads, comm, name + "bias", name + "weight")
     h = z.shape[1]
@@ -759,8 +772,8 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
             dzs, sums, colsum = K.bn_bwd(dcur, None, None, L["s"], L.get("mean"), L.get("rstd"), P.get(name + "weight"),
                                          P.get(name + "bias"), zb, use_bn, True, training, p, seed + _SEED_GCN_LAYER + i, gs,
                                          want_dz_colsum=zb is not None, out_row_scale=dinv, reduce_fn=red, stat_rows=nstat)
-            if use_bn and training:     # not in eval: those sums would also need the conv bias (zbias) the eval path omits
-                _bn_param_grads(grads, comm, P, name, sums, dcur, None, None, L["s"], L["mean"], L["rstd"], True)
+            if use_bn:
+                _bn_param_grads(grads, comm, P, name, sums, dcur, None, None, L["s"], L["mean"], L["rstd"], True, gs, zb)
         gs = 1.0
         if zb is not None:
             grads[f"{pfx}convs.{i}.bias"] = colsum
@@ -934,12 +947,12 @@ def head_forward(P, cfg: dict, feats: List[Tensor], prec: Precision, tape: Optio
     pfx: the Linear's parameter prefix (DIFFormer's output Linear is "fcs.1.")."""
     h, c = cfg["hidden"], cfg["out_channels"]
     n = feats[0].shape[0]
-    w = _w(P, pfx + "weight", prec)
+    w, at = _b_blocks(P[pfx + "weight"], [h] * len(feats), prec)
     ops = [K.as_operand(f, prec.planes) for f in feats]
-    pairs = [(j, 0, 0, j * h, h) for j in range(len(feats))]
+    pairs = [(j, 0, at[j][0], at[j][1], h) for j in range(len(feats))]
     # pitch padded to a 16-byte multiple (c = 47 -> 48 floats): the GEMM epilogue can then use its TMA-store path
     out = K.alloc_act(n, c, torch.float32, feats[0].device)
-    K.gemm_nt(ops, [w], pairs, c, out, bias=P[pfx + "bias"])
+    K.gemm_nt(ops, w, pairs, c, out, bias=P[pfx + "bias"])
     if tape is not None:
         tape.update(ops=ops, nfeat=len(feats))
     return out

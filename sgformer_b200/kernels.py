@@ -621,6 +621,8 @@ def gemm_nt(A: Sequence[Operand], B: Sequence[Operand], pairs: Sequence[Tuple[in
     segs = []
     combos = _PAIRS3 if planes == 3 else [(0, 0)]
     for (ai, ak, bi, bk, klen) in pairs:
+        if ak % 8 or bk % 8:       # a TMA load starts on a 16-byte boundary; elsewhere its barrier never completes
+            raise ValueError(f"gemm_nt: K offsets must be multiples of 8 columns, got {ak} / {bk}")
         for (pa, pb) in combos:
             segs.append((ai, pa * A[ai].kp + ak, bi, pb * B[bi].kp + bk, klen))
     if len(segs) > _lib.SGF_MAX_SEG:
