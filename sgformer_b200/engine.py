@@ -130,52 +130,63 @@ def input_operand(x: Tensor, prec: Precision) -> K.Operand:
 # linear attention core (full_attention_conv)
 # =================================================================================================
 def attention_forward(q: Tensor, k: Tensor, v: Tensor, heads: int, prec: Precision, tape: Optional[Tape],
-                      comm: Comm = SINGLE, stats=None) -> Tensor:
+                      comm: Comm = SINGLE, stats=None, shared_v: bool = False) -> Tensor:
     """q,k: [N, H*M], v: [N, H*D] activations (views allowed) -> o [N, H*D].  medium/ours.py:14-34.
     One Frobenius norm over all heads (medium/ours.py:16-17); N is the query count (the GLOBAL node count when the rows
-    are sharded: the un-normalised partials {S', z', ||q||^2, ||k||^2} are all-reduced once, C1)."""
+    are sharded: the un-normalised partials {S', z', ||q||^2, ||k||^2} are all-reduced once, C1).
+    shared_v: v is [N, D], one value for every head (the reference's one-head vs broadcast by einsum, medium/ours.py:21-23)."""
     n_loc = q.shape[0]
     n = comm.n_global if comm.active else n_loc
     m = q.shape[1] // heads
-    d = v.shape[1] // heads
+    d = v.shape[1] if shared_v else v.shape[1] // heads
     dev = q.device
     if stats is not None:        # (sum of squares of q columns, column sums of k, sum of squares of k columns) from the
         sq_q, z_raw, sq_k = stats    # producing GEMM's epilogue
     else:
         _, sq_q = K.colstats(q, want_sum=False)
         z_raw, sq_k = K.colstats(k)
-    s_list = []
-    for hd in range(heads):
-        kh, vh = k[:, hd * m:(hd + 1) * m], v[:, hd * d:(hd + 1) * d]
-        s_raw = torch.empty((m, d), dtype=torch.float32, device=dev)
-        K.gemm_tn(K.as_operand(kh, prec.planes, memo=True), K.as_operand(vh, prec.planes, memo=True), s_raw)
-        s_list.append(s_raw)
-    comm.allreduce_(sq_q, z_raw, sq_k, *s_list)
+    if shared_v:            # S'_h = k_h^T v of every head in one GEMM: [H*M, D], k and v read once
+        s_all = torch.empty((heads * m, d), dtype=torch.float32, device=dev)
+        K.gemm_tn(K.as_operand(k, prec.planes, memo=True), K.as_operand(v, prec.planes, memo=True), s_all)
+        s_list = list(s_all.split(m))
+        comm.allreduce_(sq_q, z_raw, sq_k, s_all)
+    else:
+        s_list = []
+        for hd in range(heads):
+            kh, vh = k[:, hd * m:(hd + 1) * m], v[:, hd * d:(hd + 1) * d]
+            s_raw = torch.empty((m, d), dtype=torch.float32, device=dev)
+            K.gemm_tn(K.as_operand(kh, prec.planes, memo=True), K.as_operand(vh, prec.planes, memo=True), s_raw)
+            s_list.append(s_raw)
+        comm.allreduce_(sq_q, z_raw, sq_k, *s_list)
     o = K.alloc_act(n_loc, heads * d, q.dtype, dev)
     den = torch.empty((heads, n_loc), dtype=torch.float32, device=dev)
     scal = None
     for hd in range(heads):
-        qh, vh = q[:, hd * m:(hd + 1) * m], v[:, hd * d:(hd + 1) * d]
+        qh, vh = q[:, hd * m:(hd + 1) * m], v if shared_v else v[:, hd * d:(hd + 1) * d]
         bmat, btail, scal = K.attn_prepare_fwd(s_list[hd], z_raw[hd * m:(hd + 1) * m], sq_q, sq_k, prec.planes)
         K.gemm_nt([K.as_operand(qh, prec.planes, memo=True)], [bmat], [(0, 0, 0, 0, m)], d, o[:, hd * d:(hd + 1) * d],
                   epi=EPI_ATTN_APPLY, aux=vh, tail=btail, nf=float(n), den_out=den[hd])
     if tape is not None:
-        tape.update(q=q, k=k, v=v, o=o, den=den, s=s_list, z=z_raw, scal=scal, heads=heads, m=m, d=d, n=n)
+        tape.update(q=q, k=k, v=v, o=o, den=den, s=s_list, z=z_raw, scal=scal, heads=heads, m=m, d=d, n=n, shared_v=shared_v)
     return o
 
 
 def attention_backward(tape: Tape, g: Tensor, gscale: float, prec: Precision, dq: Tensor, dk: Tensor,
                        dv: Optional[Tensor], dv_accumulate: bool = False, comm: Comm = SINGLE):
-    """g = dL/do [N, H*D] (times gscale).  Writes dq, dk [N, H*M] and dv [N, H*D] (+= if dv_accumulate).
+    """g = dL/do [N, H*D] (times gscale), or [N, D] when every head receives the same gradient (the head mean's backward).
+    Writes dq, dk [N, H*M] and dv [N, H*D] (+= if dv_accumulate).  With a shared v (attention_forward(shared_v=True)) dv is
+    [N, D]: the heads' contributions are summed into it in head order (the first one += only if dv_accumulate).
     SURVEY.md Appendix A.1 in the raw-q/k form documented at sgf_attn_prepare_bwd; row-sharded: {dS', dz'} all-reduced (C2)."""
     q, k, v, o, den = tape["q"], tape["k"], tape["v"], tape["o"], tape["den"]
     heads, m, d, n = tape["heads"], tape["m"], tape["d"], tape["n"]
+    shared_v = tape.get("shared_v", False)
+    shared_g = g.shape[1] == d
     dev = q.device
     scal_bwd = torch.zeros((heads, 8), dtype=torch.float32, device=dev)
     part = []
     for hd in range(heads):
         qh = q[:, hd * m:(hd + 1) * m]
-        gnum, gden = K.attn_bwd_prep(g[:, hd * d:(hd + 1) * d], o[:, hd * d:(hd + 1) * d], den[hd], gscale)
+        gnum, gden = K.attn_bwd_prep(g if shared_g else g[:, hd * d:(hd + 1) * d], o[:, hd * d:(hd + 1) * d], den[hd], gscale)
         gnum_op = K.as_operand(gnum, prec.planes)
         ds_raw = torch.empty((m, d), dtype=torch.float32, device=dev)
         K.gemm_tn(K.as_operand(qh, prec.planes, memo=True), gnum_op, ds_raw)
@@ -192,15 +203,17 @@ def attention_backward(tape: Tape, g: Tensor, gscale: float, prec: Precision, dq
         K.attn_combine_scal(scal_bwd, heads, tape["scal"])
     for hd in range(heads):
         gnum, gden, gnum_op, (b_dq, b_dv, b_dk, r1_col, dk_bias) = per_head[hd]
-        qh, kh, vh = q[:, hd * m:(hd + 1) * m], k[:, hd * m:(hd + 1) * m], v[:, hd * d:(hd + 1) * d]
+        qh, kh = q[:, hd * m:(hd + 1) * m], k[:, hd * m:(hd + 1) * m]
+        vh = v if shared_v else v[:, hd * d:(hd + 1) * d]
         sb = scal_bwd[hd]
         K.gemm_nt([gnum_op], [b_dq], [(0, 0, 0, 0, d)], m, dq[:, hd * m:(hd + 1) * m], alpha_dev=sb[0:1], aux=qh, beta=1.0,
                   beta_dev=sb[1:2], r1_row=gden, r1_col=r1_col)
         K.gemm_nt([K.as_operand(vh, prec.planes, memo=True)], [b_dk], [(0, 0, 0, 0, d)], m, dk[:, hd * m:(hd + 1) * m], alpha_dev=sb[0:1],
                   aux=kh, beta=1.0, beta_dev=sb[2:3], bias=dk_bias)
         if dv is not None:
-            K.gemm_nt([K.as_operand(kh, prec.planes, memo=True)], [b_dv], [(0, 0, 0, 0, m)], d, dv[:, hd * d:(hd + 1) * d],
-                      alpha_dev=sb[0:1], aux=gnum, beta=float(n), accumulate=dv_accumulate)
+            K.gemm_nt([K.as_operand(kh, prec.planes, memo=True)], [b_dv], [(0, 0, 0, 0, m)], d,
+                      dv if shared_v else dv[:, hd * d:(hd + 1) * d], alpha_dev=sb[0:1], aux=gnum, beta=float(n),
+                      accumulate=dv_accumulate or (shared_v and hd > 0))
 
 
 # =================================================================================================
@@ -369,8 +382,6 @@ def trans_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precisi
         tape.update(xin=xin, t0=t0, st0=st, layers=[], p=p, seed=seed, n=xin.rows)
     ca, cb, use_res = _res_coef(cfg)
     use_weight = bool(cfg["trans_use_weight"])
-    if not use_weight and H != 1:
-        raise ValueError("use_weight=False requires num_heads == 1 (medium/ours.py:84)")
     for i in range(cfg["trans_num_layers"]):
         lp = f"{pfx}convs.{i}."
         at = Tape() if tape is not None else None
@@ -378,10 +389,13 @@ def trans_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precisi
             a = attention_gram_forward(P, lp, x, use_weight, prec, at, comm)
             saved = dict(gram=True)
         else:
-            # K^T 1, ||Q||^2, ||K||^2 fall out of the projection's epilogue
+            # K^T 1, ||Q||^2, ||K||^2 fall out of the projection's epilogue.  use_weight=False: every head attends over the
+            # layer input itself (the reference's one-head V broadcast across heads, medium/ours.py:84 and :21-23)
             qkv, csum, csq = _project_qkv(P, lp, K.as_operand(x, prec.planes, memo=True), use_weight, prec, stats=True)
-            q, k, v = qkv[:, :H * h], qkv[:, H * h:2 * H * h], qkv[:, 2 * H * h:]
-            o = attention_forward(q, k, v, H, prec, at, comm, stats=(csq[:H * h], csum[H * h:2 * H * h], csq[H * h:2 * H * h]))
+            q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
+            v = qkv[:, 2 * H * h:] if use_weight else x
+            o = attention_forward(q, k, v, H, prec, at, comm, stats=(csq[:H * h], csum[H * h:2 * H * h], csq[H * h:2 * H * h]),
+                                  shared_v=not use_weight)
             a = K.head_mean(o, H, h)
             saved = dict(nout=qkv.shape[1])
         y, st = K.ln_fwd(a, x if use_res else None, ca, cb, P.get(f"{pfx}bns.{i + 1}.weight"), P.get(f"{pfx}bns.{i + 1}.bias"),
@@ -414,7 +428,7 @@ def trans_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Prec
         q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
         v = qkv[:, 2 * H * h:] if use_weight else x
         at = Tape()
-        o = attention_forward(q, k, v, H, prec, at)
+        o = attention_forward(q, k, v, H, prec, at, shared_v=not use_weight)
         inv_norm = at["den"].mean(dim=0).reciprocal_().contiguous()       # [N]: 1 / mean_h(den_h)  (an [N]-vector; not a hot path)
         att = K.alloc_act(n, n, torch.float32, dev)
         K.gemm_nt([K.as_operand(q, prec.planes)], [K.as_operand(k, prec.planes)], [(0, 0, 0, 0, H * h)], n, att, alpha=1.0 / H,
@@ -448,23 +462,28 @@ def trans_backward(P, cfg: dict, tape: Tape, dout: Tensor, gscale: float, prec: 
                                                        seed + _SEED_LAYER + i, gs, use_res, dg, db, at["den"])
             dprev = dr if dr is not None else K.new_like(x_in)
             attention_gram_backward(P, lp, at, x_in, gnum, gden, cs, pg, sg, use_weight, prec, dprev, dr is not None, grads, comm)
-        else:       # materialised q, k, v: several heads, so use_weight is set
+        else:       # materialised q, k (and v with use_weight): several heads
             nout = L["nout"]
             da, dr = K.ln_bwd(dcur, L["a"], x_in if use_res else None, ca, cb, P.get(bn + "weight"), P.get(bn + "bias"), L["st"],
                               use_ln, bool(cfg["trans_use_act"]), p, seed + _SEED_LAYER + i, gs, use_res, dg, db)
-            # head mean: every head receives da / H; da has pitch h, per-head slices of g are the same columns for all heads
             dqkv = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
             dprev = dr if dr is not None else K.new_like(x_in)
-            attention_backward(at, _tile_heads(da, H), 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h],
-                               dqkv[:, 2 * H * h:], comm=comm)
+            if use_weight:
+                # head mean: every head receives da / H; da has pitch h, per-head slices of g are the same columns for all heads
+                attention_backward(at, _tile_heads(da, H), 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h],
+                                   dqkv[:, 2 * H * h:], comm=comm)
+            else:
+                # shared value v = x_in: every head reads the same da / H, and the heads' dv sum into dprev in head order
+                attention_backward(at, da, 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:], dprev, dv_accumulate=dr is not None,
+                                   comm=comm)
             wcat, _ = _qkv_weight(P, lp, use_weight)
             dqkv_op = K.as_operand(dqkv, prec.planes)
             K.gemm_nt([dqkv_op], [K.pack_operand(wcat, True, prec.planes)], [(0, 0, 0, 0, nout)], h, dprev,
-                      accumulate=dr is not None)
+                      accumulate=dr is not None or not use_weight)
             dw = torch.empty((nout, h), dtype=torch.float32, device=dev)
             K.gemm_tn(dqkv_op, K.as_operand(x_in, prec.planes, memo=True), dw)
             dbias, _ = K.colstats(dqkv, want_sumsq=False)
-            for j, nm in enumerate(("Wq", "Wk", "Wv")):
+            for j, nm in enumerate(("Wq", "Wk", "Wv")[:nout // (H * h)]):
                 grads[lp + nm + ".weight"] = dw[j * H * h:(j + 1) * H * h]
                 grads[lp + nm + ".bias"] = dbias[j * H * h:(j + 1) * H * h]
         if use_ln:

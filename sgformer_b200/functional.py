@@ -259,32 +259,36 @@ class HeadFn(Function):
 
 
 class AttentionFn(_TapeFunction):
-    """full_attention_conv(qs, ks, vs) -> [N, H, D]  (medium/ours.py:14-34, 100M/ours.py:12-43)."""
+    """full_attention_conv(qs, ks, vs) -> [N, H, D]  (medium/ours.py:14-34, 100M/ours.py:12-43).  A one-head vs [N, 1, D]
+    is shared by all H heads, as the reference's einsum broadcasts it; its gradient is the sum over the heads."""
 
     @staticmethod
     def forward(ctx, q, k, v, prec):
         n, heads, m = q.shape
-        d = v.shape[2]
+        vh, d = v.shape[1], v.shape[2]
+        if k.shape != q.shape or v.shape[0] != n or vh not in (1, heads):
+            raise ValueError(f"full_attention_conv: qs {tuple(q.shape)}, ks {tuple(k.shape)}, vs {tuple(v.shape)}: ks must match qs "
+                             f"and vs must have {n} rows and 1 or {heads} heads")
         qa, ka, va = (_to_act(t.reshape(n, -1), prec) for t in (q, k, v))
         need = _want_tape(ctx)
         tape = E.Tape() if need else None
-        o = E.attention_forward(qa, ka, va, heads, prec, tape)
+        o = E.attention_forward(qa, ka, va, heads, prec, tape, shared_v=vh != heads)
         if need:
-            ctx.state = (prec, tape, q.dtype, k.dtype, v.dtype, heads, m, d)
+            ctx.state = (prec, tape, q.dtype, k.dtype, v.dtype, heads, vh, m, d)
         return _from_act(o, q.dtype).reshape(n, heads, d)
 
     @staticmethod
     def backward(ctx, g):
-        prec, tape, dtq, dtk, dtv, heads, m, d = ctx.state
+        prec, tape, dtq, dtk, dtv, heads, vh, m, d = ctx.state
         n = g.shape[0]
         ga = _to_act(g.reshape(n, heads * d), prec)
         dq = K.alloc_act(n, heads * m, prec.act_dtype, g.device)
         dk = K.alloc_act(n, heads * m, prec.act_dtype, g.device)
-        dv = K.alloc_act(n, heads * d, prec.act_dtype, g.device)
+        dv = K.alloc_act(n, vh * d, prec.act_dtype, g.device)
         E.attention_backward(tape, ga, 1.0, prec, dq, dk, dv)
         ctx.state = None
         return (_from_act(dq, dtq).reshape(n, heads, m), _from_act(dk, dtk).reshape(n, heads, m),
-                _from_act(dv, dtv).reshape(n, heads, d), None)
+                _from_act(dv, dtv).reshape(n, vh, d), None)
 
 
 class LinearFn(Function):

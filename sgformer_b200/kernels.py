@@ -909,9 +909,19 @@ def axpby(x: Tensor, y: Optional[Tensor], a: float, b: float, out_dtype=None, ro
     return out
 
 
+def _heads_fit(x: Tensor, heads: int, d: int, name: str):
+    """Kernels that take a head count read `heads` blocks of d columns from every row of x: refuse a narrower x (the kernel
+    would read past the end of the row, or of the allocation)."""
+    rows, cols, ld = _mat(x, name)
+    if heads < 1 or d < 1 or cols < heads * d:
+        raise ValueError(f"{name}: {cols} columns, but {heads} heads of width {d} need {heads * d}")
+    return rows, cols, ld
+
+
 def head_mean(x: Tensor, heads: int, d: int) -> Tensor:
+    """x [N, >= heads*d] -> [N, d]: the mean of the heads' column blocks."""
     _use(x)
-    rows, _, ld = _mat(x, "x")
+    rows, _, ld = _heads_fit(x, heads, d, "x")
     out = alloc_act(rows, d, x.dtype, x.device)
     check(lib().sgf_head_mean(_p(x), ld, rows, heads, d, dcode(x), _p(out), out.stride(0), _stream()), "sgf_head_mean")
     return out
@@ -927,7 +937,7 @@ GAT_MAX_HEADS = 8    # SGF_GAT_MAX_HEADS
 def gat_logits(xp: Tensor, heads: int, c: int, att_src: Tensor, att_dst: Tensor) -> Tuple[Tensor, Tensor]:
     """xp [N, heads*c] -> (a_src, a_dst) fp32 [N, heads]."""
     _use(xp)
-    n, _, ld = _mat(xp, "xp")
+    n, _, ld = _heads_fit(xp, heads, c, "xp")
     a_src = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
     a_dst = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
     check(lib().sgf_gat_logits(_p(xp), ld, n, heads, c, dcode(xp), _p(_f32vec(att_src, heads * c, "att_src")),
@@ -939,7 +949,7 @@ def gat_fwd(rowptr: Tensor, col: Tensor, xp: Tensor, a_src: Tensor, a_dst: Tenso
             bias: Optional[Tensor], p: float, seed: int) -> Tuple[Tensor, Tensor]:
     """-> (out [N, c] if mean else [N, heads*c] in xp's dtype, lse fp32 [N, heads]).  See sgf_gat_fwd."""
     _use(xp)
-    n, _, ld = _mat(xp, "xp")
+    n, _, ld = _heads_fit(xp, heads, c, "xp")
     out = alloc_act(n, c if mean else heads * c, xp.dtype, xp.device)
     lse = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
     check(lib().sgf_gat_fwd(_p(rowptr), _p(col), _p(xp), ld, _p(a_src), _p(a_dst), n, heads, c, dcode(xp), int(mean),
@@ -952,8 +962,8 @@ def gat_bwd(rowptr: Tensor, col: Tensor, rowptr_t: Tensor, col_t: Tensor, xp: Te
             g: Tensor, att_src: Tensor, att_dst: Tensor, heads: int, c: int, mean: bool, p: float, seed: int):
     """g = dL/dout -> (dxp [N, heads*c] in xp's dtype, da_src fp32 [heads, N], da_dst fp32 [heads, N]).  See sgf_gat_bwd."""
     _use(xp)
-    n, _, ld = _mat(xp, "xp")
-    _, _, ldg = _mat(g, "g")
+    n, _, ld = _heads_fit(xp, heads, c, "xp")
+    _, _, ldg = _heads_fit(g, 1 if mean else heads, c, "g")
     if g.dtype != xp.dtype:
         raise TypeError("gat_bwd: g and xp must share the activation dtype")
     dev = xp.device
@@ -1032,6 +1042,8 @@ def attn_prepare_bwd(s_raw: Tensor, z_raw: Tensor, ds_raw: Tensor, dz_raw: Tenso
 
 def attn_combine_scal(scal_bwd_all: Tensor, heads: int, scal_fwd: Tensor):
     _use(scal_bwd_all)
+    if heads < 1 or scal_bwd_all.dim() != 2 or scal_bwd_all.shape[0] < heads or scal_bwd_all.shape[1] < 4:
+        raise ValueError(f"attn_combine_scal: scal_bwd_all {tuple(scal_bwd_all.shape)} holds fewer than {heads} rows of 4 scalars")
     check(lib().sgf_attn_combine_scal(_p(scal_bwd_all), heads, scal_bwd_all.stride(0), _p(scal_fwd), _stream()),
           "sgf_attn_combine_scal")
 

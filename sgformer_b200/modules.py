@@ -64,8 +64,8 @@ class _Base(nn.Module):
 # attention
 # =================================================================================================
 def full_attention_conv(qs: Tensor, ks: Tensor, vs: Tensor, output_attn: bool = False, precision: Optional[str] = None):
-    """Reference free function (medium/ours.py:14-46, 100M/ours.py:12-53): qs,ks [N,H,M], vs [N,H,D] -> [N,H,D]
-    (+ the [N,N] visualisation matrix when output_attn)."""
+    """Reference free function (medium/ours.py:14-46, 100M/ours.py:12-53): qs,ks [N,H,M], vs [N,H,D] or [N,1,D] (one value
+    shared by all heads) -> [N,H,D] (+ the [N,N] visualisation matrix when output_attn)."""
     if not qs.is_cuda:
         _require_cuda("full_attention_conv")
         raise RuntimeError("sgformer_b200.full_attention_conv needs CUDA tensors (no CPU fallback)")
@@ -110,9 +110,7 @@ class TransConvLayerBase(_Base):
         k = Fn.LinearFn.apply(source_input, self.Wk.weight, self.Wk.bias, prec).reshape(-1, self.num_heads, self.out_channels)
         if self.use_weight:
             v = Fn.LinearFn.apply(source_input, self.Wv.weight, self.Wv.bias, prec).reshape(-1, self.num_heads, self.out_channels)
-        else:
-            if self.num_heads != 1:
-                raise ValueError("use_weight=False requires num_heads == 1 (medium/ours.py:84: V is the single-head layer input)")
+        else:       # medium/ours.py:84: one value, the layer input, shared by every head
             v = source_input.reshape(-1, 1, self.out_channels)
         out = Fn.AttentionFn.apply(q, k, v, prec).mean(dim=1)
         if output_attn:
