@@ -916,19 +916,23 @@ def gat_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         last = i == nl - 1
         lp = f"{pfx}convs.{i}."
         H, C, cp = L["H"], L["C"], L["cp"]
+        db = None
         if last:
             g = K.axpby(dcur, None, gs, 0.0) if gs != 1.0 else dcur
         else:
+            # the bias gradient is the column sum of dz taken in fp32 inside bn_bwd: in bf16, summing the stored dz would add its
+            # rounding to a sum that a training BatchNorm makes exactly zero
             name = f"{pfx}bns.{i}."
-            g, sums, _ = K.bn_bwd(dcur, None, None, L["z"], L["mean"], L["rstd"], P.get(name + "weight"), P.get(name + "bias"), None,
-                                  use_bn, K.ACT_ELU, training, p, seed + _SEED_GAT_ACT + i, 1.0)
+            g, sums, db = K.bn_bwd(dcur, None, None, L["z"], L["mean"], L["rstd"], P.get(name + "weight"), P.get(name + "bias"), None,
+                                   use_bn, K.ACT_ELU, training, p, seed + _SEED_GAT_ACT + i, 1.0, want_dz_colsum=True)
             if use_bn and training:
                 _bn_param_grads(grads, comm, P, name, sums, dcur, None, None, L["z"], L["mean"], L["rstd"], K.ACT_ELU)
         if cp != C:            # zero-padded heads (see _gat_layer): the gradient of the padding columns is zero
             gp = torch.zeros((n, cp), dtype=g.dtype, device=dev)
             K.axpby(g, None, 1.0, 0.0, out=gp[:, :C])
             g = gp
-        db, _ = K.colstats(g, want_sumsq=False)
+        if db is None:
+            db, _ = K.colstats(g, want_sumsq=False)
         grads[lp + "bias"] = db if cp == C else db[:C]
         att_s, att_d = L["att"]
         xp = L["xp"]
