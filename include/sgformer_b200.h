@@ -166,6 +166,14 @@ int sgf_spmm_weighted(const int64_t* rowptr, const int32_t* col, const float* va
 int sgf_spmm_heavy_weighted(const int32_t* col, const float* val, const float* row_scale, const void* x, int64_t ldx, void* y,
                             int64_t ldy, int h, int dtype, const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg,
                             float* partial, const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, void* stream);
+/* Unscaled SpMM (GCNConv(normalize=False) of the large variant's GCN):  y[r,:] = sum_{j in row r} x[col[j], :]  over the CSR as
+ * built (duplicates kept, no self loops added), fp32 accumulation in CSR order; no row scale is read or applied.  The hub-row
+ * segment path likewise; otherwise as sgf_spmm / sgf_spmm_heavy. */
+int sgf_spmm_sum(const int64_t* rowptr, const int32_t* col, const void* x, int64_t ldx, void* y, int64_t ldy, int64_t n_rows, int h,
+                 int dtype, int64_t max_row_len, void* stream);
+int sgf_spmm_heavy_sum(const int32_t* col, const void* x, int64_t ldx, void* y, int64_t ldy, int h, int dtype,
+                       const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg, float* partial, const int64_t* heavy_rows,
+                       const int64_t* heavy_seg_ptr, int64_t n_heavy, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K12 — GAT edge softmax (replaces PyG GATConv's message passing as medium/models.py:116-155 uses it: per-edge logits, softmax

@@ -164,6 +164,8 @@ _SIGS = {
     "sgf_spmm_weighted": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, C.c_int, C.c_int, _i64, _vp]),
     "sgf_spmm_heavy_weighted": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, C.c_int, C.c_int, _vp, _vp, _i64, _vp, _vp, _vp,
                                           _i64, _vp]),
+    "sgf_spmm_sum": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _i64, _i64, C.c_int, C.c_int, _i64, _vp]),
+    "sgf_spmm_heavy_sum": (C.c_int, [_vp, _vp, _i64, _vp, _i64, C.c_int, C.c_int, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp]),
     "sgf_edge_weight_grad": (C.c_int, [_vp, _vp, _vp, _i64, C.c_int, C.c_int, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp,
                                        _vp, _i64, _vp, _vp, _vp]),
     "sgf_attn_prepare_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _i64, _vp, _i64, _vp, _i64, _i64,

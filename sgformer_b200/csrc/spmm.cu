@@ -19,6 +19,11 @@
 // (32 at a time, broadcast by shuffle like the column ids) and FMA it into the fp32 accumulation: nnz*8 index + value bytes
 // instead of nnz*4.  The dinv pre-scale by the producer and the row_scale post-scale stay as they are.  The value pointer is the
 // kernels' last parameter, so the unweighted instantiations compile to the same code as before.
+//
+// Unscaled sums (the large variant's GCNConv(normalize=False), DESIGN.md §4.11): the SCALED=false instantiations of the row kernel
+// and of the hub-row finalize kernel compute y[r,:] = sum_{j in row r} x[col[j], :] with no row_scale read and no multiply; the
+// segment kernel has no scale and is shared.  SCALED is the last template parameter and defaults to true, so the existing
+// instantiations compile to the same SASS as before.
 #include "common.cuh"
 #include "launch_count.h"
 #include "../../include/sgformer_b200.h"
@@ -230,7 +235,7 @@ spmm_range_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict_
     }
 }
 
-template <typename T, int CPL, bool FLAGS = false, bool WEIGHTED = false>
+template <typename T, int CPL, bool FLAGS = false, bool WEIGHTED = false, bool SCALED = true>
 __global__ void __launch_bounds__(kSpmmBlock, kMinBlocks)
 spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col, const float* __restrict__ row_scale,
                  const T* __restrict__ x, int64_t ldx, T* __restrict__ y, int64_t ldy, int64_t n_rows, int chunks, int lpr_log2,
@@ -300,7 +305,7 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
 #pragma unroll
                         for (int i = 0; i < VN; ++i) acc[c][i] += __shfl_xor_sync(0xffffffffu, acc[c][i], o);
                 }
-                const float rs = row_scale ? row_scale[r] : 1.0f;
+                const float rs = (SCALED && row_scale) ? row_scale[r] : 1.0f;
                 if (grp == 0) {
                     T* dst = y + r * ldy;
 #pragma unroll
@@ -308,7 +313,7 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
                         if (!cval[c]) continue;
                         float f[VN];
 #pragma unroll
-                        for (int i = 0; i < VN; ++i) f[i] = acc[c][i] * rs;
+                        for (int i = 0; i < VN; ++i) f[i] = SCALED ? acc[c][i] * rs : acc[c][i];
                         stg_na(dst + coff[c], Vec16<T>::pack(f));
                     }
                 }
@@ -342,7 +347,7 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
 #pragma unroll
                 for (int i = 0; i < VN; ++i) acc[c][i] += __shfl_xor_sync(0xffffffffu, acc[c][i], o);
         }
-        const float rs = row_scale ? row_scale[r] : 1.0f;
+        const float rs = (SCALED && row_scale) ? row_scale[r] : 1.0f;
         if (grp == 0) {
             T* dst = y + r * ldy;
 #pragma unroll
@@ -350,7 +355,7 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
                 if (!cval[c]) continue;
                 float f[VN];
 #pragma unroll
-                for (int i = 0; i < VN; ++i) f[i] = acc[c][i] * rs;
+                for (int i = 0; i < VN; ++i) f[i] = SCALED ? acc[c][i] * rs : acc[c][i];
                 stg_na(dst + coff[c], Vec16<T>::pack(f));
             }
         }
@@ -406,7 +411,7 @@ spmm_segments_kernel(const int32_t* __restrict__ col, const T* __restrict__ x, i
     }
 }
 
-template <typename T>
+template <typename T, bool SCALED = true>
 __global__ void spmm_heavy_finalize_kernel(const float* __restrict__ partial, const int64_t* __restrict__ heavy_rows,
                                            const int64_t* __restrict__ heavy_seg_ptr, int64_t n_heavy,
                                            const float* __restrict__ row_scale, T* __restrict__ y, int64_t ldy, int h) {
@@ -417,11 +422,11 @@ __global__ void spmm_heavy_finalize_kernel(const float* __restrict__ partial, co
         float s = 0.f;
         for (int64_t sg = heavy_seg_ptr[i]; sg < heavy_seg_ptr[i + 1]; ++sg) s += partial[sg * h + c];
         const int64_t r = heavy_rows[i];
-        y[r * ldy + c] = from_f32<T>(s * (row_scale ? row_scale[r] : 1.f));
+        y[r * ldy + c] = from_f32<T>(SCALED ? s * (row_scale ? row_scale[r] : 1.f) : s);
     }
 }
 
-template <typename T>
+template <typename T, bool SCALED = true>
 static int launch_spmm(const int64_t* rowptr, const int32_t* col, const float* row_scale, const void* x, int64_t ldx,
                        void* y, int64_t ldy, int64_t n_rows, int h, int64_t max_len, cudaStream_t st, const SlotWait* slots = nullptr,
                        const float* val = nullptr) {
@@ -454,8 +459,8 @@ static int launch_spmm(const int64_t* rowptr, const int32_t* col, const float* r
             spmm_rows_kernel<T, N, false, true><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(rowptr, col, row_scale, xp, ldx, yp, \
                                                                                    ldy, n_rows, chunks, lpr_log2, max_len, sw, val); \
         else                                                                                                          \
-            spmm_rows_kernel<T, N><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(rowptr, col, row_scale, xp, ldx, yp, ldy,  \
-                                                                            n_rows, chunks, lpr_log2, max_len, sw);    \
+            spmm_rows_kernel<T, N, false, false, SCALED><<<(unsigned)blocks, kSpmmBlock, 0, st>>>(                   \
+                rowptr, col, row_scale, xp, ldx, yp, ldy, n_rows, chunks, lpr_log2, max_len, sw);                        \
         break;
     switch (cpl) {
         SGF_SPMM_CASE(1)
@@ -507,7 +512,7 @@ static int launch_range(const int64_t* rowptr, const int32_t* col, const float* 
     return SGF_OK;
 }
 
-template <typename T>
+template <typename T, bool SCALED = true>
 static int launch_heavy(const int32_t* col, const float* row_scale, const void* x, int64_t ldx, void* y, int64_t ldy, int h,
                         const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg, float* partial,
                         const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, cudaStream_t st,
@@ -544,7 +549,7 @@ static int launch_heavy(const int32_t* col, const float* row_scale, const void* 
     count_launch();
     int64_t fb = (n_heavy * h + 255) / 256;
     if (fb > cap) fb = cap;
-    spmm_heavy_finalize_kernel<T><<<(unsigned)fb, 256, 0, st>>>(partial, heavy_rows, heavy_seg_ptr, n_heavy, row_scale,
+    spmm_heavy_finalize_kernel<T, SCALED><<<(unsigned)fb, 256, 0, st>>>(partial, heavy_rows, heavy_seg_ptr, n_heavy, row_scale,
                                                                 static_cast<T*>(y), ldy, h);
     SGF_LAUNCH_CHECK();
     count_launch();
@@ -660,5 +665,30 @@ extern "C" int sgf_spmm_heavy_weighted(const int32_t* col, const float* val, con
     if (dtype == 1)
         return sgf::launch_heavy<__nv_bfloat16>(col, row_scale, x, ldx, y, ldy, h, seg_start, seg_len, n_seg, partial, heavy_rows,
                                                 heavy_seg_ptr, n_heavy, st, val);
+    return SGF_ERR_ARG;
+}
+
+extern "C" int sgf_spmm_sum(const int64_t* rowptr, const int32_t* col, const void* x, int64_t ldx, void* y, int64_t ldy,
+                            int64_t n_rows, int h, int dtype, int64_t max_row_len, void* stream) {
+    if (!rowptr || n_rows < 0 || h <= 0 || (n_rows > 0 && (!col || !x || !y)) || max_row_len < 0) return SGF_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == 0) return sgf::launch_spmm<float, false>(rowptr, col, nullptr, x, ldx, y, ldy, n_rows, h, max_row_len, st);
+    if (dtype == 1) return sgf::launch_spmm<__nv_bfloat16, false>(rowptr, col, nullptr, x, ldx, y, ldy, n_rows, h, max_row_len, st);
+    return SGF_ERR_ARG;
+}
+
+extern "C" int sgf_spmm_heavy_sum(const int32_t* col, const void* x, int64_t ldx, void* y, int64_t ldy, int h, int dtype,
+                                  const int64_t* seg_start, const int32_t* seg_len, int64_t n_seg, float* partial,
+                                  const int64_t* heavy_rows, const int64_t* heavy_seg_ptr, int64_t n_heavy, void* stream) {
+    if (!col || !x || !y || h <= 0 || n_seg < 0 || n_heavy < 0) return SGF_ERR_ARG;
+    if (n_seg == 0 || n_heavy == 0) return SGF_OK;
+    if (!seg_start || !seg_len || !partial || !heavy_rows || !heavy_seg_ptr) return SGF_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == 0)
+        return sgf::launch_heavy<float, false>(col, nullptr, x, ldx, y, ldy, h, seg_start, seg_len, n_seg, partial, heavy_rows,
+                                               heavy_seg_ptr, n_heavy, st);
+    if (dtype == 1)
+        return sgf::launch_heavy<__nv_bfloat16, false>(col, nullptr, x, ldx, y, ldy, h, seg_start, seg_len, n_seg, partial,
+                                                       heavy_rows, heavy_seg_ptr, n_heavy, st);
     return SGF_ERR_ARG;
 }

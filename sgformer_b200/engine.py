@@ -715,6 +715,17 @@ def _weighted_spmm(g: Graph, transposed: bool, row_scale: Tensor, x: Tensor) -> 
     return K.spmm(g.rowptr, g.col, row_scale, x, heavy=g.heavy, val=g.val)
 
 
+def _gcn_spmm(g: Graph, transposed: bool, dinv: Optional[Tensor], x: Tensor, comm: Comm) -> Tensor:
+    """Â x (or Âᵀ x) of one GCN layer; dinv None: the unnormalised conv (cfg gcn_normalize False), a plain sum over the edges as
+    given (sgf_spmm_sum)."""
+    if dinv is None:
+        rp, cl = g.transpose() if transposed else (g.rowptr, g.col)
+        return K.spmm_sum(rp, cl, x, heavy=g.heavy_t if transposed else g.heavy)
+    if _is_weighted(g):
+        return _weighted_spmm(g, transposed, dinv, x)
+    return comm.spmm_gathered(K, g, transposed, dinv, x)
+
+
 def _want_edge_grad(P) -> bool:
     w = P.get(EDGE_WEIGHT)
     return w is not None and w.requires_grad
@@ -723,14 +734,19 @@ def _want_edge_grad(P) -> bool:
 def gcn_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, training: bool, seed: int,
                 tape: Optional[Tape], mix: Optional[Tensor] = None, gw: float = 1.0, pfx: str = "gnn.",
                 comm: Comm = SINGLE) -> Tensor:
-    """models.GCN.forward (medium/models.py:49-63).  `graph` is built with PyG self-loop semantics (gcn_norm)."""
+    """models.GCN.forward (medium/models.py:49-63).  `graph` is built with PyG self-loop semantics (gcn_norm).  With
+    cfg["gcn_normalize"] False it is gnns.GCN(save_mem=True).forward (large/gnns.py:212-220): every conv is
+    GCNConv(normalize=False), a plain sum over the edges of `graph` as built (self-loop mode 0), with no degree scaling."""
     nl = cfg["gcn_num_layers"]
+    norm = bool(cfg.get("gcn_normalize", True))
     n = xin.rows
     dev = xin.data.device
     p = float(cfg["gcn_dropout"]) if training else 0.0
     use_bn = bool(cfg["gcn_use_bn"])
     if _is_weighted(graph) and comm.active:
         raise NotImplementedError("sgformer_b200: row sharding of a weighted graph is not supported")
+    if not norm and (comm.active or _is_weighted(graph)):
+        raise NotImplementedError("sgformer_b200: the unnormalised GCN runs unsharded on an unweighted graph")
     keep_t = tape is not None and _is_weighted(graph) and _want_edge_grad(P)
     cur_op, cur_k = xin, cfg["in_channels"]
     layers = []
@@ -738,13 +754,13 @@ def gcn_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, tra
     for i in range(nl):
         last = i == nl - 1
         g = _layer_graph(graph, last)
-        dinv = g.dinv
+        dinv = g.dinv if norm else None
         wname = f"{pfx}convs.{i}.lin.weight"
         hout = P[wname].shape[0]
         check_width(hout, prec, f"GCN layer {i} out_channels")
         t = K.gemm_nt([cur_op], [_w(P, wname, prec)], [(0, 0, 0, 0, cur_k)], hout, K.alloc_act(n, hout, prec.act_dtype, dev),
                       row_scale=dinv)
-        s = _weighted_spmm(g, False, dinv, t) if _is_weighted(g) else comm.spmm_gathered(K, g, False, dinv, t)
+        s = _gcn_spmm(g, False, dinv, t, comm)
         zb = P.get(f"{pfx}convs.{i}.bias")
         if last:
             out, _ = K.bn_fwd(s, None, mix, None, None, None, None, zb, False, False, 0.0, 0, gw, None, True, False)
@@ -780,7 +796,7 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         L = tape["layers"][i]
         last = i == nl - 1
         g = _layer_graph(graph, last)
-        dinv = g.dinv
+        dinv = g.dinv if cfg.get("gcn_normalize", True) else None
         zb = P.get(f"{pfx}convs.{i}.bias")
         hout = L["hout"]
         if last:
@@ -796,13 +812,10 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         gs = 1.0
         if zb is not None:
             grads[f"{pfx}convs.{i}.bias"] = colsum
-        if _is_weighted(g):
-            u = _weighted_spmm(g, True, dinv, dzs)
-            if dew is not None:     # dL/dw of this layer: <dzs_c, t_r> + the degree term of row c
-                K.edge_weight_grad(g.rowptr, g.col, g.eid, dzs, L["t"], dew, y=L["s"], u=u, dinv=dinv, edge_index=g.edge_index,
-                                   loops=True)
-        else:
-            u = comm.spmm_gathered(K, g, True, dinv, dzs)        # = Â^T dz = gradient of (x W^T)
+        u = _gcn_spmm(g, True, dinv, dzs, comm)        # = Â^T dz = gradient of (x W^T)
+        if _is_weighted(g) and dew is not None:     # dL/dw of this layer: <dzs_c, t_r> + the degree term of row c
+            K.edge_weight_grad(g.rowptr, g.col, g.eid, dzs, L["t"], dew, y=L["s"], u=u, dinv=dinv, edge_index=g.edge_index,
+                               loops=True)
         u_op = K.as_operand(u, prec.planes)
         wname = f"{pfx}convs.{i}.lin.weight"
         dw = torch.empty((hout, L["cur_k"]), dtype=torch.float32, device=dev)

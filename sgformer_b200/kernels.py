@@ -349,6 +349,34 @@ def spmm(rowptr: Tensor, col: Tensor, row_scale: Optional[Tensor], x: Tensor, ou
     return out
 
 
+def spmm_sum(rowptr: Tensor, col: Tensor, x: Tensor, out: Optional[Tensor] = None, heavy: Optional[HeavyRows] = None) -> Tensor:
+    """y = A x over the CSR (rowptr, col) as built: the plain neighbour sum of GCNConv(normalize=False) (sgf_spmm_sum)."""
+    _use(x)
+    n = rowptr.numel() - 1
+    rows, h, ldx = _mat(x, "x")
+    if out is None:
+        out = alloc_act(n, h, x.dtype, x.device)
+    _, ho, ldy = _mat(out, "out")
+    if ho != h or out.dtype != x.dtype:
+        raise ValueError("spmm_sum: out shape/dtype mismatch")
+    ev = spmm_events
+    if ev is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    check(lib().sgf_spmm_sum(_p(rowptr), _p(col), _p(x), ldx, _p(out), ldy, n, h, dcode(x), HEAVY_ROW if heavy is not None else 0,
+                             _stream()), "sgf_spmm_sum")
+    if heavy is not None:
+        ns = heavy.seg_start.numel()
+        partial = torch.empty((ns, h), dtype=torch.float32, device=x.device)
+        check(lib().sgf_spmm_heavy_sum(_p(col), _p(x), ldx, _p(out), ldy, h, dcode(x), _p(heavy.seg_start), _p(heavy.seg_len), ns,
+                                       _p(partial), _p(heavy.rows), _p(heavy.seg_ptr), heavy.rows.numel(), _stream()),
+              "sgf_spmm_heavy_sum")
+    if ev is not None:
+        e1.record()
+        ev.append((e0, e1))
+    return out
+
+
 def _spmm_weighted(rowptr: Tensor, col: Tensor, val: Tensor, row_scale: Optional[Tensor], x: Tensor, out: Optional[Tensor],
                    heavy: Optional[HeavyRows]) -> Tensor:
     _use(x)

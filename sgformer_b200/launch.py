@@ -18,8 +18,9 @@ def main(argv=None):
     ap.add_argument("--precision", choices=["bf16", "fp32"], default=None)
     ap.add_argument("--native-backbones", action="store_true",
                     help="medium: make the GAT and GCN that the reference's parse.py builds backbones from resolve to "
-                         "sgformer_b200.medium.GAT / GCN, so that --backbone gat|gcn (and --method gat|gcn) run on the kernels "
-                         "(models.py still imports torch_geometric)")
+                         "sgformer_b200.medium.GAT / GCN, so that --backbone gat|gcn (and --method gat|gcn) run on the kernels; "
+                         "large: make parse.py's GCN and GAT (from gnns.py) resolve to sgformer_b200.large_gnns.GCN / GAT, so that "
+                         "--method gcn|gat runs on the kernels (models.py / gnns.py still import torch_geometric)")
     ap.add_argument("script")
     ap.add_argument("script_args", nargs=argparse.REMAINDER)
     a = ap.parse_args(argv)
@@ -31,15 +32,20 @@ def main(argv=None):
     sys.argv = [script] + a.script_args
     os.chdir(sdir)
     if a.native_backbones:
-        if a.variant != "medium":
-            ap.error("--native-backbones applies to --variant medium")
-        # parse.py star-imports models, ours, ..., graphtrans (whose own GCN shadows models.GCN); parse_method looks the classes up
-        # in parse's namespace, so that is where they are replaced (main.py's `from parse import ...` then reuses this module)
-        import models
+        if a.variant == "100M":
+            ap.error("--native-backbones applies to --variant medium and large")
+        # parse.py star-imports models (medium) / gnns (large), ours, ... (medium's graphtrans has a GCN of its own that shadows
+        # models.GCN); parse_method looks the classes up in parse's namespace, so that is where they are replaced (main.py's
+        # `from parse import ...` then reuses this module)
+        if a.variant == "medium":
+            import models as gnn_mod
+            from . import medium as native
+        else:
+            import gnns as gnn_mod
+            from . import large_gnns as native
         import parse
-        from . import medium
-        for mod in (models, parse):
-            mod.GAT, mod.GCN = medium.GAT, medium.GCN
+        for mod in (gnn_mod, parse):
+            mod.GAT, mod.GCN = native.GAT, native.GCN
     runpy.run_path(script, run_name="__main__")
 
 

@@ -239,10 +239,15 @@ class GAT(_Base):
         _check_gat_data(data)
         if not x.is_cuda:
             raise RuntimeError("sgformer_b200.GAT needs CUDA tensors (no CPU fallback)")
-        names, tensors = _gat_flat(self, "gnn.")
+        return self._run(x, edge_index)
+
+    def _run(self, x, edge_index, names=None, tensors=None):
+        """The stack on CUDA x / edge_index; (names, tensors) default to this module's own (large_gnns.GAT passes device copies)."""
+        if names is None:
+            names, tensors = _gat_flat(self, "")
         cfg = make_config("medium", x.shape[1], self.convs[0].lin_src.weight.shape[0], self.convs[-1].out_channels, **self._cfg_kw())
         graph = get_graph(edge_index, x.shape[0], 1)
-        return Fn.GraphBranchFn.apply(x, graph, cfg, E.precision(self.precision), self.training, "gat", "gnn.", names, *tensors)
+        return Fn.GraphBranchFn.apply(x, graph, cfg, E.precision(self.precision), self.training, "gat", "", names, *tensors)
 
 
 def _check_gat_data(data):
