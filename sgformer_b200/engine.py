@@ -15,7 +15,7 @@ from __future__ import annotations
 import itertools
 from collections import OrderedDict
 from dataclasses import dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -838,35 +838,201 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
 # (sgf_gat_fwd; concat for the hidden layers, head mean for the last), then BatchNorm?/ELU/dropout in one bn_fwd pass whose
 # statistics come from one colstats pass.  Backward: bn_bwd (ELU code), sgf_gat_bwd (two gathers: forward CSR, then transposed
 # CSR) -> dxp incl. the logits' share, d att_* by per-head weighted column sums, dW and dx by the GEMMs.
+# Wide layers (DESIGN.md §4.9): one launch of the GAT kernels serves at most SGF_GAT_MAX_HEADS heads and 2 KB of a row (512 fp32 /
+# 1024 bf16 values), and so does one launch of the BatchNorm / ELU / dropout row kernels.  The edge softmax is independent per head,
+# so a wider layer runs as a schedule over head groups (gat_groups): each group runs the unchanged kernels on column views of xp,
+# att_*, z and g.  Group k draws its attention and post-ELU dropout under the layer's seed + k * _GAT_GROUP_SEED, so heads of
+# different groups get independent masks and group 0 (all of a layer that fits one launch) keeps the layer's seeds.
+_GAT_GROUP_SEED = 0x632BE59BD9B4E019       # odd 64-bit constant
+_M64 = (1 << 64) - 1
+
+
+def _gat_group_seed(seed: int, k: int) -> int:
+    return (seed + k * _GAT_GROUP_SEED) & _M64 if k else seed
+
+
+def gat_groups(dtype: str, heads: int, c: int) -> Tuple[int, List[Tuple[int, int]]]:
+    """-> (cp, [(first head, head count), ...]): how a GAT layer of `heads` heads of `c` channels runs in precision `dtype` ('fp32' /
+    'bf16').  cp is c rounded up to whole 16-byte chunks (4 fp32 / 8 bf16 values), the width every head runs at.  Each head is in
+    exactly one group; a group has at most SGF_GAT_MAX_HEADS heads and 2 KB of a row (group heads * cp <= 512 fp32 / 1024 bf16);
+    the groups are as few as that allows, in head order, sizes differing by at most one (larger first).  A layer that fits one
+    launch is one group.  ValueError when a single head is wider than one launch."""
+    if dtype not in ("fp32", "bf16"):
+        raise ValueError(f"unknown precision {dtype!r}")
+    vn = 8 if dtype == "bf16" else 4
+    row_max = 128 * vn
+    if heads < 1 or c < 1:
+        raise ValueError(f"heads={heads}, out_channels={c}: both must be at least 1")
+    cp = (c + vn - 1) // vn * vn
+    per = min(K.GAT_MAX_HEADS, row_max // cp)
+    if per < 1:
+        raise ValueError(f"heads={heads}, out_channels={c} is not supported in precision '{dtype}': one head must fit one launch of the "
+                         f"GAT kernels, out_channels at most {row_max}"
+                         + (" (set_precision('bf16') runs heads of up to 1024 channels)" if dtype == "fp32" and cp <= 1024 else ""))
+    ng = -(-heads // per)
+    q, r = divmod(heads, ng)
+    groups, h0 = [], 0
+    for k in range(ng):
+        hg = q + (k < r)
+        groups.append((h0, hg))
+        h0 += hg
+    return cp, groups
+
+
+@dataclass
+class _GatPlan:
+    """One GAT layer: heads x c channels run at cp (gat_groups); mean: a head-mean (concat=False) layer."""
+    heads: int
+    c: int
+    cp: int
+    mean: bool
+    groups: List[Tuple[int, int]]
+
+    def cols(self, grp) -> slice:
+        """Columns of head group grp in xp / z / g of a concatenating layer (xp of either)."""
+        return slice(grp[0] * self.cp, (grp[0] + grp[1]) * self.cp)
+
+
+def _gat_plan(prec: Precision, heads: int, c: int, mean: bool, i: int) -> _GatPlan:
+    try:
+        cp, groups = gat_groups(prec.name, heads, c)
+    except ValueError as e:
+        raise ValueError(f"sgformer_b200 GAT layer {i}: {e}") from None
+    return _GatPlan(heads, c, cp, mean, groups)
+
+
 def _gat_dims(P, pfx: str, i: int):
     att = P[f"{pfx}convs.{i}.att_src"]
     return int(att.shape[-2]), int(att.shape[-1])
 
 
-def _gat_layer(P, lp: str, heads: int, c: int, mean: bool, prec: Precision, i: int):
-    """-> (cp, weight [heads*cp, in], att_src [heads*cp], att_dst [heads*cp], bias) of layer i.  The kernels move rows in 16-byte
-    chunks per head, so a head-mean layer (the last conv: out_channels = classes in `--method gat`) whose width is not a multiple of
-    4 (fp32) / 8 (bf16) runs on zero-padded heads: the padded channels have zero weights and attention vectors, so they change
-    neither the logits nor the real channels, and the output is the real columns of the padded one."""
-    vn = 8 if prec.name == "bf16" else 4
-    cp = K.ceil_to(c, vn)
-    hc_max = 1024 if prec.name == "bf16" else 512
-    if heads > K.GAT_MAX_HEADS or (cp != c and not mean) or heads * cp > hc_max:
-        raise ValueError(f"sgformer_b200 GAT layer {i}: heads={heads}, out_channels={c} is not supported in precision '{prec.name}': "
-                         f"heads must be at most {K.GAT_MAX_HEADS}, the out_channels of a concatenating layer a multiple of {vn} and "
-                         f"heads*out_channels at most {hc_max}")
-    w, a_s, a_d, b = P[lp + "lin_src.weight"], P[lp + "att_src"].reshape(-1), P[lp + "att_dst"].reshape(-1), P[lp + "bias"]
+def _pad_heads(t: Tensor, heads: int, c: int, cp: int, dim: int = 0, fill: float = 0.0) -> Tensor:
+    """t whose axis `dim` is `heads` blocks of c -> blocks of cp: each block's c values, then `fill` (fp32).  t itself when cp == c."""
     if cp == c:
-        return cp, w, a_s, a_d, b
-    dev = w.device
+        return t
+    t = t.detach().movedim(dim, 0)
+    rest = tuple(t.shape[1:])
+    out = torch.full((heads, cp) + rest, fill, dtype=torch.float32, device=t.device)
+    out[:, :c] = t.reshape((heads, c) + rest)
+    return out.reshape((heads * cp,) + rest).movedim(0, dim).contiguous()
 
-    def pad(t, rows):      # [heads*c, ...] -> [heads*cp, ...], zeros in each head's padding
-        out = torch.zeros((heads, cp) + tuple(t.shape[1:]), dtype=torch.float32, device=dev)
-        out[:, :c] = t.detach().reshape((heads, c) + tuple(t.shape[1:]))
-        return out.reshape((heads * cp,) + tuple(t.shape[1:]))
-    bp = torch.zeros(cp, dtype=torch.float32, device=dev)
-    bp[:c] = b.detach()
-    return cp, pad(w, True), pad(a_s, False), pad(a_d, False), bp
+
+def _unpad_heads(t: Tensor, heads: int, c: int, cp: int, dim: int = 0) -> Tensor:
+    """Inverse of _pad_heads: the real c of every cp-wide block along `dim`."""
+    if cp == c:
+        return t
+    t = t.movedim(dim, 0)
+    rest = tuple(t.shape[1:])
+    return t.reshape((heads, cp) + rest)[:, :c].reshape((heads * c,) + rest).movedim(0, dim).contiguous()
+
+
+def _gat_layer(P, lp: str, heads: int, c: int, mean: bool, prec: Precision, i: int, prev: Optional[_GatPlan] = None):
+    """-> (cp, weight [heads*cp, in], att_src [heads*cp], att_dst [heads*cp], bias [heads*cp | cp]) of layer i at its run widths.
+    The kernels move rows in 16-byte chunks per head, so a head whose width is not a multiple of 4 (fp32) / 8 (bf16) runs
+    zero-padded to cp: the padded channels have zero weights, attention entries and bias, so they change neither the logits nor
+    the real channels and stay exactly 0 (through BatchNorm too, whose padded affine is zero).  `prev`: the previous layer, whose
+    padded channels this layer's weight reads through zero columns (`in` = its heads * cp)."""
+    cp = _gat_plan(prec, heads, c, mean, i).cp
+    w = _pad_heads(P[lp + "lin_src.weight"], heads, c, cp)
+    if prev is not None:
+        w = _pad_heads(w, prev.heads, prev.c, prev.cp, dim=1)
+    a_s = _pad_heads(P[lp + "att_src"].reshape(-1), heads, c, cp)
+    a_d = _pad_heads(P[lp + "att_dst"].reshape(-1), heads, c, cp)
+    return cp, w, a_s, a_d, _pad_heads(P[lp + "bias"], 1 if mean else heads, c, cp)
+
+
+def _sl(t: Optional[Tensor], cols: slice) -> Optional[Tensor]:
+    return None if t is None else t[cols]
+
+
+def _gat_conv_fwd(graph: Graph, xp: Tensor, lay: _GatPlan, att_s: Tensor, att_d: Tensor, bias: Tensor, p: float, seed: int):
+    """Edge softmax aggregation of one layer over its head groups -> (z [N, heads*cp] | head mean [N, cp], [(a_src, a_dst, lse)] per
+    group).  A concatenating group writes its own column block of z.  A head-mean layer of several groups sums the groups' means
+    weighted by group heads / heads in group order (sgf_axpby) and adds the bias once (sgf_bn_fwd's zbias): no float atomics."""
+    H, cp = lay.heads, lay.cp
+    if len(lay.groups) == 1:
+        a_s, a_d = K.gat_logits(xp, H, cp, att_s, att_d)
+        z, lse = K.gat_fwd(graph.rowptr, graph.col, xp, a_s, a_d, H, cp, lay.mean, bias, p, seed)
+        return z, [(a_s, a_d, lse)]
+    n = xp.shape[0]
+    z = None if lay.mean else K.alloc_act(n, H * cp, xp.dtype, xp.device)
+    parts, means = [], []
+    for k, grp in enumerate(lay.groups):
+        cols, hg = lay.cols(grp), grp[1]
+        xg = xp[:, cols]
+        a_s, a_d = K.gat_logits(xg, hg, cp, att_s[cols], att_d[cols])
+        if lay.mean:
+            zk, lse = K.gat_fwd(graph.rowptr, graph.col, xg, a_s, a_d, hg, cp, True, None, p, _gat_group_seed(seed, k))
+            means.append((zk, hg / H))
+        else:
+            _, lse = K.gat_fwd(graph.rowptr, graph.col, xg, a_s, a_d, hg, cp, False, bias[cols], p, _gat_group_seed(seed, k),
+                               out=z[:, cols])
+        parts.append((a_s, a_d, lse))
+    if lay.mean:
+        acc = K.axpby(means[0][0], means[1][0], means[0][1], means[1][1])
+        for zk, wk in means[2:]:
+            acc = K.axpby(zk, acc, wk, 1.0)
+        z, _ = K.bn_fwd(acc, None, None, None, None, None, None, bias, False, False, 0.0, 0, 1.0, None, True, False)
+    return z, parts
+
+
+def _gat_conv_bwd(graph: Graph, rp_t: Tensor, col_t: Tensor, L: dict, g: Tensor, p: float, seed: int):
+    """Backward of _gat_conv_fwd for g = dL/dz -> (dxp [N, heads*cp], [(da_src, da_dst) fp32 [group heads, N]] per group).  Group k
+    of a concatenating layer reads its column block of g; of a head-mean layer, g * group heads / heads.  Each group writes its
+    column block of dxp."""
+    lay, xp = L["lay"], L["xp"]
+    att_s, att_d = L["att"]
+    H, cp = lay.heads, lay.cp
+    if len(lay.groups) == 1:
+        a_s, a_d, lse = L["parts"][0]
+        dxp, da_s, da_d = K.gat_bwd(graph.rowptr, graph.col, rp_t, col_t, xp, a_s, a_d, lse, g, att_s, att_d, H, cp, lay.mean, p,
+                                    seed)
+        das = [(da_s, da_d)]
+    else:
+        dxp = K.new_like(xp)
+        das, scaled = [], {}
+        for k, (grp, (a_s, a_d, lse)) in enumerate(zip(lay.groups, L["parts"])):
+            cols, hg = lay.cols(grp), grp[1]
+            if lay.mean:
+                if hg not in scaled:
+                    scaled[hg] = K.axpby(g, None, hg / H, 0.0)
+                gk = scaled[hg]
+            else:
+                gk = g[:, cols]
+            _, da_s, da_d = K.gat_bwd(graph.rowptr, graph.col, rp_t, col_t, xp[:, cols], a_s, a_d, lse, gk, att_s[cols], att_d[cols],
+                                      hg, cp, lay.mean, p, _gat_group_seed(seed, k), dxp_out=dxp[:, cols])
+            das.append((da_s, da_d))
+    return dxp, das
+
+
+def _gat_att_grads(xp: Tensor, lay: _GatPlan, das) -> Tuple[Tensor, Tensor]:
+    """d att_src, d att_dst [heads, cp]: per head, the column sums of xp's head block weighted by the head's da_src / da_dst."""
+    H, cp = lay.heads, lay.cp
+    datt_s = torch.zeros((H, cp), dtype=torch.float32, device=xp.device)
+    datt_d = torch.zeros((H, cp), dtype=torch.float32, device=xp.device)
+    for (h0, hg), (da_s, da_d) in zip(lay.groups, das):
+        for j in range(hg):
+            xh = xp[:, (h0 + j) * cp:(h0 + j + 1) * cp]
+            K.colstats(xh, w=da_s[j], want_sumsq=False, sum_out=datt_s[h0 + j])
+            K.colstats(xh, w=da_d[j], want_sumsq=False, sum_out=datt_d[h0 + j])
+    return datt_s, datt_d
+
+
+def _gat_bn_stats(z: Tensor, P, name: str, use_bn: bool, training: bool, lay: _GatPlan):
+    """_bn_stats over the padded z of a concatenating layer: the running buffers are padded for the call (mean 0, variance 1 in the
+    padding) and their real columns written back."""
+    if not use_bn or lay.cp == lay.c:
+        return _bn_stats(z, P, name, use_bn, training)
+    H, c, cp = lay.heads, lay.c, lay.cp
+    rm, rv = P[name + "running_mean"], P[name + "running_var"]
+    Pp = {name + "running_mean": _pad_heads(rm, H, c, cp), name + "running_var": _pad_heads(rv, H, c, cp, fill=1.0)}
+    if P.get(name + "num_batches_tracked") is not None:
+        Pp[name + "num_batches_tracked"] = P[name + "num_batches_tracked"]
+    mean, rstd = _bn_stats(z, Pp, name, True, training)
+    if training:
+        rm.copy_(_unpad_heads(Pp[name + "running_mean"], H, c, cp))
+        rv.copy_(_unpad_heads(Pp[name + "running_var"], H, c, cp))
+    return mean, rstd
 
 
 def gat_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, training: bool, seed: int,
@@ -887,28 +1053,42 @@ def gat_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, tra
         cur_op = K.pack_operand(K.dense_dropout(xr, p, seed + _SEED_GAT_INPUT), False, prec.planes)
     layers = []
     out = None
+    prev = None
     for i in range(nl):
         last = i == nl - 1
         H, C = _gat_dims(P, pfx, i)
         lp = f"{pfx}convs.{i}."
-        cp, w, att_s, att_d, bias = _gat_layer(P, lp, H, C, last, prec, i)
+        lay = _gat_plan(prec, H, C, last, i)
+        cp, w, att_s, att_d, bias = _gat_layer(P, lp, H, C, last, prec, i, prev)
         xp = K.gemm_nt([cur_op], [K.pack_operand(w, False, prec.planes)], [(0, 0, 0, 0, cur_op.k)], H * cp,
                        K.alloc_act(n, H * cp, prec.act_dtype, dev))
-        a_s, a_d = K.gat_logits(xp, H, cp, att_s, att_d)
-        z, lse = K.gat_fwd(graph.rowptr, graph.col, xp, a_s, a_d, H, cp, last, bias, p, seed + _SEED_GAT_ATT + i)
-        if cp != C:
-            z = z[:, :C]
-        L = dict(cur_op=cur_op, xp=xp, a_s=a_s, a_d=a_d, lse=lse, H=H, C=C, cp=cp, w=w, att=(att_s, att_d))
+        z, parts = _gat_conv_fwd(graph, xp, lay, att_s, att_d, bias, p, seed + _SEED_GAT_ATT + i)
+        L = dict(cur_op=cur_op, xp=xp, parts=parts, lay=lay, w=w, att=(att_s, att_d), prev=prev)
         if last:
+            if cp != C:
+                z = z[:, :C]
             out = K.axpby(z, mix, gw, 1.0 - gw) if mix is not None else z
         else:
+            # BatchNorm / ELU / dropout per head group: column blocks of at most 2 KB (the row kernels' width); the statistics
+            # are per column, so the blocks share one colstats / bn_finalize over the whole z
             name = f"{pfx}bns.{i}."
-            mean, rstd = _bn_stats(z, P, name, use_bn, training)
-            y, _ = K.bn_fwd(z, None, None, mean, rstd, P.get(name + "weight"), P.get(name + "bias"), None, use_bn, K.ACT_ELU, p,
-                            seed + _SEED_GAT_ACT + i, 1.0, None, True, False)
-            L.update(z=z, mean=mean, rstd=rstd)
+            mean, rstd = _gat_bn_stats(z, P, name, use_bn, training, lay)
+            bw, bb = P.get(name + "weight"), P.get(name + "bias")
+            if use_bn:
+                bw, bb = _pad_heads(bw, H, C, cp), _pad_heads(bb, H, C, cp)
+            if len(lay.groups) == 1:
+                y, _ = K.bn_fwd(z, None, None, mean, rstd, bw, bb, None, use_bn, K.ACT_ELU, p, seed + _SEED_GAT_ACT + i, 1.0, None,
+                                True, False)
+            else:
+                y = K.new_like(z)
+                for k, grp in enumerate(lay.groups):
+                    cs = lay.cols(grp)
+                    K.bn_fwd(z[:, cs], None, None, _sl(mean, cs), _sl(rstd, cs), _sl(bw, cs), _sl(bb, cs), None, use_bn, K.ACT_ELU,
+                             p, _gat_group_seed(seed + _SEED_GAT_ACT + i, k), 1.0, None, True, False, y_out=y[:, cs])
+            L.update(z=z, mean=mean, rstd=rstd, bn=(bw, bb))
             cur_op = K.as_operand(y, prec.planes)
         layers.append(L)
+        prev = lay
     if tape is not None:
         tape.update(layers=layers, p=p, seed=seed, n=n, training=training, mixed=mix is not None, gw=gw)
     return out
@@ -928,41 +1108,55 @@ def gat_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         L = tape["layers"][i]
         last = i == nl - 1
         lp = f"{pfx}convs.{i}."
-        H, C, cp = L["H"], L["C"], L["cp"]
+        lay, prev = L["lay"], L["prev"]
+        H, C, cp = lay.heads, lay.c, lay.cp
         db = None
         if last:
             g = K.axpby(dcur, None, gs, 0.0) if gs != 1.0 else dcur
+            if cp != C:        # zero-padded heads (see _gat_layer): the gradient of the padding columns is zero
+                gp = torch.zeros((n, cp), dtype=g.dtype, device=dev)
+                K.axpby(g, None, 1.0, 0.0, out=gp[:, :C])
+                g = gp
         else:
             # the bias gradient is the column sum of dz taken in fp32 inside bn_bwd: in bf16, summing the stored dz would add its
-            # rounding to a sum that a training BatchNorm makes exactly zero
+            # rounding to a sum that a training BatchNorm makes exactly zero.  One bn_bwd per head group (<= 2 KB of a row).
             name = f"{pfx}bns.{i}."
-            g, sums, db = K.bn_bwd(dcur, None, None, L["z"], L["mean"], L["rstd"], P.get(name + "weight"), P.get(name + "bias"), None,
-                                   use_bn, K.ACT_ELU, training, p, seed + _SEED_GAT_ACT + i, 1.0, want_dz_colsum=True)
+            bw, bb = L["bn"]
+            one = len(lay.groups) == 1
+            if one:
+                g, s_k, db = K.bn_bwd(dcur, None, None, L["z"], L["mean"], L["rstd"], bw, bb, None, use_bn, K.ACT_ELU, training, p,
+                                      seed + _SEED_GAT_ACT + i, 1.0, want_dz_colsum=True)
+                sums = [s_k]
+            else:
+                g = K.new_like(L["z"])
+                sums, dbs = [], []
+                for k, grp in enumerate(lay.groups):
+                    cs = lay.cols(grp)
+                    _, s_k, db_k = K.bn_bwd(dcur[:, cs], None, None, L["z"][:, cs], _sl(L["mean"], cs), _sl(L["rstd"], cs),
+                                            _sl(bw, cs), _sl(bb, cs), None, use_bn, K.ACT_ELU, training, p,
+                                            _gat_group_seed(seed + _SEED_GAT_ACT + i, k), 1.0, want_dz_colsum=True, dz_out=g[:, cs])
+                    sums.append(s_k)
+                    dbs.append(db_k)
+                db = torch.cat(dbs)
             if use_bn and training:
-                _bn_param_grads(grads, comm, P, name, sums, dcur, None, None, L["z"], L["mean"], L["rstd"], K.ACT_ELU)
-        if cp != C:            # zero-padded heads (see _gat_layer): the gradient of the padding columns is zero
-            gp = torch.zeros((n, cp), dtype=g.dtype, device=dev)
-            K.axpby(g, None, 1.0, 0.0, out=gp[:, :C])
-            g = gp
+                if one and cp == C:
+                    _bn_param_grads(grads, comm, P, name, sums[0], dcur, None, None, L["z"], L["mean"], L["rstd"], K.ACT_ELU)
+                else:
+                    halves = [s.view(2, -1) for s in sums]
+                    grads[name + "bias"] = _unpad_heads(torch.cat([s[0] for s in halves]), H, C, cp)
+                    grads[name + "weight"] = _unpad_heads(torch.cat([s[1] for s in halves]), H, C, cp)
         if db is None:
             db, _ = K.colstats(g, want_sumsq=False)
-        grads[lp + "bias"] = db if cp == C else db[:C]
-        att_s, att_d = L["att"]
-        xp = L["xp"]
-        dxp, da_s, da_d = K.gat_bwd(graph.rowptr, graph.col, rp_t, col_t, xp, L["a_s"], L["a_d"], L["lse"], g, att_s, att_d, H, cp,
-                                    last, p, seed + _SEED_GAT_ATT + i)
-        datt_s = torch.zeros((H, cp), dtype=torch.float32, device=dev)
-        datt_d = torch.zeros((H, cp), dtype=torch.float32, device=dev)
-        for hd in range(H):
-            xh = xp[:, hd * cp:(hd + 1) * cp]
-            K.colstats(xh, w=da_s[hd], want_sumsq=False, sum_out=datt_s[hd])
-            K.colstats(xh, w=da_d[hd], want_sumsq=False, sum_out=datt_d[hd])
+        grads[lp + "bias"] = _unpad_heads(db, 1 if last else H, C, cp)
+        dxp, das = _gat_conv_bwd(graph, rp_t, col_t, L, g, p, seed + _SEED_GAT_ATT + i)
+        datt_s, datt_d = _gat_att_grads(L["xp"], lay, das)
         grads[lp + "att_src"], grads[lp + "att_dst"] = datt_s[:, :C], datt_d[:, :C]
         dxp_op = K.as_operand(dxp, prec.planes)
         cur_op = L["cur_op"]
         dw = torch.empty((H * cp, cur_op.k), dtype=torch.float32, device=dev)
         K.gemm_tn(dxp_op, cur_op, dw)
-        grads[lp + "lin_src.weight"] = dw if cp == C else dw.view(H, cp, -1)[:, :C].reshape(H * C, -1)
+        dw = _unpad_heads(dw, H, C, cp)
+        grads[lp + "lin_src.weight"] = dw if prev is None else _unpad_heads(dw, prev.heads, prev.c, prev.cp, dim=1)
         wt = K.pack_operand(L["w"], True, prec.planes)
         if i > 0:
             dcur = K.alloc_act(n, cur_op.k, prec.act_dtype, dev)

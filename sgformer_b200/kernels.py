@@ -76,6 +76,16 @@ def alloc_act(rows: int, h: int, dtype, device) -> Tensor:
     return buf[:, :h] if hp != h else buf
 
 
+def _out_like(out: Optional[Tensor], x: Tensor, name: str) -> Tensor:
+    """`out` checked to have x's shape, dtype and pitch (an output the caller placed, e.g. a column block), or new_like(x)."""
+    if out is None:
+        return new_like(x)
+    if out.shape != x.shape or out.dtype != x.dtype or out.device != x.device or _mat(out, name)[2] != x.stride(0):
+        raise ValueError(f"{name}: expected {tuple(x.shape)} {x.dtype} with pitch {x.stride(0)}, got {tuple(out.shape)} {out.dtype} "
+                         f"with pitch {out.stride(0)}")
+    return out
+
+
 def new_like(x: Tensor) -> Tensor:
     """Uninitialised activation with the same shape and pitch as the 2-D row-major tensor x."""
     rows, h, ld = _mat(x, "x")
@@ -873,10 +883,11 @@ def bn_finalize(sum_: Optional[Tensor], sumsq: Optional[Tensor], rows: int, h: i
 
 def bn_fwd(z: Tensor, res: Optional[Tensor], mix: Optional[Tensor], mean, rstd, gamma, beta, zbias, use_bn: bool,
            use_relu: bool, p: float, seed: int, gw: float, row_scale: Optional[Tensor], want_y: bool, want_scaled: bool,
-           ys_out: Optional[Tensor] = None):
+           ys_out: Optional[Tensor] = None, y_out: Optional[Tensor] = None):
+    """y_out (z's shape, dtype and pitch): y is written there (a column block of a wider activation)."""
     _use(z)
     rows, h, ld = _mat(z, "z")
-    y = new_like(z) if want_y else None
+    y = _out_like(y_out, z, "y_out") if want_y else None
     ys = (ys_out if (ys_out is not None and ys_out.stride(0) == ld) else new_like(z)) if want_scaled else None
     _same_ld(ld, res, mix, y, ys)
     check(lib().sgf_bn_fwd(_p(z), _p(res), _p(mix), ld, rows, h, dcode(z), _p(mean), _p(rstd), _p(gamma), _p(beta),
@@ -888,13 +899,13 @@ def bn_fwd(z: Tensor, res: Optional[Tensor], mix: Optional[Tensor], mean, rstd, 
 def bn_bwd(dy: Optional[Tensor], dy2: Optional[Tensor], row_scale2: Optional[Tensor], z: Tensor, mean, rstd, gamma, beta,
            zbias, use_bn: bool, use_relu: bool, training: bool, p: float, seed: int, gscale: float,
            dres: Optional[Tensor] = None, dres_accumulate: bool = False, want_dz_colsum: bool = False,
-           out_row_scale: Optional[Tensor] = None, reduce_fn=None, stat_rows: int = 0):
+           out_row_scale: Optional[Tensor] = None, reduce_fn=None, stat_rows: int = 0, dz_out: Optional[Tensor] = None):
     """-> (dz, sums [2h] or None (dbeta, dgamma), dz_colsum [h] or None).
     `reduce_fn(sums)` runs between the two phases (the row-sharded all-reduce of the BatchNorm sums); `stat_rows` is then
-    the global row count."""
+    the global row count.  dz_out (z's shape, dtype and pitch): dz is written there."""
     _use(z)
     rows, h, ld = _mat(z, "z")
-    dz = new_like(z)
+    dz = _out_like(dz_out, z, "dz_out")
     _same_ld(ld, dy, dy2, dz, dres)
     sums = None
     if use_bn and training:
@@ -974,11 +985,17 @@ def gat_logits(xp: Tensor, heads: int, c: int, att_src: Tensor, att_dst: Tensor)
 
 
 def gat_fwd(rowptr: Tensor, col: Tensor, xp: Tensor, a_src: Tensor, a_dst: Tensor, heads: int, c: int, mean: bool,
-            bias: Optional[Tensor], p: float, seed: int) -> Tuple[Tensor, Tensor]:
-    """-> (out [N, c] if mean else [N, heads*c] in xp's dtype, lse fp32 [N, heads]).  See sgf_gat_fwd."""
+            bias: Optional[Tensor], p: float, seed: int, out: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+    """-> (out [N, c] if mean else [N, heads*c] in xp's dtype, lse fp32 [N, heads]).  See sgf_gat_fwd.
+    out: written in place when given (a column block of a wider activation)."""
     _use(xp)
     n, _, ld = _heads_fit(xp, heads, c, "xp")
-    out = alloc_act(n, c if mean else heads * c, xp.dtype, xp.device)
+    width = c if mean else heads * c
+    if out is None:
+        out = alloc_act(n, width, xp.dtype, xp.device)
+    elif tuple(out.shape) != (n, width) or out.dtype != xp.dtype or out.device != xp.device:
+        raise ValueError(f"gat_fwd: out must be [{n}, {width}] {xp.dtype}, got {tuple(out.shape)} {out.dtype}")
+    _mat(out, "out")
     lse = torch.empty((n, heads), dtype=torch.float32, device=xp.device)
     check(lib().sgf_gat_fwd(_p(rowptr), _p(col), _p(xp), ld, _p(a_src), _p(a_dst), n, heads, c, dcode(xp), int(mean),
                             _p(_f32vec(bias, out.shape[1], "bias")), _p(out), out.stride(0), _p(lse), p, seed, _stream()),
@@ -987,8 +1004,10 @@ def gat_fwd(rowptr: Tensor, col: Tensor, xp: Tensor, a_src: Tensor, a_dst: Tenso
 
 
 def gat_bwd(rowptr: Tensor, col: Tensor, rowptr_t: Tensor, col_t: Tensor, xp: Tensor, a_src: Tensor, a_dst: Tensor, lse: Tensor,
-            g: Tensor, att_src: Tensor, att_dst: Tensor, heads: int, c: int, mean: bool, p: float, seed: int):
-    """g = dL/dout -> (dxp [N, heads*c] in xp's dtype, da_src fp32 [heads, N], da_dst fp32 [heads, N]).  See sgf_gat_bwd."""
+            g: Tensor, att_src: Tensor, att_dst: Tensor, heads: int, c: int, mean: bool, p: float, seed: int,
+            dxp_out: Optional[Tensor] = None):
+    """g = dL/dout -> (dxp [N, heads*c] in xp's dtype, da_src fp32 [heads, N], da_dst fp32 [heads, N]).  See sgf_gat_bwd.
+    dxp_out (xp's shape and dtype, any 16-byte pitch): dxp is written there."""
     _use(xp)
     n, _, ld = _heads_fit(xp, heads, c, "xp")
     _, _, ldg = _heads_fit(g, 1 if mean else heads, c, "g")
@@ -998,7 +1017,10 @@ def gat_bwd(rowptr: Tensor, col: Tensor, rowptr_t: Tensor, col_t: Tensor, xp: Te
     r_ws = torch.empty((n, heads), dtype=torch.float32, device=dev)
     da_src = torch.empty((heads, n), dtype=torch.float32, device=dev)
     da_dst = torch.empty((heads, n), dtype=torch.float32, device=dev)
-    dxp = new_like(xp)
+    dxp = new_like(xp) if dxp_out is None else dxp_out
+    if dxp.shape != xp.shape or dxp.dtype != xp.dtype or dxp.device != xp.device:
+        raise ValueError(f"gat_bwd: dxp_out must be {tuple(xp.shape)} {xp.dtype}, got {tuple(dxp.shape)} {dxp.dtype}")
+    _mat(dxp, "dxp_out")
     check(lib().sgf_gat_bwd(_p(rowptr), _p(col), _p(rowptr_t), _p(col_t), _p(xp), ld, _p(a_src), _p(a_dst), _p(lse), _p(g), ldg,
                             _p(_f32vec(att_src, heads * c, "att_src")), _p(_f32vec(att_dst, heads * c, "att_dst")), n, heads, c,
                             dcode(xp), int(mean), p, seed, _p(r_ws), _p(da_src), _p(da_dst), _p(dxp), dxp.stride(0), _stream()),
