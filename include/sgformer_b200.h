@@ -8,7 +8,7 @@
  *     (workspaces are passed in; *_ws_bytes tells the size);
  *   - sums across thread blocks are deterministic (fixed order, no float atomics): a result is bit-identical
  *     from run to run.  The launchers that sum columns or a loss across blocks (sgf_colstats, sgf_ln_bwd,
- *     sgf_ln_bwd_attn, sgf_bn_bwd_reduce, sgf_bn_bwd_apply, sgf_pack_operand with colsum, sgf_softmax_nll)
+ *     sgf_ln_bwd_attn, sgf_bn_bwd_reduce(_jk), sgf_bn_bwd_apply(_jk), sgf_pack_operand with colsum, sgf_softmax_nll)
  *     take a device workspace `ws` of at least sgf_reduce_ws_bytes(width) bytes (16-byte aligned; width = h,
  *     cols, or 1 for the loss) that holds the blocks' partials and arrival counters; the launcher resets the
  *     counters on `stream`.  Calls whose kernels may run at the same time need distinct workspaces;
@@ -373,6 +373,29 @@ int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* row_scale2, c
                      global node count when row-sharded and `sums` was all-reduced) */, const float* sums, void* dz,
                      void* dres, int dres_accumulate, float* dz_colsum, const float* out_row_scale, void* ws,
                      size_t ws_bytes, void* stream);
+
+/* Jumping knowledge over a GCN stack (GCNJK, medium/models.py:157-205), fused into the BatchNorm passes.  jk_mode: 1 max, 2 cat
+ * (0 is refused: use the entry points above).  `jk` has the activation dtype, pitch ld_jk (elements; 16-byte aligned rows);
+ * jk_idx (max only) is uint8 with the same pitch in bytes.  jk_layer = the layer index l (0..255) of the call.
+ * sgf_bn_fwd_jk: sgf_bn_fwd without res/mix/y_scaled; a = act(BN(z + zbias)) before dropout, rounded to the dtype, is
+ *   max: l == 0: jk = a, jk_idx = 0;  l > 0: where a > jk (strictly; a tie keeps the lower layer): jk = a, jk_idx = l;
+ *   cat: jk[r, :] = a (`jk` points at column block l of the [rows, L*h] concatenation);
+ *   y (nullable) = dropout(a) as in sgf_bn_fwd.
+ * sgf_bn_bwd_reduce_jk / sgf_bn_bwd_apply_jk: sgf_bn_bwd_reduce / _apply with dy2, dres = NULL and gscale = 1, and the upstream
+ *   gradient g = dropout mask * dy (dy nullable) + JK addend, then * act'; the addend is jk[r, c] where jk_idx[r, c] == l (max)
+ *   or jk[r, c] (cat: block l of g_out W^T).  dz_colsum includes the addend. */
+int sgf_bn_fwd_jk(const void* z, int64_t ld, int64_t rows, int h, int dtype, const float* mean, const float* rstd,
+                  const float* gamma, const float* beta, const float* zbias, int use_bn, int use_relu, float p, uint64_t seed,
+                  void* y, int jk_mode, void* jk, int64_t ld_jk, uint8_t* jk_idx, int jk_layer, void* stream);
+int sgf_bn_bwd_reduce_jk(const void* dy, const void* z, int64_t ld, int64_t rows, int h, int dtype, const float* mean,
+                         const float* rstd, const float* gamma, const float* beta, const float* zbias, int use_bn, int use_relu,
+                         float p, uint64_t seed, float* sums, int jk_mode, const void* jk_g, int64_t ld_jk, const uint8_t* jk_idx,
+                         int jk_layer, void* ws, size_t ws_bytes, void* stream);
+int sgf_bn_bwd_apply_jk(const void* dy, const void* z, int64_t ld, int64_t rows, int h, int dtype, const float* mean,
+                        const float* rstd, const float* gamma, const float* beta, const float* zbias, int use_bn, int use_relu,
+                        int training, float p, uint64_t seed, const float* sums, void* dz, float* dz_colsum,
+                        const float* out_row_scale, int jk_mode, const void* jk_g, int64_t ld_jk, const uint8_t* jk_idx,
+                        int jk_layer, void* ws, size_t ws_bytes, void* stream);
 
 /* out = (a*x + b*y) * row_scale[r]  (y, row_scale nullable; y has x's dtype); in/out dtypes may differ (casts). */
 int sgf_axpby(const void* x, int64_t ldx, int x_dtype, const void* y, int64_t ldy, int y_dtype, float a, float b,

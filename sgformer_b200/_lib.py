@@ -140,6 +140,12 @@ _SIGS = {
                                     C.c_int, _f32, _u64, _f32, _vp, _vp, _sz, _vp]),
     "sgf_bn_bwd_apply": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int,
                                    C.c_int, C.c_int, _f32, _u64, _f32, _i64, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _sz, _vp]),
+    "sgf_bn_fwd_jk": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _f32, _u64, _vp,
+                                C.c_int, _vp, _i64, _vp, C.c_int, _vp]),
+    "sgf_bn_bwd_reduce_jk": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _f32,
+                                       _u64, _vp, C.c_int, _vp, _i64, _vp, C.c_int, _vp, _sz, _vp]),
+    "sgf_bn_bwd_apply_jk": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int,
+                                      C.c_int, _f32, _u64, _vp, _vp, _vp, _vp, C.c_int, _vp, _i64, _vp, C.c_int, _vp, _sz, _vp]),
     "sgf_axpby": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _f32, _f32, _vp, _vp, _i64, C.c_int, _i64, C.c_int,
                             _vp]),
     "sgf_pack_operand": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _i64, C.c_int, _i64, _vp, _vp, _vp, _sz, _vp]),

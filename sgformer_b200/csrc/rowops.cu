@@ -619,7 +619,100 @@ __global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* _
     }
 }
 
-template <typename T, int CPL, bool DROP>
+// Jumping knowledge over a GCN stack (GCNJK, medium/models.py:157-205), fused into the BatchNorm passes the GCN schedule makes.
+// kJkMax: `buf` [rows, ld] (activation dtype) holds the running element-wise maximum over the layers' activations and `idx`
+// [rows, ld] (uint8) the layer it came from.  Layer 0 initialises both; layer l > 0 replaces an element only when its value is
+// strictly greater, so a tie keeps the lowest layer index (torch.max's first maximal index).  Values are compared as stored
+// (rounded to the activation dtype).  kJkCat: `buf` is layer l's column block of the [rows, L*h] concatenation (pitch ld).
+// Backward: the JK gradient g (`buf`) is added to the gradient of layer l's activation after the dropout mask (JK reads the
+// pre-dropout value): where idx == l (kJkMax), or everywhere (kJkCat, g = column block l of g_out W^T).
+constexpr int kJkNone = 0, kJkMax = 1, kJkCat = 2;
+struct JkArgs {
+    void* buf;
+    int64_t ld;
+    uint8_t* idx;
+    int layer;
+};
+
+template <int VN>
+__device__ __forceinline__ void ld_idx(const uint8_t* p, uint8_t (&b)[VN]) {
+    if constexpr (VN == 4) {
+        const uint32_t u = *reinterpret_cast<const uint32_t*>(p);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) b[i] = (uint8_t)(u >> (8 * i));
+    } else {
+        const uint2 u = *reinterpret_cast<const uint2*>(p);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { b[i] = (uint8_t)(u.x >> (8 * i)); b[4 + i] = (uint8_t)(u.y >> (8 * i)); }
+    }
+}
+template <int VN>
+__device__ __forceinline__ void st_idx(uint8_t* p, const uint8_t (&b)[VN]) {
+    if constexpr (VN == 4) {
+        *reinterpret_cast<uint32_t*>(p) = (uint32_t)b[0] | ((uint32_t)b[1] << 8) | ((uint32_t)b[2] << 16) | ((uint32_t)b[3] << 24);
+    } else {
+        uint2 u;
+        u.x = (uint32_t)b[0] | ((uint32_t)b[1] << 8) | ((uint32_t)b[2] << 16) | ((uint32_t)b[3] << 24);
+        u.y = (uint32_t)b[4] | ((uint32_t)b[5] << 8) | ((uint32_t)b[6] << 16) | ((uint32_t)b[7] << 24);
+        *reinterpret_cast<uint2*>(p) = u;
+    }
+}
+
+template <typename T, int CPL, int JK>
+__device__ __forceinline__ void jk_fwd_row(const Lane<T, CPL>& L, const float (&v)[CPL][Vec16<T>::N], const JkArgs& jk, int64_t r) {
+    constexpr int VN = Vec16<T>::N;
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) {
+        if (!L.cval[c]) continue;
+        const int64_t o = r * jk.ld + L.coff[c];
+        T* bp = static_cast<T*>(jk.buf) + o;
+        const uint4 pa = Vec16<T>::pack(v[c]);
+        if constexpr (JK == kJkCat) {
+            stg_na(bp, pa);
+        } else {
+            uint8_t id[VN];
+            if (jk.layer == 0) {
+#pragma unroll
+                for (int i = 0; i < VN; ++i) id[i] = 0;
+                stg_na(bp, pa);
+            } else {
+                float a[VN], m[VN];
+                Vec16<T>::unpack(pa, a);
+                Vec16<T>::unpack(*reinterpret_cast<const uint4*>(bp), m);
+                ld_idx<VN>(jk.idx + o, id);
+#pragma unroll
+                for (int i = 0; i < VN; ++i)
+                    if (a[i] > m[i]) { m[i] = a[i]; id[i] = (uint8_t)jk.layer; }
+                stg_na(bp, Vec16<T>::pack(m));
+            }
+            st_idx<VN>(jk.idx + o, id);
+        }
+    }
+}
+
+// gy += the JK gradient of row r (see above)
+template <typename T, int CPL, int JK>
+__device__ __forceinline__ void jk_bwd_row(const Lane<T, CPL>& L, float (&gy)[CPL][Vec16<T>::N], const JkArgs& jk, int64_t r) {
+    constexpr int VN = Vec16<T>::N;
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) {
+        if (!L.cval[c]) continue;
+        const int64_t o = r * jk.ld + L.coff[c];
+        float t[VN];
+        Vec16<T>::unpack(ldg_nc_na(static_cast<const T*>(jk.buf) + o), t);
+        if constexpr (JK == kJkMax) {
+            uint8_t id[VN];
+            ld_idx<VN>(jk.idx + o, id);
+#pragma unroll
+            for (int i = 0; i < VN; ++i) gy[c][i] += id[i] == (uint8_t)jk.layer ? t[i] : 0.f;
+        } else {
+#pragma unroll
+            for (int i = 0; i < VN; ++i) gy[c][i] += t[i];
+        }
+    }
+}
+
+template <typename T, int CPL, bool DROP, int JK = kJkNone>
 __global__ void __launch_bounds__(kRowBlock, 3) bn_fwd_kernel(const T* __restrict__ z, const T* __restrict__ res, const T* __restrict__ mix,
                                                             int64_t ld, int64_t rows, int h, int chunks, int lpr_log2,
                                                             const float* __restrict__ mean, const float* __restrict__ rstd,
@@ -627,7 +720,7 @@ __global__ void __launch_bounds__(kRowBlock, 3) bn_fwd_kernel(const T* __restric
                                                             const float* __restrict__ zbias, int use_bn,
                                                             int use_relu, float p, SeedArg seed_arg, float gw,
                                                             const float* __restrict__ row_scale, T* __restrict__ y,
-                                                            T* __restrict__ y_scaled) {
+                                                            T* __restrict__ y_scaled, JkArgs jk) {
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     Lane<T, CPL> L(chunks, lpr_log2);
@@ -664,6 +757,7 @@ __global__ void __launch_bounds__(kRowBlock, 3) bn_fwd_kernel(const T* __restric
         SGF_FOR_ELEMS v[c][i] = v[c][i] * sc[c][i] + sh[c][i];
         if (use_relu == kActElu) SGF_FOR_ELEMS v[c][i] = v[c][i] > 0.f ? v[c][i] : expm1f(v[c][i]);
         else if (use_relu) SGF_FOR_ELEMS v[c][i] = fmaxf(v[c][i], 0.f);
+        if constexpr (JK != kJkNone) jk_fwd_row<T, CPL, JK>(L, v, jk, r);      // the pre-dropout activation
         if (DROP) L.dropout(v, seed, r, chunks, thr16, inv_keep);
         if (res) SGF_FOR_ELEMS v[c][i] += tr[c][i];
         if (y_scaled) {
@@ -683,7 +777,7 @@ __global__ void __launch_bounds__(kRowBlock, 3) bn_fwd_kernel(const T* __restric
 // of one row of packed registers: at 123-128 registers the kernel holds 2 CTAs = 16 warps per SM, and one 512-byte row per warp and
 // tensor in flight is 16-32 KB per SM - ncu (r2l): 45 % (reduce) / 57-62 % (apply) of the DRAM peak at 25 % occupancy.
 constexpr int kRingDepth = 4, kRingTensors = 4;
-template <typename T, int CPL, bool APPLY, bool DROP, bool RING>
+template <typename T, int CPL, bool APPLY, bool DROP, bool RING, int JK = kJkNone>
 __global__ void __launch_bounds__(kRowBlock, 2) bn_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ dy2,
                                                                const float* __restrict__ rs2, const T* __restrict__ z, int64_t ld,
                                                                int64_t rows, int h, int chunks, int lpr_log2, const float* __restrict__ mean,
@@ -693,7 +787,8 @@ __global__ void __launch_bounds__(kRowBlock, 2) bn_bwd_kernel(const T* __restric
                                                                int64_t stat_rows, float* __restrict__ sums, T* __restrict__ dz,
                                                                T* __restrict__ dres,
                                                                int dres_acc, float* __restrict__ dz_colsum,
-                                                               const float* __restrict__ out_scale, RedWs red) {
+                                                               const float* __restrict__ out_scale, RedWs red, JkArgs jk) {
+    static_assert(JK == kJkNone || !RING, "the JK addend is read by the register pipeline");
     const uint64_t seed = DROP ? seed_arg.get() : 0;
     constexpr int VN = Vec16<T>::N;
     extern __shared__ float sm[];
@@ -825,6 +920,7 @@ __global__ void __launch_bounds__(kRowBlock, 2) bn_bwd_kernel(const T* __restric
             }
         }
         if (DROP) L.dropout(gy, seed, r, chunks, thr16, inv_keep);
+        if constexpr (JK != kJkNone) jk_bwd_row<T, CPL, JK>(L, gy, jk, r);
         const float os = (APPLY && out_scale) ? out_scale[r] : 1.f;
         SGF_FOR_ELEMS {
             const float zv = zz[c][i];
@@ -1409,10 +1505,26 @@ extern "C" int sgf_bn_finalize(const float* sum, const float* sumsq, int64_t row
     return SGF_OK;
 }
 
-extern "C" int sgf_bn_fwd(const void* z, const void* res, const void* mix, int64_t ld, int64_t rows, int h, int dtype,
-                          const float* mean, const float* rstd, const float* gamma, const float* beta, const float* zbias,
-                          int use_bn, int use_relu, float p, uint64_t seed, float gw, const float* row_scale, void* y,
-                          void* y_scaled, void* stream) {
+// the JK modes as template instances: the mode-0 instances are the plain BatchNorm kernels
+#define SGF_DISPATCH_JK(mode, ...)                                                             \
+    do {                                                                                       \
+        if ((mode) == kJkMax) { constexpr int JK = kJkMax; __VA_ARGS__; }                      \
+        else if ((mode) == kJkCat) { constexpr int JK = kJkCat; __VA_ARGS__; }                 \
+        else { constexpr int JK = kJkNone; __VA_ARGS__; }                                      \
+    } while (0)
+
+static int jk_check(int jk_mode, int dtype, const JkArgs& jk) {
+    if (jk_mode == kJkNone) return SGF_OK;
+    if (jk_mode != kJkMax && jk_mode != kJkCat) return SGF_ERR_ARG;
+    if (!jk.buf || !aligned16(jk.buf) || !ld_ok(dtype, jk.ld) || jk.layer < 0 || jk.layer > 255) return SGF_ERR_ARG;
+    if (jk_mode == kJkMax && (!jk.idx || (reinterpret_cast<uintptr_t>(jk.idx) & (dtype == 0 ? 3 : 7)))) return SGF_ERR_ARG;
+    return SGF_OK;
+}
+
+static int bn_fwd_launch(const void* z, const void* res, const void* mix, int64_t ld, int64_t rows, int h, int dtype,
+                         const float* mean, const float* rstd, const float* gamma, const float* beta, const float* zbias,
+                         int use_bn, int use_relu, float p, uint64_t seed, float gw, const float* row_scale, void* y,
+                         void* y_scaled, int jk_mode, JkArgs jk, void* stream) {
     RowGeom g;
     if (!geom_for(dtype, h, g) || !aligned16(z) || !aligned16(res) || !aligned16(mix) || !aligned16(y) || !aligned16(y_scaled) ||
         !ld_ok(dtype, ld) || rows < 0)
@@ -1420,11 +1532,63 @@ extern "C" int sgf_bn_fwd(const void* z, const void* res, const void* mix, int64
     if (use_bn && (!mean || !rstd || !gamma || !beta)) return SGF_ERR_ARG;
     if (y_scaled && !row_scale) return SGF_ERR_ARG;
     if (p < 0.f || p >= 1.f) return SGF_ERR_ARG;
+    if (int rc = jk_check(jk_mode, dtype, jk)) return rc;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_fwd_kernel<T, CPL, DROP><<<row_grid(rows, g), kRowBlock, 0, st>>>(
+    SGF_DISPATCH_JK(jk_mode, SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_fwd_kernel<T, CPL, DROP, JK><<<row_grid(rows, g), kRowBlock, 0, st>>>(
                                          (const T*)z, (const T*)res, (const T*)mix, ld, rows, h, g.chunks, g.lpr_log2, mean, rstd,
-                                         gamma, beta, zbias, use_bn, use_relu, p, seed, gw, row_scale, (T*)y, (T*)y_scaled)));
+                                         gamma, beta, zbias, use_bn, use_relu, p, seed, gw, row_scale, (T*)y, (T*)y_scaled, jk))));
+    SGF_LAUNCH_CHECK(); count_launch();
+    return SGF_OK;
+}
+
+extern "C" int sgf_bn_fwd(const void* z, const void* res, const void* mix, int64_t ld, int64_t rows, int h, int dtype,
+                          const float* mean, const float* rstd, const float* gamma, const float* beta, const float* zbias,
+                          int use_bn, int use_relu, float p, uint64_t seed, float gw, const float* row_scale, void* y,
+                          void* y_scaled, void* stream) {
+    return bn_fwd_launch(z, res, mix, ld, rows, h, dtype, mean, rstd, gamma, beta, zbias, use_bn, use_relu, p, seed, gw, row_scale, y,
+                         y_scaled, kJkNone, JkArgs{nullptr, 0, nullptr, 0}, stream);
+}
+
+extern "C" int sgf_bn_fwd_jk(const void* z, int64_t ld, int64_t rows, int h, int dtype, const float* mean, const float* rstd,
+                             const float* gamma, const float* beta, const float* zbias, int use_bn, int use_relu, float p,
+                             uint64_t seed, void* y, int jk_mode, void* jk, int64_t ld_jk, uint8_t* jk_idx, int jk_layer,
+                             void* stream) {
+    if (jk_mode == kJkNone) return SGF_ERR_ARG;
+    return bn_fwd_launch(z, nullptr, nullptr, ld, rows, h, dtype, mean, rstd, gamma, beta, zbias, use_bn, use_relu, p, seed, 1.f,
+                         nullptr, y, nullptr, jk_mode, JkArgs{jk, ld_jk, jk_idx, jk_layer}, stream);
+}
+
+static int bn_bwd_reduce_launch(const void* dy, const void* dy2, const float* row_scale2, const void* z, int64_t ld, int64_t rows,
+                                int h, int dtype, const float* mean, const float* rstd, const float* gamma, const float* beta,
+                                const float* zbias, int use_bn, int use_relu, float p, uint64_t seed, float gscale, float* sums,
+                                int jk_mode, JkArgs jk, void* ws, size_t ws_bytes, void* stream) {
+    RowGeom g;
+    if (!geom_for(dtype, h, g) || !aligned16(dy) || !aligned16(dy2) || !aligned16(z) || !ld_ok(dtype, ld) || rows < 0 || !sums ||
+        (!dy && !dy2 && jk_mode == kJkNone))
+        return SGF_ERR_ARG;
+    if (use_bn && (!mean || !rstd || !gamma || !beta)) return SGF_ERR_ARG;
+    if (int rc = jk_check(jk_mode, dtype, jk)) return rc;
+    if (rows == 0) return SGF_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    RedWs red;
+    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
+    if (g.cpl == 1 && bn_bwd_ring() && jk_mode == kJkNone) {
+        const size_t smem = bn_bwd_ring_smem(h);
+        SGF_DISPATCH_T_DROP(dtype, p > 0.f, {
+            SGF_CUDA_TRY(cudaFuncSetAttribute(bn_bwd_kernel<T, 1, false, DROP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            bn_bwd_kernel<T, 1, false, DROP, true><<<row_grid(rows, g), kRowBlock, smem, st>>>(
+                (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean, rstd, gamma, beta, zbias,
+                use_bn, use_relu, 1, p, seed, gscale, (int64_t)0, sums, (T*)nullptr, (T*)nullptr, 0, (float*)nullptr,
+                (const float*)nullptr, red, jk);
+        });
+        SGF_LAUNCH_CHECK(); count_launch();
+        return SGF_OK;
+    }
+    SGF_DISPATCH_JK(jk_mode, SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_bwd_kernel<T, CPL, false, DROP, false, JK><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
+                                         (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean,
+                                         rstd, gamma, beta, zbias, use_bn, use_relu, 1, p, seed, gscale, (int64_t)0, sums,
+                                         (T*)nullptr, (T*)nullptr, 0, (float*)nullptr, (const float*)nullptr, red, jk))));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1433,31 +1597,43 @@ extern "C" int sgf_bn_bwd_reduce(const void* dy, const void* dy2, const float* r
                                  int h, int dtype, const float* mean, const float* rstd, const float* gamma, const float* beta,
                                  const float* zbias, int use_bn, int use_relu, float p, uint64_t seed, float gscale, float* sums,
                                  void* ws, size_t ws_bytes, void* stream) {
+    return bn_bwd_reduce_launch(dy, dy2, row_scale2, z, ld, rows, h, dtype, mean, rstd, gamma, beta, zbias, use_bn, use_relu, p, seed,
+                                gscale, sums, kJkNone, JkArgs{nullptr, 0, nullptr, 0}, ws, ws_bytes, stream);
+}
+
+static int bn_bwd_apply_launch(const void* dy, const void* dy2, const float* row_scale2, const void* z, int64_t ld, int64_t rows,
+                               int h, int dtype, const float* mean, const float* rstd, const float* gamma, const float* beta,
+                               const float* zbias, int use_bn, int use_relu, int training, float p, uint64_t seed, float gscale,
+                               int64_t stat_rows, const float* sums, void* dz, void* dres, int dres_accumulate,
+                               float* dz_colsum, const float* out_row_scale, int jk_mode, JkArgs jk, void* ws, size_t ws_bytes,
+                               void* stream) {
     RowGeom g;
-    if (!geom_for(dtype, h, g) || !aligned16(dy) || !aligned16(dy2) || !aligned16(z) || !ld_ok(dtype, ld) || rows < 0 || !sums ||
-        (!dy && !dy2))
+    if (!geom_for(dtype, h, g) || !aligned16(dy) || !aligned16(dy2) || !aligned16(z) || !aligned16(dz) || !aligned16(dres) ||
+        !ld_ok(dtype, ld) || rows < 0 || (!dy && !dy2 && jk_mode == kJkNone))
         return SGF_ERR_ARG;
     if (use_bn && (!mean || !rstd || !gamma || !beta)) return SGF_ERR_ARG;
+    if (use_bn && training && !sums) return SGF_ERR_ARG;
+    if (int rc = jk_check(jk_mode, dtype, jk)) return rc;
     if (rows == 0) return SGF_OK;
     cudaStream_t st = (cudaStream_t)stream;
     RedWs red;
     if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
-    if (g.cpl == 1 && bn_bwd_ring()) {
+    if (g.cpl == 1 && bn_bwd_ring() && jk_mode == kJkNone) {
         const size_t smem = bn_bwd_ring_smem(h);
         SGF_DISPATCH_T_DROP(dtype, p > 0.f, {
-            SGF_CUDA_TRY(cudaFuncSetAttribute(bn_bwd_kernel<T, 1, false, DROP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            bn_bwd_kernel<T, 1, false, DROP, true><<<row_grid(rows, g), kRowBlock, smem, st>>>(
+            SGF_CUDA_TRY(cudaFuncSetAttribute(bn_bwd_kernel<T, 1, true, DROP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            bn_bwd_kernel<T, 1, true, DROP, true><<<row_grid(rows, g), kRowBlock, smem, st>>>(
                 (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean, rstd, gamma, beta, zbias,
-                use_bn, use_relu, 1, p, seed, gscale, (int64_t)0, sums, (T*)nullptr, (T*)nullptr, 0, (float*)nullptr,
-                (const float*)nullptr, red);
+                use_bn, use_relu, training, p, seed, gscale, stat_rows, const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate,
+                dz_colsum, out_row_scale, red, jk);
         });
         SGF_LAUNCH_CHECK(); count_launch();
         return SGF_OK;
     }
-    SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_bwd_kernel<T, CPL, false, DROP, false><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
+    SGF_DISPATCH_JK(jk_mode, SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_bwd_kernel<T, CPL, true, DROP, false, JK><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
                                          (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean,
-                                         rstd, gamma, beta, zbias, use_bn, use_relu, 1, p, seed, gscale, (int64_t)0, sums,
-                                         (T*)nullptr, (T*)nullptr, 0, (float*)nullptr, (const float*)nullptr, red)));
+                                         rstd, gamma, beta, zbias, use_bn, use_relu, training, p, seed, gscale, stat_rows,
+                                         const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate, dz_colsum, out_row_scale, red, jk))));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }
@@ -1468,34 +1644,30 @@ extern "C" int sgf_bn_bwd_apply(const void* dy, const void* dy2, const float* ro
                                 int64_t stat_rows, const float* sums, void* dz, void* dres, int dres_accumulate,
                                 float* dz_colsum, const float* out_row_scale, void* ws, size_t ws_bytes,
                                 void* stream) {
-    RowGeom g;
-    if (!geom_for(dtype, h, g) || !aligned16(dy) || !aligned16(dy2) || !aligned16(z) || !aligned16(dz) || !aligned16(dres) ||
-        !ld_ok(dtype, ld) || rows < 0 || (!dy && !dy2))
-        return SGF_ERR_ARG;
-    if (use_bn && (!mean || !rstd || !gamma || !beta)) return SGF_ERR_ARG;
-    if (use_bn && training && !sums) return SGF_ERR_ARG;
-    if (rows == 0) return SGF_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    RedWs red;
-    if (int rc = red_args(ws, ws_bytes, h, st, red)) return rc;
-    if (g.cpl == 1 && bn_bwd_ring()) {
-        const size_t smem = bn_bwd_ring_smem(h);
-        SGF_DISPATCH_T_DROP(dtype, p > 0.f, {
-            SGF_CUDA_TRY(cudaFuncSetAttribute(bn_bwd_kernel<T, 1, true, DROP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            bn_bwd_kernel<T, 1, true, DROP, true><<<row_grid(rows, g), kRowBlock, smem, st>>>(
-                (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean, rstd, gamma, beta, zbias,
-                use_bn, use_relu, training, p, seed, gscale, stat_rows, const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate,
-                dz_colsum, out_row_scale, red);
-        });
-        SGF_LAUNCH_CHECK(); count_launch();
-        return SGF_OK;
-    }
-    SGF_DISPATCH_T_CPL_DROP(dtype, g.cpl, p > 0.f, (bn_bwd_kernel<T, CPL, true, DROP, false><<<row_grid(rows, g), kRowBlock, h * sizeof(float), st>>>(
-                                         (const T*)dy, (const T*)dy2, row_scale2, (const T*)z, ld, rows, h, g.chunks, g.lpr_log2, mean,
-                                         rstd, gamma, beta, zbias, use_bn, use_relu, training, p, seed, gscale, stat_rows,
-                                         const_cast<float*>(sums), (T*)dz, (T*)dres, dres_accumulate, dz_colsum, out_row_scale, red)));
-    SGF_LAUNCH_CHECK(); count_launch();
-    return SGF_OK;
+    return bn_bwd_apply_launch(dy, dy2, row_scale2, z, ld, rows, h, dtype, mean, rstd, gamma, beta, zbias, use_bn, use_relu, training, p,
+                               seed, gscale, stat_rows, sums, dz, dres, dres_accumulate, dz_colsum, out_row_scale, kJkNone,
+                               JkArgs{nullptr, 0, nullptr, 0}, ws, ws_bytes, stream);
+}
+
+extern "C" int sgf_bn_bwd_reduce_jk(const void* dy, const void* z, int64_t ld, int64_t rows, int h, int dtype, const float* mean,
+                                    const float* rstd, const float* gamma, const float* beta, const float* zbias, int use_bn,
+                                    int use_relu, float p, uint64_t seed, float* sums, int jk_mode, const void* jk_g, int64_t ld_jk,
+                                    const uint8_t* jk_idx, int jk_layer, void* ws, size_t ws_bytes, void* stream) {
+    if (jk_mode == kJkNone) return SGF_ERR_ARG;
+    return bn_bwd_reduce_launch(dy, nullptr, nullptr, z, ld, rows, h, dtype, mean, rstd, gamma, beta, zbias, use_bn, use_relu, p, seed,
+                                1.f, sums, jk_mode, JkArgs{const_cast<void*>(jk_g), ld_jk, const_cast<uint8_t*>(jk_idx), jk_layer},
+                                ws, ws_bytes, stream);
+}
+
+extern "C" int sgf_bn_bwd_apply_jk(const void* dy, const void* z, int64_t ld, int64_t rows, int h, int dtype, const float* mean,
+                                   const float* rstd, const float* gamma, const float* beta, const float* zbias, int use_bn,
+                                   int use_relu, int training, float p, uint64_t seed, const float* sums, void* dz, float* dz_colsum,
+                                   const float* out_row_scale, int jk_mode, const void* jk_g, int64_t ld_jk, const uint8_t* jk_idx,
+                                   int jk_layer, void* ws, size_t ws_bytes, void* stream) {
+    if (jk_mode == kJkNone) return SGF_ERR_ARG;
+    return bn_bwd_apply_launch(dy, nullptr, nullptr, z, ld, rows, h, dtype, mean, rstd, gamma, beta, zbias, use_bn, use_relu, training, p,
+                               seed, 1.f, 0, sums, dz, nullptr, 0, dz_colsum, out_row_scale, jk_mode,
+                               JkArgs{const_cast<void*>(jk_g), ld_jk, const_cast<uint8_t*>(jk_idx), jk_layer}, ws, ws_bytes, stream);
 }
 
 static inline int ew_grid(int64_t total) {

@@ -72,6 +72,7 @@ _SEED_GCN_LAYER = 503       # + i: GCN layer i
 _SEED_GAT_INPUT = 601       # GAT input dropout
 _SEED_GAT_ACT = 611         # + i: dropout after GAT layer i's ELU
 _SEED_GAT_ATT = 653         # + i: attention dropout of GAT layer i
+_SEED_GCNJK_LAYER = 701     # + i: GCNJK layer i
 
 
 def check_width(h: int, prec: Precision, what: str):
@@ -827,6 +828,132 @@ def gcn_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Pre
         elif want_dx:
             dx = torch.empty((n, L["cur_k"]), dtype=torch.float32, device=dev)
             K.gemm_nt([u_op], [_w(P, wname, prec, transpose=True)], [(0, 0, 0, 0, hout)], L["cur_k"], dx)
+    return dx
+
+
+# =================================================================================================
+# GCNJK baseline (medium): GCNConv stack + jumping knowledge + final Linear
+# =================================================================================================
+# models.GCNJK (medium/models.py:157-205) is the GCN stack above with BatchNorm on every conv but the last, no edge weights, and
+# xs = [a_0 .. a_{L-1}] (each hidden layer's activation BEFORE its dropout, and the last conv's output) aggregated by
+# JumpingKnowledge: 'max' = element-wise max over the layers (gradient to the first maximal layer), 'cat' = concatenation; then
+# final_project.  The aggregation rides in the layers' bn_fwd passes (sgf_bn_fwd_jk: running max + uint8 layer index, or the
+# layer's column block of the concatenation) and its gradient in their bn_bwd passes (sgf_bn_bwd_*_jk: an addend of dy after the
+# dropout mask); the last conv's bias pass is a bn_fwd without BN/ReLU and finalises the max in place.  DESIGN.md §4.12.
+def _gcnjk_dims(P, pfx: str, nl: int, jk: str):
+    h = P[f"{pfx}convs.0.lin.weight"].shape[0]
+    kfp = P[f"{pfx}final_project.weight"].shape[1]
+    if kfp != (h * nl if jk == "cat" else h):
+        raise ValueError(f"sgformer_b200: GCNJK final_project takes {kfp} inputs, but JumpingKnowledge('{jk}') over {nl} layers of "
+                         f"{h} channels gives {h * nl if jk == 'cat' else h}")
+    return h, kfp
+
+
+def gcnjk_forward(P, cfg: dict, xin: K.Operand, graph: Graph, prec: Precision, training: bool, seed: int,
+                  tape: Optional[Tape], mix: Optional[Tensor] = None, gw: float = 1.0, pfx: str = "gnn.",
+                  comm: Comm = SINGLE, out_dtype=torch.float32) -> Tensor:
+    """models.GCNJK.forward -> final_project(JK(xs)) [N, out] in `out_dtype` (gw*that + (1-gw)*mix when `mix` is given).  `graph`:
+    the GCN's self-loop mode 1 graph, unweighted (GCNJK passes no edge weight)."""
+    if comm.active:
+        raise NotImplementedError("sgformer_b200: row sharding of GCNJK is not supported")
+    nl, jk = cfg["gcn_num_layers"], cfg["gcn_jk"]
+    n = xin.rows
+    dev = xin.data.device
+    p = float(cfg["gcn_dropout"]) if training else 0.0
+    h, kfp = _gcnjk_dims(P, pfx, nl, jk)
+    check_width(h, prec, "GCNJK hidden_channels")
+    if nl > 256:
+        raise ValueError("sgformer_b200: GCNJK runs at most 256 layers (uint8 layer index)")
+    dinv = graph.dinv
+    idx = None
+    if jk == "max":
+        jbuf = K.alloc_act(n, h, prec.act_dtype, dev)
+        idx = torch.empty((n, jbuf.stride(0)), dtype=torch.uint8, device=dev)
+    else:
+        jbuf = K.alloc_act(n, nl * h, prec.act_dtype, dev)
+    cur_op, cur_k = xin, cfg["in_channels"]
+    layers = []
+    for i in range(nl):
+        last = i == nl - 1
+        t = K.gemm_nt([cur_op], [_w(P, f"{pfx}convs.{i}.lin.weight", prec)], [(0, 0, 0, 0, cur_k)], h,
+                      K.alloc_act(n, h, prec.act_dtype, dev), row_scale=dinv)
+        s = _gcn_spmm(graph, False, dinv, t, comm)
+        zb = P[f"{pfx}convs.{i}.bias"]
+        blk = jbuf if jk == "max" else jbuf[:, i * h:(i + 1) * h]
+        L = dict(s=s, cur_op=cur_op, cur_k=cur_k)
+        if last:
+            K.bn_fwd_jk(s, None, None, None, None, zb, False, False, 0.0, 0, False, jk, blk, idx, i)
+        else:
+            name = f"{pfx}bns.{i}."
+            mean, rstd = _bn_stats(s, P, name, True, training, zbias=zb)
+            # 'cat' without dropout: the next conv reads the activation from its block of the concatenation
+            want_y = jk == "max" or p > 0.0
+            y = K.bn_fwd_jk(s, mean, rstd, P[name + "weight"], P[name + "bias"], zb, True, True, p, seed + _SEED_GCNJK_LAYER + i,
+                            want_y, jk, blk, idx, i)
+            L.update(mean=mean, rstd=rstd)
+            cur_op, cur_k = K.as_operand(y if want_y else blk, prec.planes), h
+        layers.append(L)
+    jk_op = K.as_operand(jbuf, prec.planes)
+    c = P[f"{pfx}final_project.weight"].shape[0]
+    out = K.alloc_act(n, c, out_dtype, dev)
+    K.gemm_nt([jk_op], [_w(P, f"{pfx}final_project.weight", prec)], [(0, 0, 0, 0, kfp)], c, out, bias=P[f"{pfx}final_project.bias"])
+    if mix is not None:
+        out = K.axpby(out, mix, gw, 1.0 - gw)
+    if tape is not None:
+        tape.update(layers=layers, jk_op=jk_op, idx=idx, h=h, kfp=kfp, p=p, seed=seed, n=n, training=training,
+                    mixed=mix is not None, gw=gw)
+    return out
+
+
+def gcnjk_backward(P, cfg: dict, tape: Tape, graph: Graph, dout: Tensor, prec: Precision, grads: Dict[str, Tensor],
+                   pfx: str = "gnn.", want_dx: bool = False, comm: Comm = SINGLE) -> Optional[Tensor]:
+    nl, jk = cfg["gcn_num_layers"], cfg["gcn_jk"]
+    n, p, seed, training, h, kfp = tape["n"], tape["p"], tape["seed"], tape["training"], tape["h"], tape["kfp"]
+    dev = dout.device
+    gs = tape["gw"] if tape["mixed"] else 1.0
+    dinv = graph.dinv
+    # final_project: d bias = column sums of g_out (taken while packing), dW = g_out^T JK, g_jk = g_out W
+    if gs != 1.0 or dout.dtype != torch.float32 or dout.stride(-1) != 1:
+        dout = K.axpby(dout, None, gs, 0.0, out_dtype=torch.float32)
+    c = dout.shape[1]
+    db = torch.zeros(c, dtype=torch.float32, device=dev)
+    dl_op = K.pack_operand(dout, False, prec.planes, colsum=db)
+    wname = f"{pfx}final_project.weight"
+    dw = torch.empty((c, kfp), dtype=torch.float32, device=dev)
+    K.gemm_tn(dl_op, tape["jk_op"], dw)
+    grads[wname], grads[f"{pfx}final_project.bias"] = dw, db
+    g_jk = K.alloc_act(n, kfp, prec.act_dtype, dev)
+    K.gemm_nt([dl_op], [_w(P, wname, prec, transpose=True)], [(0, 0, 0, 0, c)], kfp, g_jk)
+    idx = tape["idx"]
+    dcur = None
+    dx = None
+    for i in reversed(range(nl)):
+        L = tape["layers"][i]
+        last = i == nl - 1
+        zb = P[f"{pfx}convs.{i}.bias"]
+        blk = g_jk if jk == "max" else g_jk[:, i * h:(i + 1) * h]
+        if last:
+            dzs, _, colsum = K.bn_bwd_jk(None, L["s"], None, None, None, None, zb, False, False, training, 0.0, 0, jk, blk, idx, i,
+                                         want_dz_colsum=True, out_row_scale=dinv)
+        else:
+            name = f"{pfx}bns.{i}."
+            dzs, sums, colsum = K.bn_bwd_jk(dcur, L["s"], L["mean"], L["rstd"], P[name + "weight"], P[name + "bias"], zb, True, True,
+                                            training, p, seed + _SEED_GCNJK_LAYER + i, jk, blk, idx, i, want_dz_colsum=True,
+                                            out_row_scale=dinv)
+            grads[name + "bias"], grads[name + "weight"] = sums[:h], sums[h:]
+        grads[f"{pfx}convs.{i}.bias"] = colsum
+        u = _gcn_spmm(graph, True, dinv, dzs, comm)        # = Â^T dz = gradient of (x W^T)
+        u_op = K.as_operand(u, prec.planes)
+        wname = f"{pfx}convs.{i}.lin.weight"
+        dw = torch.empty((h, L["cur_k"]), dtype=torch.float32, device=dev)
+        K.gemm_tn(u_op, L["cur_op"], dw)
+        grads[wname] = dw
+        if i > 0:
+            dcur = K.alloc_act(n, L["cur_k"], prec.act_dtype, dev)
+            K.gemm_nt([u_op], [_w(P, wname, prec, transpose=True)], [(0, 0, 0, 0, h)], L["cur_k"], dcur)
+        elif want_dx:
+            dx = torch.empty((n, L["cur_k"]), dtype=torch.float32, device=dev)
+            K.gemm_nt([u_op], [_w(P, wname, prec, transpose=True)], [(0, 0, 0, 0, h)], L["cur_k"], dx)
     return dx
 
 

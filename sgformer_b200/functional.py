@@ -79,6 +79,9 @@ def _from_act(t: Tensor, dtype) -> Tensor:
     return t.to(dtype)
 
 
+_MEDIUM_GNN_BACKWARD = {"gcn": E.gcn_backward, "gat": E.gat_backward, "gcnjk": E.gcnjk_backward}
+
+
 class SGFormerFn(_TapeFunction):
     """Fused encoder: logits = fc(mix(TransConv(x), GNN(x, graph))).  Returns fp32 [N, c]."""
 
@@ -103,6 +106,8 @@ class SGFormerFn(_TapeFunction):
                 fwd = E.gconv_forward
             elif cfg["gnn_kind"] == "gat":
                 fwd = functools.partial(E.gat_forward, x_raw=x)
+            elif cfg["gnn_kind"] == "gcnjk":
+                fwd = functools.partial(E.gcnjk_forward, out_dtype=prec.act_dtype)
             else:
                 fwd = E.gcn_forward
             x2 = fwd(P, cfg, xin, graph, prec, training, seed, tg, mix=x1 if add else None, gw=gw, comm=comm)
@@ -125,7 +130,7 @@ class SGFormerFn(_TapeFunction):
         gw = float(cfg["graph_weight"])
         dx = None
         if cfg["use_graph"]:
-            bwd = E.gconv_backward if cfg["variant"] != "medium" else E.gat_backward if cfg["gnn_kind"] == "gat" else E.gcn_backward
+            bwd = E.gconv_backward if cfg["variant"] != "medium" else _MEDIUM_GNN_BACKWARD[cfg["gnn_kind"]]
             if cfg["aggregate"] == "add":
                 dm = dfeats[0]
                 dxg = bwd(P, cfg, tg, graph, dm, prec, grads, want_dx=want_dx, comm=comm)
@@ -196,8 +201,8 @@ class TransConvFn(_TapeFunction):
 
 
 class GraphBranchFn(_TapeFunction):
-    """Standalone GNN branch: GraphConv (large/100M), the PyG-GCN or the PyG-GAT backbone (medium).  Returns [N, h] in x's
-    dtype."""
+    """Standalone GNN branch: GraphConv (large/100M), the PyG-GCN or the PyG-GAT backbone, or the GCNJK baseline (medium).
+    Returns [N, h] in x's dtype."""
 
     @staticmethod
     def forward(ctx, x, graph, cfg, prec, training, kind, pfx, names, *params):
@@ -207,7 +212,7 @@ class GraphBranchFn(_TapeFunction):
         if kind == "gat":
             fwd = functools.partial(E.gat_forward, x_raw=x)
         else:
-            fwd = E.gcn_forward if kind == "gcn" else E.gconv_forward
+            fwd = {"gcn": E.gcn_forward, "gcnjk": E.gcnjk_forward}.get(kind, E.gconv_forward)
         out = fwd(P, cfg, E.input_operand(x, prec), graph, prec, training, E.next_seed(), tape, pfx=pfx)
         if need_tape:
             ctx.state = (cfg, prec, graph, kind, pfx, names, params, tape, x.requires_grad)
@@ -217,8 +222,10 @@ class GraphBranchFn(_TapeFunction):
     def backward(ctx, dout):
         cfg, prec, graph, kind, pfx, names, params, tape, want_dx = ctx.state
         grads: Dict[str, Tensor] = {}
-        bwd = E.gat_backward if kind == "gat" else E.gcn_backward if kind == "gcn" else E.gconv_backward
-        dx = bwd(_pdict(names, params), cfg, tape, graph, _to_act(dout, prec), prec, grads, pfx=pfx, want_dx=want_dx)
+        bwd = {"gat": E.gat_backward, "gcn": E.gcn_backward, "gcnjk": E.gcnjk_backward}.get(kind, E.gconv_backward)
+        # GCNJK returns fp32 logits and takes their gradient as it comes
+        g = dout if kind == "gcnjk" else _to_act(dout, prec)
+        dx = bwd(_pdict(names, params), cfg, tape, graph, g, prec, grads, pfx=pfx, want_dx=want_dx)
         ctx.state = None
         return (dx, None, None, None, None, None, None, None, *_grad_list(names, params, grads))
 

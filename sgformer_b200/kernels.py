@@ -935,6 +935,64 @@ def bn_bwd_sums(dy, dy2, row_scale2, z: Tensor, mean, rstd, gamma, beta, zbias, 
     return sums
 
 
+JK_MAX, JK_CAT = 1, 2      # jk_mode of sgf_bn_fwd_jk / sgf_bn_bwd_*_jk
+_JK_MODES = {"max": JK_MAX, "cat": JK_CAT}
+
+
+def _jk_args(mode: str, buf: Tensor, idx: Optional[Tensor], layer: int, z: Tensor, name: str):
+    """(mode code, buf, pitch, idx) of a JK call, checked: `buf` has z's rows and width and the activation dtype; `idx` (max) is
+    uint8 with buf's pitch in bytes."""
+    code = _JK_MODES[mode]
+    rows, h, ld = _mat(buf, name)
+    if rows != z.shape[0] or h != z.shape[1] or buf.dtype != z.dtype or buf.device != z.device:
+        raise ValueError(f"{name}: expected {tuple(z.shape)} {z.dtype}, got {tuple(buf.shape)} {buf.dtype}")
+    if not 0 <= layer <= 255:
+        raise ValueError(f"JK layer index {layer} out of range 0..255")
+    if code == JK_MAX:
+        if idx is None or idx.dtype != torch.uint8 or _mat(idx, "jk_idx")[2] != ld or idx.shape[0] != rows or idx.shape[1] < h:
+            raise ValueError("jk_idx: expected uint8 [rows, >= h] with the JK buffer's pitch")
+    return code, ld
+
+
+def bn_fwd_jk(z: Tensor, mean, rstd, gamma, beta, zbias, use_bn: bool, use_relu: bool, p: float, seed: int, want_y: bool,
+              mode: str, jk: Tensor, jk_idx: Optional[Tensor], layer: int) -> Optional[Tensor]:
+    """bn_fwd of GCN layer `layer` that also folds its pre-dropout activation into the jumping knowledge (include/sgformer_b200.h:
+    sgf_bn_fwd_jk): the running max / layer index (mode 'max'), or column block `jk` of the concatenation (mode 'cat')."""
+    _use(z)
+    rows, h, ld = _mat(z, "z")
+    code, ld_jk = _jk_args(mode, jk, jk_idx, layer, z, "jk")
+    y = new_like(z) if want_y else None
+    check(lib().sgf_bn_fwd_jk(_p(z), ld, rows, h, dcode(z), _p(mean), _p(rstd), _p(gamma), _p(beta), _p(zbias), int(use_bn),
+                              int(use_relu), p, seed, _p(y), code, _p(jk), ld_jk, _p(jk_idx), layer, _stream()), "sgf_bn_fwd_jk")
+    return y
+
+
+def bn_bwd_jk(dy: Optional[Tensor], z: Tensor, mean, rstd, gamma, beta, zbias, use_bn: bool, use_relu: bool, training: bool,
+              p: float, seed: int, mode: str, jk_g: Tensor, jk_idx: Optional[Tensor], layer: int, want_dz_colsum: bool = False,
+              out_row_scale: Optional[Tensor] = None):
+    """bn_bwd whose upstream gradient is dropout(dy) + the JK gradient of layer `layer` (sgf_bn_bwd_*_jk) -> (dz, sums [2h] or None,
+    dz_colsum or None).  Eval mode with BatchNorm returns the sums too (the affine gradients need them)."""
+    _use(z)
+    rows, h, ld = _mat(z, "z")
+    code, ld_jk = _jk_args(mode, jk_g, jk_idx, layer, z, "jk_g")
+    _same_ld(ld, dy)
+    dz = new_like(z)
+    sums = None
+    if use_bn:
+        sums = torch.zeros(2 * h, dtype=torch.float32, device=z.device)
+        ws, nws = _red_ws(h, z.device)
+        check(lib().sgf_bn_bwd_reduce_jk(_p(dy), _p(z), ld, rows, h, dcode(z), _p(mean), _p(rstd), _p(gamma), _p(beta), _p(zbias),
+                                         int(use_bn), int(use_relu), p, seed, _p(sums), code, _p(jk_g), ld_jk, _p(jk_idx), layer,
+                                         _p(ws), nws, _stream()), "sgf_bn_bwd_reduce_jk")
+    colsum = torch.zeros(h, dtype=torch.float32, device=z.device) if want_dz_colsum else None
+    ws, nws = _red_ws(h, z.device)
+    check(lib().sgf_bn_bwd_apply_jk(_p(dy), _p(z), ld, rows, h, dcode(z), _p(mean), _p(rstd), _p(gamma), _p(beta), _p(zbias),
+                                    int(use_bn), int(use_relu), int(training), p, seed, _p(sums), _p(dz), _p(colsum),
+                                    _p(out_row_scale), code, _p(jk_g), ld_jk, _p(jk_idx), layer, _p(ws), nws, _stream()),
+          "sgf_bn_bwd_apply_jk")
+    return dz, sums, colsum
+
+
 def axpby(x: Tensor, y: Optional[Tensor], a: float, b: float, out_dtype=None, row_scale: Optional[Tensor] = None,
           out: Optional[Tensor] = None) -> Tensor:
     _use(x)

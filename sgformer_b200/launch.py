@@ -17,8 +17,9 @@ def main(argv=None):
     ap.add_argument("--variant", required=True, choices=["large", "medium", "100M"])
     ap.add_argument("--precision", choices=["bf16", "fp32"], default=None)
     ap.add_argument("--native-backbones", action="store_true",
-                    help="medium: make the GAT and GCN that the reference's parse.py builds backbones from resolve to "
-                         "sgformer_b200.medium.GAT / GCN, so that --backbone gat|gcn (and --method gat|gcn) run on the kernels; "
+                    help="medium: make the GAT, GCN and GCNJK that the reference's parse.py builds backbones from resolve to "
+                         "sgformer_b200.medium.GAT / GCN / GCNJK, so that --backbone gat|gcn|gcnjk (and --method gat|gcn|gcnjk) "
+                         "run on the kernels; "
                          "large: make parse.py's GCN and GAT (from gnns.py) resolve to sgformer_b200.large_gnns.GCN / GAT, so that "
                          "--method gcn|gat runs on the kernels (models.py / gnns.py still import torch_geometric)")
     ap.add_argument("script")
@@ -46,6 +47,8 @@ def main(argv=None):
         import parse
         for mod in (gnn_mod, parse):
             mod.GAT, mod.GCN = native.GAT, native.GCN
+            if a.variant == "medium":
+                mod.GCNJK = native.GCNJK
     runpy.run_path(script, run_name="__main__")
 
 

@@ -1,6 +1,6 @@
-"""Drop-in for the reference's medium/ours.py (`--method ours`, medium/parse.py:97-104) plus native `GCN` and `GAT` backbones
-with the semantics of medium/models.py:14-63 (PyG GCNConv stack) and :116-155 (PyG GATConv stack) for users without
-torch_geometric."""
+"""Drop-in for the reference's medium/ours.py (`--method ours`, medium/parse.py:97-104) plus native `GCN`, `GAT` and `GCNJK`
+backbones with the semantics of medium/models.py:14-63 (PyG GCNConv stack), :116-155 (PyG GATConv stack) and :157-205 (GCNConv
+stack with JumpingKnowledge) for users without torch_geometric."""
 import math
 
 import torch
@@ -14,9 +14,9 @@ from .dist import SINGLE
 from .graph import get_graph
 from .modules import SGFormerBase, TransConvBase, TransConvLayerBase, _Base, full_attention_conv
 
-# GAT / GATConv stay out of __all__: the medium drop-in star-imports this module after the reference's `models`, and a star export
-# would replace the reference's GAT in its parse.py (`--method gat`, `--backbone gat`) without being asked to
-# (`launch --native-backbones` opts in)
+# GAT / GATConv / GCNJK stay out of __all__: the medium drop-in star-imports this module after the reference's `models`, and a star
+# export would replace the reference's GAT / GCNJK in its parse.py (`--method gat|gcnjk`, `--backbone gat|gcnjk`) without being
+# asked to (`launch --native-backbones` opts in)
 __all__ = ["full_attention_conv", "TransConvLayer", "TransConv", "SGFormer", "GCN", "GCNConv"]
 
 
@@ -268,6 +268,81 @@ def _gat_flat(gnn, prefix):
     return tuple(names), tensors
 
 
+class JumpingKnowledge(nn.Module):
+    """PyG's JumpingKnowledge in 'max' / 'cat' mode: no parameters; it runs inside `GCNJK` (one schedule for the whole model)."""
+
+    def __init__(self, mode, channels=None, num_layers=None):
+        super().__init__()
+        self.mode = mode.lower()
+        if self.mode == "lstm":
+            raise NotImplementedError("sgformer_b200.GCNJK: jk_type='lstm' is not supported (use 'max' or 'cat')")
+        if self.mode not in ("max", "cat"):
+            raise ValueError(f"JumpingKnowledge: unknown mode {mode!r}")
+
+    def reset_parameters(self):
+        pass
+
+    def forward(self, xs):
+        raise NotImplementedError("sgformer_b200.JumpingKnowledge runs inside sgformer_b200.medium.GCNJK")
+
+
+class GCNJK(_Base):
+    """models.GCNJK (medium/models.py:157-205): GCNConv(in, hidden), num_layers - 2 GCNConv(hidden, hidden) and a last
+    GCNConv(hidden, hidden) (at least two convs), BatchNorm/ReLU/dropout after every conv but the last, JumpingKnowledge over the
+    layers' activations (taken before their dropout) and final_project = Linear(hidden -> out) ('max') or Linear(hidden *
+    num_layers -> out) ('cat').  No `use_bn` attribute (BatchNorm is always on), so SGFormer never mistakes it for a models.GCN;
+    data.graph['edge_weight'] is ignored, as in the reference."""
+
+    def __init__(self, in_channels, hidden_channels, out_channels, num_layers=2, dropout=0.5, save_mem=False, jk_type='max'):
+        super().__init__()
+        if save_mem:
+            raise NotImplementedError("sgformer_b200.GCNJK: save_mem=True (GCNConv(normalize=False)) is not supported")
+        jump = JumpingKnowledge(jk_type, channels=hidden_channels, num_layers=1)
+        if jump.mode == "cat" and num_layers < 2:
+            raise ValueError(f"GCNJK(jk_type='cat', num_layers={num_layers}) concatenates 2 layers of {hidden_channels} channels, "
+                             f"but its final_project takes {hidden_channels * num_layers} (the reference fails here too)")
+        self.convs = nn.ModuleList()
+        self.convs.append(GCNConv(in_channels, hidden_channels, cached=not save_mem))
+        self.bns = nn.ModuleList()
+        self.bns.append(nn.BatchNorm1d(hidden_channels))
+        for _ in range(num_layers - 2):
+            self.convs.append(GCNConv(hidden_channels, hidden_channels, cached=not save_mem))
+            self.bns.append(nn.BatchNorm1d(hidden_channels))
+        self.convs.append(GCNConv(hidden_channels, hidden_channels, cached=not save_mem))
+        self.dropout = dropout
+        self.activation = F.relu
+        self.jump = jump
+        self.final_project = nn.Linear(hidden_channels * num_layers if jump.mode == "cat" else hidden_channels, out_channels)
+
+    def reset_parameters(self):
+        for conv in self.convs:
+            conv.reset_parameters()
+        for bn in self.bns:
+            bn.reset_parameters()
+        self.jump.reset_parameters()
+        self.final_project.reset_parameters()
+
+    def _cfg_kw(self):
+        return dict(gcn_num_layers=len(self.convs), gcn_dropout=float(self.dropout), gcn_use_bn=True, gnn_kind="gcnjk",
+                    gcn_jk=self.jump.mode)
+
+    def forward(self, data):
+        x, edge_index = data.graph['node_feat'], data.graph['edge_index']
+        if not x.is_cuda:
+            raise RuntimeError("sgformer_b200.GCNJK needs CUDA tensors (no CPU fallback)")
+        names, tensors = _gcnjk_flat(self, "")
+        cfg = make_config("medium", x.shape[1], self.convs[0].out_channels, self.final_project.out_features, **self._cfg_kw())
+        graph = get_graph(edge_index, x.shape[0], 1)
+        return Fn.GraphBranchFn.apply(x, graph, cfg, E.precision(self.precision), self.training, "gcnjk", "", names, *tensors)
+
+
+def _gcnjk_flat(gnn, prefix):
+    """(names, tensors) of a GCNJK (ours, or the reference's over PyG GCNConv): the GCN stack's, then final_project."""
+    names, tensors = _gcn_flat(gnn, prefix)
+    names = tuple(names) + (f"{prefix}final_project.weight", f"{prefix}final_project.bias")
+    return names, list(tensors) + [gnn.final_project.weight, gnn.final_project.bias]
+
+
 class SGFormer(SGFormerBase):
     """medium/ours.py:179-223: attention branch + an injected GNN (`gnn=`)."""
     variant = "medium"
@@ -291,7 +366,7 @@ class SGFormer(SGFormerBase):
         self.params2.extend(list(self.fc.parameters()))
         self._io = (in_channels, hidden_channels, out_channels)
 
-    def _cfg(self, gcn_layers=2, gcn_dropout=0.5, gcn_use_bn=True, gnn_kind="gcn") -> dict:
+    def _cfg(self, gcn_layers=2, gcn_dropout=0.5, gcn_use_bn=True, gnn_kind="gcn", gcn_jk="max") -> dict:
         d, h, c = self._io
         t = self.trans_conv
         _, _, tnl, tnh = t._dims
@@ -300,7 +375,7 @@ class SGFormer(SGFormerBase):
                            trans_use_weight=t.convs[0].use_weight if tnl else True, trans_use_act=False, alpha=t.alpha,
                            use_graph=bool(self.use_graph), graph_weight=float(self.graph_weight),
                            aggregate=self.aggregate, gcn_num_layers=gcn_layers, gcn_dropout=gcn_dropout,
-                           gcn_use_bn=gcn_use_bn, gnn_kind=gnn_kind)
+                           gcn_use_bn=gcn_use_bn, gnn_kind=gnn_kind, gcn_jk=gcn_jk)
 
     def forward(self, data):
         x, edge_index = data.graph['node_feat'], data.graph['edge_index']
@@ -321,6 +396,13 @@ class SGFormer(SGFormerBase):
                 raise NotImplementedError("sgformer_b200: row sharding of the GAT branch is not supported")
             gn, gt = _gat_flat(self.gnn, "gnn.")
             cfg = self._cfg(len(self.gnn.convs), float(self.gnn.dropout), bool(self.gnn.use_bn), "gat")
+            graph = get_graph(edge_index, x.shape[0], 1)
+            return Fn.SGFormerFn.apply(x, graph, cfg, prec, self.training, self._comm, tuple(names) + tuple(gn), *tensors, *gt)
+        if isinstance(self.gnn, GCNJK) and self.gnn.final_project.out_features == self._io[1]:
+            if self._comm.active:
+                raise NotImplementedError("sgformer_b200: row sharding of the GCNJK branch is not supported")
+            gn, gt = _gcnjk_flat(self.gnn, "gnn.")
+            cfg = self._cfg(len(self.gnn.convs), float(self.gnn.dropout), True, "gcnjk", self.gnn.jump.mode)
             graph = get_graph(edge_index, x.shape[0], 1)
             return Fn.SGFormerFn.apply(x, graph, cfg, prec, self.training, self._comm, tuple(names) + tuple(gn), *tensors, *gt)
         if fused:
