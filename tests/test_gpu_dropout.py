@@ -10,13 +10,13 @@ applies the same mask:
   (e) guards against a vacuous pass (call counts, the masks' effect, eval mode)."""
 import contextlib
 import functools
-import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from dropout_mask import DropoutRecorder, MaskReplayer, current_epoch, keep_mask, keep_scale
+from row_ref import BN_CASES, bn_reference, bn_untie, check_bn_chain, ln_reference
+from row_ref import attn_reference as _attn_reference, close as _close, untie as _untie
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -153,43 +153,8 @@ def _tol(dtype):
     return 2e-5 if dtype == F32 else 5e-3
 
 
-def _close(got, ref, tol, what, colsum_rows=0, elem=0.0):
-    """max-abs error relative to the reference's max; column sums get a sqrt(rows) allowance and, where they cancel, are
-    measured against their largest summand `elem`."""
-    got, ref = got.detach().double().reshape(ref.shape), ref.detach().double()
-    err = (got - ref).abs().max().item() if ref.numel() else 0.0
-    scale = max(ref.abs().max().item(), float(elem), 1e-6)
-    allow = tol * scale * (math.sqrt(colsum_rows) if colsum_rows else 1.0)
-    assert err == err and err <= allow, f"{what}: max err {err:.3e} (ref max {scale:.3e}, allowed {allow:.3e})"
-
-
 def _rand(rows, h, dtype, gen, scale=1.0):
     return (scale * torch.randn(rows, h, generator=gen)).to(DEV).to(dtype)
-
-
-def ln_reference(x, r, gy, a, b, c, gamma, beta, use_ln, use_relu, M, dy, gscale):
-    """fp64 autograd of y = dropout(relu?(LN?(a*x + b*r + c*gy))) -> y and the gradients of sum(gscale * dy * y)."""
-    h = x.shape[1]
-    xd = x.double().requires_grad_(True)
-    rd = r.double().requires_grad_(True) if r is not None else None
-    gd, bd = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
-    u = a * xd + (b * rd if rd is not None else 0.0) + (c * gy.double() if gy is not None else 0.0)
-    u.retain_grad()
-    t = F.layer_norm(u, (h,), gd, bd, 1e-5) if use_ln else u
-    if use_relu:
-        t = t.clamp_min(0)
-    y = t * M
-    (y * dy.double() * gscale).sum().backward()
-    return dict(y=y.detach(), du=u.grad, dx=xd.grad, dr=rd.grad if rd is not None else None, dgamma=gd.grad, dbeta=bd.grad)
-
-
-def _untie(dy, x, r, a, b, gamma, beta, use_ln):
-    """Zero the incoming gradient where the fp64 ReLU pre-activation LN?(a*x + b*r) is within 1e-3 of its largest magnitude of
-    zero: there fp32 and fp64 may open the gate differently, and with no gradient through it the choice does not matter.  Every
-    other output is then compared at the ordinary tolerance."""
-    u = a * x.double() + (b * r.double() if r is not None else 0.0)
-    pre = F.layer_norm(u, (u.shape[1],), gamma.double(), beta.double(), 1e-5) if use_ln else u
-    return dy.masked_fill(pre.abs() <= 1e-3 * pre.abs().max(), 0)
 
 
 def _ln_inputs(rows, h, dtype, seed):
@@ -228,15 +193,6 @@ def test_ln_fwd_ln_bwd_pair(K, dtype, h):
         if use_ln:
             _close(dg, R["dgamma"], 1e-5, f"dgamma {tag}", rows)
             _close(db, R["dbeta"], 1e-5, f"dbeta {tag}", rows)
-
-
-def _attn_reference(R, o, xa, a, den):
-    ga = a * R["du"]
-    gnum = ga / den.double()[:, None]
-    gden = -(ga * o.double()).sum(1) / den.double()
-    pgt = xa.double() * gden[:, None]
-    return dict(gnum=gnum, gden=gden, cs=gnum.sum(0), pg=pgt.sum(0), sg=gden.sum().reshape(1),
-                elem=dict(cs=gnum.abs().max().item(), pg=pgt.abs().max().item(), sg=gden.abs().max().item()))
 
 
 @pytest.mark.parametrize("dtype,h", PAIR_SHAPES, ids=[f"{'fp32' if d == F32 else 'bf16'}-h{h}" for d, h in PAIR_SHAPES])
@@ -313,15 +269,6 @@ def test_ln_fwd_graph_ln_bwd_attn_graph_pair(K, dtype, h):
                           f"ln={use_ln} r={with_r} xa_is_r={alias} rows={rows} p={p}")
 
 
-BN_CASES = [   # (use_bn, training, relu, res, mix, dy2, dres_acc, out_row_scale)
-    (True, True, True, True, False, True, True, False),       # GraphConv middle layer: residual, pre-scaled gradient
-    (True, True, True, False, True, False, False, False),     # last layer: branch mix with gw
-    (True, False, False, True, False, True, False, True),     # BatchNorm in eval mode
-    (False, True, True, False, False, False, False, True),    # no BatchNorm (GCN backbone)
-    (True, True, False, False, False, False, False, True),    # training BatchNorm, no ReLU, GCN-style row scale
-]
-
-
 def _bn_chain(K, dtype, rows, h, case, p, seed):
     use_bn, training, relu, with_res, with_mix, with_dy2, dres_acc, with_ors = case
     g = torch.Generator().manual_seed(seed)
@@ -332,15 +279,7 @@ def _bn_chain(K, dtype, rows, h, case, p, seed):
     rs, rs2, ors = (0.2 + torch.rand(rows, generator=g)).to(DEV), (0.2 + torch.rand(rows, generator=g)).to(DEV), \
         (0.2 + torch.rand(rows, generator=g)).to(DEV)
     gw, gscale = 0.7, 0.9
-    if relu:      # as _untie: no gradient through a ReLU gate that fp32 and fp64 may decide differently
-        zz = z.double()
-        if use_bn:
-            mu, var = (zz.mean(0), zz.var(0, unbiased=False)) if training else (rm.double(), rv.double())
-            pre = (zz - mu) / torch.sqrt(var + 1e-5) * gamma.double() + beta.double()
-        else:
-            pre = zz
-        amb = pre.abs() <= 1e-3 * pre.abs().max()
-        dy, dy2 = dy.masked_fill(amb, 0), dy2.masked_fill(amb, 0)
+    dy, dy2 = bn_untie(case, z, gamma, beta, rm, rv, dy, dy2)
     mean = rstd = None
     if use_bn:
         if training:
@@ -358,28 +297,7 @@ def _bn_chain(K, dtype, rows, h, case, p, seed):
     if use_bn and not training:
         sums = K.bn_bwd_sums(dy, dy2 if with_dy2 else None, rs2 if with_dy2 else None, z, mean, rstd, gamma, beta, None, True, relu,
                              p, seed, gscale)
-    # fp64 reference
-    zd = z.double().requires_grad_(True)
-    gd, bd = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
-    if use_bn:
-        if training:
-            mu, var = zd.mean(0), zd.var(0, unbiased=False)
-        else:
-            mu, var = rm.double(), rv.double()
-        xh = (zd - mu) / torch.sqrt(var + 1e-5)
-        t = xh * gd + bd
-    else:
-        t = zd
-    if relu:
-        t = t.clamp_min(0)
-    t = t * dmask(seed, rows, h, p)
-    if with_res:
-        t = t + res.double()
-    G = gscale * (dy.double() + (rs2.double()[:, None] * dy2.double() if with_dy2 else 0.0))
-    (t * G).sum().backward()
-    ref = dict(y=(gw * t + (1 - gw) * mix.double()) if with_mix else t, ys=t * rs.double()[:, None],
-               dres=G + (dres0.double() if dres_acc else 0.0), dz=zd.grad * (ors.double()[:, None] if with_ors else 1.0),
-               colsum=zd.grad.sum(0), dbeta=bd.grad, dgamma=gd.grad)
+    ref = bn_reference(case, z, res, mix, dy, dy2, dres0, gamma, beta, rm, rv, rs, rs2, ors, gw, gscale, dmask(seed, rows, h, p))
     return dict(y=y, ys=ys, dres=dres, dz=dz, colsum=colsum, sums=sums), ref
 
 
@@ -390,20 +308,7 @@ def test_bn_fwd_bn_bwd_chain(K, dtype, h):
         for rows in (5, 777):
             p, seed = (0.2, 0.5, 0.6)[(k + rows) % 3], 500 + 7 * k + rows + h
             got, ref = _bn_chain(K, dtype, rows, h, case, p, seed)
-            tag = f"case={case} rows={rows} p={p}"
-            use_bn, training, relu = case[:3]
-            _close(got["y"], ref["y"], tol, f"y {tag}")
-            _close(got["ys"], ref["ys"], tol, f"ys {tag}")
-            _close(got["dres"], ref["dres"], tol, f"dres {tag}")
-            # a training BatchNorm backward subtracts column means: its error is relative to the whole gradient's scale
-            dz_tol = tol if not (use_bn and training) else 4 * tol
-            _close(got["dz"], ref["dz"], dz_tol, f"dz {tag}")
-            cs_tol = 1e-5
-            if not (use_bn and training):     # training: the column sums of dz are ~0 (the BatchNorm backward centres dz)
-                _close(got["colsum"], ref["colsum"], cs_tol, f"dz colsum {tag}", rows)
-            if use_bn:
-                _close(got["sums"][:h], ref["dbeta"], cs_tol, f"dbeta {tag}", rows)
-                _close(got["sums"][h:], ref["dgamma"], cs_tol, f"dgamma {tag}", rows)
+            check_bn_chain(got, ref, case, tol, f"case={case} rows={rows} p={p}", rows, h)
 
 
 # ------------------------------------------------------------------------------------------------
