@@ -512,6 +512,45 @@ int sgf_attn_gram_prepare_bwd(const sgf_attn_gram_args* args /* host */, void* s
  *   dWv = beta dS^T kx + cs s^T / N,   a4 += Wv^T cs / N     (everything else unchanged)  in the backward. */
 int sgf_attn_gram_prepare_fwd_vsum(const sgf_attn_gram_args* args /* host */, void* stream);
 int sgf_attn_gram_prepare_bwd_vsum(const sgf_attn_gram_args* args /* host */, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Fused softmax attention of SGFormerSOFT (medium/ablation/oursSOFT.py:14-34; derivation and the |s| <= 1 bound at the top of
+ * csrc/attn_softmax.cu): s[n,l,h] = q~[n,h].k~[l,h] with one Frobenius norm over all nodes and heads, P = softmax over the HEADS
+ * of s[n,l,:] (the reference's F.softmax(dim=-1) of its [N, L, H] scores), o[n,h] = sum_l P[n,l,h] v[l,h].
+ * q, k: [n, heads*m], v: [n, heads*d] (or [n, d] with shared_v: one v for every head), activations of `dtype` (0 fp32, 1 bf16)
+ * whose pointers and pitches are 16-byte aligned; m, d multiples of 16 bytes of the dtype; the heads' blocks of one q row, each
+ * padded to 16 elements, and those of one v row take at most SGF_ATTN_SOFTMAX_MAX_ROW_BYTES (else SGF_ERR_UNSUPPORTED).
+ * sq_q / sq_k: fp32 [heads*m] column sums of squares of q / k (||q||^2 = their sum).
+ * No N x N buffer is ever written; every output element is written by one thread in a fixed order (deterministic, no atomics).
+ *   fwd:      o [n, heads*d]
+ *   bwd_q:    with g the gradient of o (times gscale), head h's block at column h*g_hstride (g_hstride = d, or 0: one [n, d]
+ *             block for every head, the head mean's backward):  aq [n, heads*m] (fp32, pitch ld_a) = c dS k per head
+ *             (c = 1/(||q|| ||k||), dS_h = P_h (g_h v_h^T - sum_h' P_h' g_h' v_h'^T))
+ *   bwd_kv:   ak (fp32, pitch ld_a) = c dS^T q,  dv (+)= gscale P^T g  (with shared_v: the heads summed in head order)
+ *   bwd_norm: dq = gscale (aq - <q,aq>/||q||^2 q), dk likewise (dtype, pitches lddq / lddk): the Frobenius-norm backward
+ *   probs:    att [n, n] (fp32, pitch ld_att) = the head mean of P (inference, small n)
+ * ws: fp32 scratch of sgf_attn_softmax_ws_floats for the bwd kernels' per-CTA partial sums. */
+#define SGF_ATTN_SOFTMAX_MAX_ROW_BYTES 1024
+typedef struct {
+    int32_t n, heads, m, d, dtype, shared_v;
+    const void* q; int64_t ldq;
+    const void* k; int64_t ldk;
+    const void* v; int64_t ldv;
+    const float *sq_q, *sq_k;
+    void* o; int64_t ldo;           /* written by fwd */
+    const void* g; int64_t ldg, g_hstride; float gscale;
+    float *aq, *ak; int64_t ld_a;
+    void* dv; int64_t lddv; int32_t dv_accumulate;
+    void* dq; int64_t lddq;
+    void* dk; int64_t lddk;
+    float* ws; int64_t ws_floats;
+} sgf_attn_softmax_args;
+int sgf_attn_softmax_ws_floats(int n, int heads, int m, int d, int64_t* n_floats /* host out */);
+int sgf_attn_softmax_fwd(const sgf_attn_softmax_args* args /* host */, void* stream);
+int sgf_attn_softmax_bwd_q(const sgf_attn_softmax_args* args /* host */, void* stream);
+int sgf_attn_softmax_bwd_kv(const sgf_attn_softmax_args* args /* host */, void* stream);
+int sgf_attn_softmax_bwd_norm(const sgf_attn_softmax_args* args /* host */, void* stream);
+int sgf_attn_softmax_probs(const sgf_attn_softmax_args* args /* host */, float* att, int64_t ld_att, void* stream);
+
 /* Dropout epoch.  Every kernel that takes (p, seed) draws its mask from hash(seed + epoch * odd, row, chunk); `epoch` is read from
  * the device word registered here (NULL, the default: epoch 0).  The host seed of a call is frozen into a captured CUDA graph;
  * a step that is captured and replayed registers an epoch word and puts sgf_advance_dropout_epoch at the top of the captured

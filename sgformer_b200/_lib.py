@@ -55,6 +55,21 @@ class AttnGramArgs(C.Structure):
     ]
 
 
+class AttnSoftmaxArgs(C.Structure):
+    """sgf_attn_softmax_args (include/sgformer_b200.h)."""
+    _fields_ = [
+        ("n", _i32), ("heads", _i32), ("m", _i32), ("d", _i32), ("dtype", _i32), ("shared_v", _i32),
+        ("q", _vp), ("ldq", _i64), ("k", _vp), ("ldk", _i64), ("v", _vp), ("ldv", _i64),
+        ("sq_q", _vp), ("sq_k", _vp),
+        ("o", _vp), ("ldo", _i64),
+        ("g", _vp), ("ldg", _i64), ("g_hstride", _i64), ("gscale", _f32),
+        ("aq", _vp), ("ak", _vp), ("ld_a", _i64),
+        ("dv", _vp), ("lddv", _i64), ("dv_accumulate", _i32),
+        ("dq", _vp), ("lddq", _i64), ("dk", _vp), ("lddk", _i64),
+        ("ws", _vp), ("ws_floats", _i64),
+    ]
+
+
 SGF_ADAM_MAX_TENSORS = 32
 
 
@@ -132,6 +147,12 @@ _SIGS = {
     "sgf_attn_gram_prepare_bwd": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
     "sgf_attn_gram_prepare_fwd_vsum": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
     "sgf_attn_gram_prepare_bwd_vsum": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
+    "sgf_attn_softmax_ws_floats": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_i64)]),
+    "sgf_attn_softmax_fwd": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),
+    "sgf_attn_softmax_bwd_q": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),
+    "sgf_attn_softmax_bwd_kv": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),
+    "sgf_attn_softmax_bwd_norm": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),
+    "sgf_attn_softmax_probs": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp, _i64, _vp]),
     "sgf_adam_step": (C.c_int, [C.POINTER(AdamArgs), _vp]),
     "sgf_bn_finalize": (C.c_int, [_vp, _vp, _i64, C.c_int, _f32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sgf_bn_fwd": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int,

@@ -5,6 +5,7 @@ _DEFAULTS = dict(
     trans_use_weight=True, trans_use_act=True, alpha=0.5, gnn_num_layers=1, gnn_dropout=0.5, gnn_use_weight=True,
     gnn_use_init=False, gnn_use_bn=True, gnn_use_residual=True, gnn_use_act=True, use_graph=True, graph_weight=0.8,
     aggregate="add", gcn_num_layers=2, gcn_dropout=0.5, gcn_use_bn=True, gcn_normalize=True, gnn_kind="gcn", gcn_jk="max",
+    trans_attention="linear",
 )
 
 
@@ -21,6 +22,8 @@ def make_config(variant: str, in_channels: int, hidden: int, out_channels: int, 
         raise ValueError(f"unknown GNN kind {cfg['gnn_kind']!r}")
     if cfg["gcn_jk"] not in ("max", "cat"):
         raise ValueError(f"unknown JumpingKnowledge mode {cfg['gcn_jk']!r}")
+    if cfg["trans_attention"] not in ("linear", "softmax"):
+        raise ValueError(f"unknown TransConv attention {cfg['trans_attention']!r} (use 'linear' or 'softmax')")
     if cfg["aggregate"] not in ("add", "cat"):
         raise ValueError(f"Invalid aggregate type:{cfg['aggregate']}")
     return cfg

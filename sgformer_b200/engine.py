@@ -218,6 +218,41 @@ def attention_backward(tape: Tape, g: Tensor, gscale: float, prec: Precision, dq
 
 
 # =================================================================================================
+# softmax attention core (SGFormerSOFT's softmax_attention, medium/ablation/oursSOFT.py:14-34)
+# =================================================================================================
+def attention_softmax_forward(q: Tensor, k: Tensor, v: Tensor, heads: int, prec: Precision, tape: Optional[Tape], stats=None,
+                              shared_v: bool = False) -> Tensor:
+    """q, k: [N, H*M], v: [N, H*D] (or [N, D] shared by every head) -> o [N, H*D] of SGFormerSOFT's softmax_attention: one
+    Frobenius norm over all heads, s[n,l,h] = q~[n,h].k~[l,h], softmax over the HEADS of s[n,l,:] (oursSOFT.py:21-22 applies
+    F.softmax(dim=-1) to [N, L, H] scores), o[n,h] = sum_l P[n,l,h] v[l,h].  stats: (sums of squares of q's columns, of k's
+    columns), e.g. from the projection's epilogue.  The fused kernel never stores an N x N tile (csrc/attn_softmax.cu)."""
+    m = q.shape[1] // heads
+    d = v.shape[1] if shared_v else v.shape[1] // heads
+    if not K.attn_softmax_fits(heads, m, d, q.dtype, shared_v):
+        raise ValueError(f"sgformer_b200: softmax attention with {heads} heads of width {m} in precision '{prec.name}' is not supported: "
+                         f"the heads' columns of one row, each padded to 16, must take at most {K.ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+    if stats is None:
+        _, sq_q = K.colstats(q, want_sum=False)
+        _, sq_k = K.colstats(k, want_sum=False)
+    else:
+        sq_q, sq_k = stats
+    o = K.attn_softmax_fwd(q, k, v, heads, sq_q, sq_k, shared_v)
+    if tape is not None:
+        tape.update(q=q, k=k, v=v, sq_q=sq_q, sq_k=sq_k, heads=heads, shared_v=shared_v)
+    return o
+
+
+def attention_softmax_backward(tape: Tape, g: Tensor, gscale: float, dq: Tensor, dk: Tensor, dv: Tensor,
+                               dv_accumulate: bool = False):
+    """g = dL/do [N, H*D] (times gscale), or [N, D] when every head receives the same gradient (the head mean's backward).
+    Writes dq, dk [N, H*M] and dv (+= if dv_accumulate; [N, D] with a shared v, the heads summed in head order).  The two
+    sweeps recompute P; the norm backward dq = (dq~ - q~<q~, dq~>_F)/||q||_F reduces its scalar from per-CTA partials in a
+    fixed order (deterministic, no atomics)."""
+    K.attn_softmax_bwd(tape["q"], tape["k"], tape["v"], tape["heads"], tape["sq_q"], tape["sq_k"], tape["shared_v"], g, gscale,
+                       dq, dk, dv, dv_accumulate)
+
+
+# =================================================================================================
 # linear attention in Gram form (single head): projections + full_attention_conv without materialising q, k, v
 # =================================================================================================
 # With q = x Wq^T + bq, k = x Wk^T + bk, v = x Wv^T + bv every node-contracted quantity of full_attention_conv
@@ -383,10 +418,20 @@ def trans_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precisi
         tape.update(xin=xin, t0=t0, st0=st, layers=[], p=p, seed=seed, n=xin.rows)
     ca, cb, use_res = _res_coef(cfg)
     use_weight = bool(cfg["trans_use_weight"])
+    softmax = cfg["trans_attention"] == "softmax"
+    if softmax and comm.active:
+        raise NotImplementedError("sgformer_b200: row sharding of the softmax attention is not supported")
     for i in range(cfg["trans_num_layers"]):
         lp = f"{pfx}convs.{i}."
         at = Tape() if tape is not None else None
-        if H == 1:
+        if softmax:
+            qkv, _, csq = _project_qkv(P, lp, K.as_operand(x, prec.planes, memo=True), use_weight, prec, stats=True)
+            q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
+            v = qkv[:, 2 * H * h:] if use_weight else x
+            o = attention_softmax_forward(q, k, v, H, prec, at, stats=(csq[:H * h], csq[H * h:2 * H * h]), shared_v=not use_weight)
+            a = K.head_mean(o, H, h) if H > 1 else o
+            saved = dict(nout=qkv.shape[1], softmax=True)
+        elif H == 1:
             a = attention_gram_forward(P, lp, x, use_weight, prec, at, comm)
             saved = dict(gram=True)
         else:
@@ -429,6 +474,13 @@ def trans_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Prec
         q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
         v = qkv[:, 2 * H * h:] if use_weight else x
         at = Tape()
+        if cfg["trans_attention"] == "softmax":       # head mean of the softmax weights (oursSOFT.py:28-29)
+            o = attention_softmax_forward(q, k, v, H, prec, at, shared_v=not use_weight)
+            out.append(K.attn_softmax_probs(q, k, H, at["sq_q"], at["sq_k"]))
+            a = K.head_mean(o, H, h) if H > 1 else o
+            x, _ = K.ln_fwd(a, x if use_res else None, ca, cb, P.get(f"{pfx}bns.{i + 1}.weight"), P.get(f"{pfx}bns.{i + 1}.bias"),
+                            use_ln, with_act and bool(cfg["trans_use_act"]), 0.0, 0, False)
+            continue
         o = attention_forward(q, k, v, H, prec, at, shared_v=not use_weight)
         inv_norm = at["den"].mean(dim=0).reciprocal_().contiguous()       # [N]: 1 / mean_h(den_h)  (an [N]-vector; not a hot path)
         att = K.alloc_act(n, n, torch.float32, dev)
@@ -469,7 +521,12 @@ def trans_backward(P, cfg: dict, tape: Tape, dout: Tensor, gscale: float, prec: 
                               use_ln, bool(cfg["trans_use_act"]), p, seed + _SEED_LAYER + i, gs, use_res, dg, db)
             dqkv = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
             dprev = dr if dr is not None else K.new_like(x_in)
-            if use_weight:
+            if L.get("softmax"):
+                # head mean: every head receives da / H (one shared gradient block); a shared v = x_in sums into dprev
+                attention_softmax_backward(at, da, 1.0 / H, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h],
+                                           dqkv[:, 2 * H * h:] if use_weight else dprev,
+                                           dv_accumulate=not use_weight and dr is not None)
+            elif use_weight:
                 # head mean: every head receives da / H; da has pitch h, per-head slices of g are the same columns for all heads
                 attention_backward(at, _tile_heads(da, H), 1.0 / H, prec, dqkv[:, :H * h], dqkv[:, H * h:2 * H * h],
                                    dqkv[:, 2 * H * h:], comm=comm)

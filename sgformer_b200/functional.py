@@ -265,6 +265,42 @@ class HeadFn(Function):
         return (d1, d2, None, None, None, *_grad_list(names, params, grads))
 
 
+class SoftmaxAttentionFn(_TapeFunction):
+    """softmax_attention(qs, ks, vs) -> [N, H, D]  (medium/ablation/oursSOFT.py:14-34).  A one-head vs [N, 1, D] is shared by all
+    H heads, as the reference's einsum broadcasts it; its gradient is the sum over the heads."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, prec, want_attn):
+        n, heads, m = q.shape
+        vh, d = v.shape[1], v.shape[2]
+        if k.shape != q.shape or v.shape[0] != n or vh not in (1, heads):
+            raise ValueError(f"softmax_attention: qs {tuple(q.shape)}, ks {tuple(k.shape)}, vs {tuple(v.shape)}: ks must match qs "
+                             f"and vs must have {n} rows and 1 or {heads} heads")
+        qa, ka, va = (_to_act(t.reshape(n, -1), prec) for t in (q, k, v))
+        tape = E.Tape()
+        o = E.attention_softmax_forward(qa, ka, va, heads, prec, tape, shared_v=vh != heads)
+        att = K.attn_softmax_probs(qa, ka, heads, tape["sq_q"], tape["sq_k"]) if want_attn else None
+        ctx.state = (tape, q.dtype, k.dtype, v.dtype, heads, vh, m, d, prec) if _want_tape(ctx) else None
+        out = _from_act(o, q.dtype).reshape(n, heads, d)
+        if att is not None:
+            ctx.mark_non_differentiable(att)
+            return out, att
+        return out
+
+    @staticmethod
+    def backward(ctx, g, *_):
+        tape, dtq, dtk, dtv, heads, vh, m, d, prec = ctx.state
+        n = g.shape[0]
+        ga = _to_act(g.reshape(n, heads * d), prec)
+        dq = K.alloc_act(n, heads * m, prec.act_dtype, g.device)
+        dk = K.alloc_act(n, heads * m, prec.act_dtype, g.device)
+        dv = K.alloc_act(n, vh * d, prec.act_dtype, g.device)
+        E.attention_softmax_backward(tape, ga, 1.0, dq, dk, dv)
+        ctx.state = None
+        return (_from_act(dq, dtq).reshape(n, heads, m), _from_act(dk, dtk).reshape(n, heads, m),
+                _from_act(dv, dtv).reshape(n, vh, d), None, None)
+
+
 class AttentionFn(_TapeFunction):
     """full_attention_conv(qs, ks, vs) -> [N, H, D]  (medium/ours.py:14-34, 100M/ours.py:12-43).  A one-head vs [N, 1, D]
     is shared by all H heads, as the reference's einsum broadcasts it; its gradient is the sum over the heads."""

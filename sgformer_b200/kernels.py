@@ -14,7 +14,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from ._lib import BF16, EPI_AFFINE, EPI_ATTN_APPLY, EPI_ATTN_GRAM, F32, AttnGramArgs, GemmNtArgs, GemmTnArgs, check
+from ._lib import BF16, EPI_AFFINE, EPI_ATTN_APPLY, EPI_ATTN_GRAM, F32, AttnGramArgs, AttnSoftmaxArgs, GemmNtArgs, GemmTnArgs, check
 
 Tensor = torch.Tensor
 _tls = threading.local()
@@ -1013,6 +1013,79 @@ def _heads_fit(x: Tensor, heads: int, d: int, name: str):
     if heads < 1 or d < 1 or cols < heads * d:
         raise ValueError(f"{name}: {cols} columns, but {heads} heads of width {d} need {heads * d}")
     return rows, cols, ld
+
+
+# ------------------------------------------------------------------------------------------------
+# fused softmax attention (csrc/attn_softmax.cu)
+# ------------------------------------------------------------------------------------------------
+ATTN_SOFTMAX_MAX_ROW_BYTES = 1024     # SGF_ATTN_SOFTMAX_MAX_ROW_BYTES
+
+
+def attn_softmax_fits(heads: int, m: int, d: int, dtype, shared_v: bool) -> bool:
+    """Whether the heads' 16-element-padded blocks of a q row and of a v row fit the kernels' shared-memory tiles."""
+    es = 2 if dtype == torch.bfloat16 else 4
+    return heads * ceil_to(m, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES and \
+        (1 if shared_v else heads) * ceil_to(d, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES
+
+
+def _softmax_args(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Tensor, sq_k: Tensor, shared_v: bool) -> AttnSoftmaxArgs:
+    _use(q)
+    n, hm = q.shape
+    m = hm // heads
+    d = v.shape[1] if shared_v else v.shape[1] // heads
+    for t, nm in ((q, "q"), (k, "k"), (v, "v")):
+        if t.dtype != q.dtype or t.shape[0] != n or t.stride(1) != 1:
+            raise ValueError(f"attn_softmax: {nm} must be a row-major [{n}, *] {q.dtype} matrix")
+    a = AttnSoftmaxArgs()
+    a.n, a.heads, a.m, a.d, a.dtype, a.shared_v = n, heads, m, d, dcode(q), int(shared_v)
+    a.q, a.ldq, a.k, a.ldk, a.v, a.ldv = _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0)
+    a.sq_q, a.sq_k = _p(_f32vec(sq_q, hm, "sq_q")), _p(_f32vec(sq_k, hm, "sq_k"))
+    return a
+
+
+def attn_softmax_fwd(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Tensor, sq_k: Tensor, shared_v: bool = False) -> Tensor:
+    """SGFormerSOFT's softmax attention: P = softmax over the heads of s[n,l,:] = q~_n.k~_l per head, one Frobenius norm over all
+    heads (q~ = q/||q||_F, ||q||^2 = sum(sq_q)); o_h = sum_l P[:,l,h] v_l,h.  q, k [N, H*M], v [N, H*D] (or [N, D] shared by
+    every head) -> o [N, H*D] in q's dtype."""
+    n = q.shape[0]
+    d = v.shape[1] if shared_v else v.shape[1] // heads
+    a = _softmax_args(q, k, v, heads, sq_q, sq_k, shared_v)
+    o = alloc_act(n, heads * d, q.dtype, q.device)
+    a.o, a.ldo = _p(o), o.stride(0)
+    check(lib().sgf_attn_softmax_fwd(C.byref(a), _stream()), "sgf_attn_softmax_fwd")
+    return o
+
+
+def attn_softmax_bwd(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Tensor, sq_k: Tensor, shared_v: bool, g: Tensor,
+                     gscale: float, dq: Tensor, dk: Tensor, dv: Tensor, dv_accumulate: bool = False):
+    """Backward of attn_softmax_fwd for the gradient gscale*g of o (g [N, H*D], or [N, D] shared by every head): writes dq, dk
+    [N, H*M] and dv (+= with dv_accumulate; a shared v gets the heads' sum)."""
+    n, hm = q.shape
+    m = hm // heads
+    d = v.shape[1] if shared_v else v.shape[1] // heads
+    shared_g = g.shape[1] == d and heads > 1
+    a = _softmax_args(q, k, v, heads, sq_q, sq_k, shared_v)
+    a.g, a.ldg, a.g_hstride, a.gscale = _p(g), g.stride(0), 0 if shared_g else d, float(gscale)
+    acc = torch.empty((2, n, hm), dtype=torch.float32, device=q.device)
+    nws = C.c_int64()
+    check(lib().sgf_attn_softmax_ws_floats(n, heads, m, d, C.byref(nws)), "sgf_attn_softmax_ws_floats")
+    ws = torch.empty(nws.value, dtype=torch.float32, device=q.device)
+    a.aq, a.ak, a.ld_a = _p(acc[0]), _p(acc[1]), hm
+    a.dv, a.lddv, a.dv_accumulate = _p(dv), dv.stride(0), int(dv_accumulate)
+    a.dq, a.lddq, a.dk, a.lddk = _p(dq), dq.stride(0), _p(dk), dk.stride(0)
+    a.ws, a.ws_floats = _p(ws), nws.value
+    check(lib().sgf_attn_softmax_bwd_q(C.byref(a), _stream()), "sgf_attn_softmax_bwd_q")
+    check(lib().sgf_attn_softmax_bwd_kv(C.byref(a), _stream()), "sgf_attn_softmax_bwd_kv")
+    check(lib().sgf_attn_softmax_bwd_norm(C.byref(a), _stream()), "sgf_attn_softmax_bwd_norm")
+
+
+def attn_softmax_probs(q: Tensor, k: Tensor, heads: int, sq_q: Tensor, sq_k: Tensor) -> Tensor:
+    """[N, N] head mean of the softmax weights of attn_softmax_fwd.  O(N^2): inference on small graphs."""
+    n = q.shape[0]
+    a = _softmax_args(q, k, k, heads, sq_q, sq_k, False)
+    att = torch.empty((n, n), dtype=torch.float32, device=q.device)
+    check(lib().sgf_attn_softmax_probs(C.byref(a), _p(att), att.stride(0), _stream()), "sgf_attn_softmax_probs")
+    return att
 
 
 def head_mean(x: Tensor, heads: int, d: int) -> Tensor:

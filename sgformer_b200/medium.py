@@ -30,11 +30,12 @@ class TransConvLayer(TransConvLayerBase):
 class TransConv(TransConvBase):
     """medium/ours.py:103-177 (takes the dataset object; residual = alpha*x + (1-alpha)*prev, :152)"""
     variant = "medium"
+    _layer_cls = TransConvLayer
 
     def __init__(self, in_channels, hidden_channels, num_layers=2, num_heads=1, alpha=0.5, dropout=0.5, use_bn=True,
                  use_residual=True, use_weight=True, use_act=False):
         super().__init__()
-        self._build(in_channels, hidden_channels, num_layers, num_heads, use_weight, TransConvLayer)
+        self._build(in_channels, hidden_channels, num_layers, num_heads, use_weight, self._layer_cls)
         self.dropout = dropout
         self.activation = F.relu
         self.use_bn = use_bn
@@ -347,14 +348,15 @@ class SGFormer(SGFormerBase):
     """medium/ours.py:179-223: attention branch + an injected GNN (`gnn=`)."""
     variant = "medium"
     _self_loop_mode = 1
+    _trans_conv_cls = TransConv
 
     def __init__(self, in_channels, hidden_channels, out_channels, num_layers=2, num_heads=1, alpha=0.5, dropout=0.5,
                  use_bn=True, use_residual=True, use_weight=True, use_graph=True, use_act=False, graph_weight=0.8,
                  gnn=None, aggregate='add'):
         super().__init__()
         # medium/ours.py:183 does not forward use_act to TransConv
-        self.trans_conv = TransConv(in_channels, hidden_channels, num_layers, num_heads, alpha, dropout, use_bn,
-                                    use_residual, use_weight)
+        self.trans_conv = self._trans_conv_cls(in_channels, hidden_channels, num_layers, num_heads, alpha, dropout, use_bn,
+                                               use_residual, use_weight)
         self.gnn = gnn
         self.use_graph = use_graph
         self.graph_weight = graph_weight
@@ -375,7 +377,7 @@ class SGFormer(SGFormerBase):
                            trans_use_weight=t.convs[0].use_weight if tnl else True, trans_use_act=False, alpha=t.alpha,
                            use_graph=bool(self.use_graph), graph_weight=float(self.graph_weight),
                            aggregate=self.aggregate, gcn_num_layers=gcn_layers, gcn_dropout=gcn_dropout,
-                           gcn_use_bn=gcn_use_bn, gnn_kind=gnn_kind, gcn_jk=gcn_jk)
+                           gcn_use_bn=gcn_use_bn, gnn_kind=gnn_kind, gcn_jk=gcn_jk, trans_attention=t.attention)
 
     def forward(self, data):
         x, edge_index = data.graph['node_feat'], data.graph['edge_index']

@@ -120,6 +120,7 @@ class TransConvLayerBase(_Base):
 
 class TransConvBase(_Base):
     variant = "large"
+    attention = "linear"        # engine config `trans_attention`: "softmax" for SGFormerSOFT's TransConv
 
     def _build(self, in_channels, hidden_channels, num_layers, num_heads, use_weight, layer_cls):
         self.convs = nn.ModuleList()
@@ -145,7 +146,7 @@ class TransConvBase(_Base):
         return make_config(self.variant, d, h, h, trans_num_layers=nl, num_heads=nh, trans_dropout=self.dropout,
                            trans_use_bn=self.use_bn, trans_use_residual=self._use_residual(),
                            trans_use_weight=self.convs[0].use_weight if nl else True, trans_use_act=self.use_act,
-                           alpha=getattr(self, "alpha", 0.5))
+                           alpha=getattr(self, "alpha", 0.5), trans_attention=self.attention)
 
     def _use_residual(self):
         return getattr(self, "use_residual", getattr(self, "residual", True))
