@@ -528,7 +528,11 @@ int sgf_attn_gram_prepare_bwd_vsum(const sgf_attn_gram_args* args /* host */, vo
  *   bwd_kv:   ak (fp32, pitch ld_a) = c dS^T q,  dv (+)= gscale P^T g  (with shared_v: the heads summed in head order)
  *   bwd_norm: dq = gscale (aq - <q,aq>/||q||^2 q), dk likewise (dtype, pitches lddq / lddk): the Frobenius-norm backward
  *   probs:    att [n, n] (fp32, pitch ld_att) = the head mean of P (inference, small n)
- * ws: fp32 scratch of sgf_attn_softmax_ws_floats for the bwd kernels' per-CTA partial sums. */
+ * ws: fp32 scratch of sgf_attn_softmax_ws_floats for the bwd kernels' per-CTA partial sums.
+ * Scaled mode (scaled = 1; SGFormerGAT, medium/ablation/oursGAT.py:31-44): s[n,l,h] = scale q[n,h].k[l,h] with a host constant
+ * scale > 0 (1/sqrt(dk)), the softmax over the heads taken against each pair's maximum over the heads; sq_q, sq_k, ws, aq, ak
+ * are unused and v is per head (shared_v = 0).  fwd as above; bwd_q writes dq = gscale scale dS k and bwd_kv writes
+ * dk = gscale scale dS^T q (dtype, pitches lddq / lddk) and dv as above.  bwd_norm and probs refuse this mode. */
 #define SGF_ATTN_SOFTMAX_MAX_ROW_BYTES 1024
 typedef struct {
     int32_t n, heads, m, d, dtype, shared_v;
@@ -543,6 +547,7 @@ typedef struct {
     void* dq; int64_t lddq;
     void* dk; int64_t lddk;
     float* ws; int64_t ws_floats;
+    int32_t scaled; float scale;    /* 1: scaled mode (below); 0: the Frobenius-normalised scores above */
 } sgf_attn_softmax_args;
 int sgf_attn_softmax_ws_floats(int n, int heads, int m, int d, int64_t* n_floats /* host out */);
 int sgf_attn_softmax_fwd(const sgf_attn_softmax_args* args /* host */, void* stream);

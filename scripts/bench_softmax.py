@@ -4,7 +4,14 @@ the native linear attention (the medium SGFormer) of the same shape.  Also times
 its FLOP/s from the reference's 4 N^2 H M flops (the kernel computes every head's scores for each head it writes, H times
 the score work) against the dense BF16 data-sheet peak of the H100 SXM (989 TFLOP/s).  One JSON line per shape.
 
-    python scripts/bench_softmax.py [--shapes cora,pubmed,deezer,arxiv] [--precision fp32|bf16] [--steps 5]"""
+    python scripts/bench_softmax.py [--shapes cora,pubmed,deezer,arxiv] [--precision fp32|bf16] [--steps 5]
+
+--attention gat times SGFormerGAT's attention branch (medium/ablation/oursGAT.py, use_graph=False) instead: the native step in
+fp32 and in bf16, and the same model as the reference's torch einsums (oracle/gat_attention_oracle.py).  Flops are counted from
+shapes: the kernels' score work is 2 N^2 H^2 dk (every head's scores for each head written), the reference's 2 N^2 H dk plus
+2 N^2 H h for the values.
+
+    python scripts/bench_softmax.py --attention gat [--shapes ...] [--steps 5]"""
 import argparse
 import json
 import os
@@ -14,8 +21,9 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import gat_attention_oracle as OG  # noqa: E402
 from oracle import softmax_oracle as O  # noqa: E402
-from sgformer_b200 import ablation, medium  # noqa: E402
+from sgformer_b200 import ablation, ablation_gat, medium  # noqa: E402
 from sgformer_b200 import engine as E  # noqa: E402
 from sgformer_b200 import kernels as K  # noqa: E402
 
@@ -57,8 +65,39 @@ def _torch_step(sd, x, layers, heads):
     return f
 
 
+def _gat_torch_step(sd, x, layers, heads):
+    def f():
+        for t in sd.values():
+            t.grad = None
+        OG.sgformer_gat(sd, x, layers, heads).sum().backward()
+    return f
+
+
+def _gat_shape(name, a, card):
+    n, f, h, c = SHAPES[name]
+    H, dk = a.heads, h // a.heads
+    torch.manual_seed(0)
+    x = torch.randn(n, f, device="cuda")
+    data = _Data(x)
+    rec = dict(attention="gat", shape=name, n=n, hidden=h, heads=H, layers=a.layers, card=card,
+               kernel_score_flops=2.0 * n * n * H * H * dk * a.layers, reference_flops=(2.0 * n * n * H * dk + 2.0 * n * n * H * h) * a.layers)
+    m = ablation_gat.SGFormerGAT(f, h, c, num_layers=a.layers, num_heads=H, dropout=0.0, use_graph=False).cuda().train()
+    for prec in ("fp32", "bf16"):
+        m.set_precision(prec)
+        rec[f"native_{prec}_ms"] = _time(_step(m, data), a.steps)
+    sd = {k: v.detach().clone().requires_grad_() for k, v in m.state_dict().items()}
+    try:
+        rec["torch_ms"] = _time(_gat_torch_step(sd, x, a.layers, H), a.steps, warmup=1)
+    except torch.OutOfMemoryError:
+        rec["torch_ms"] = "out of memory"
+    print(json.dumps(rec), flush=True)
+    del m, sd
+    torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--attention", default="softmax", choices=["softmax", "gat"])
     ap.add_argument("--shapes", default="cora,pubmed,deezer,arxiv")
     ap.add_argument("--precision", default="fp32", choices=["fp32", "bf16"])
     ap.add_argument("--steps", type=int, default=5)
@@ -67,6 +106,10 @@ def main():
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                           text=True).stdout.strip()
+    if a.attention == "gat":
+        for name in a.shapes.split(","):
+            _gat_shape(name, a, card)
+        return
     for name in a.shapes.split(","):
         n, f, h, c = SHAPES[name]
         torch.manual_seed(0)

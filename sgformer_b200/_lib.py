@@ -67,6 +67,7 @@ class AttnSoftmaxArgs(C.Structure):
         ("dv", _vp), ("lddv", _i64), ("dv_accumulate", _i32),
         ("dq", _vp), ("lddq", _i64), ("dk", _vp), ("lddk", _i64),
         ("ws", _vp), ("ws_floats", _i64),
+        ("scaled", _i32), ("scale", _f32),
     ]
 
 

@@ -22,8 +22,8 @@ def make_config(variant: str, in_channels: int, hidden: int, out_channels: int, 
         raise ValueError(f"unknown GNN kind {cfg['gnn_kind']!r}")
     if cfg["gcn_jk"] not in ("max", "cat"):
         raise ValueError(f"unknown JumpingKnowledge mode {cfg['gcn_jk']!r}")
-    if cfg["trans_attention"] not in ("linear", "softmax"):
-        raise ValueError(f"unknown TransConv attention {cfg['trans_attention']!r} (use 'linear' or 'softmax')")
+    if cfg["trans_attention"] not in ("linear", "softmax", "gat"):
+        raise ValueError(f"unknown TransConv attention {cfg['trans_attention']!r} (use 'linear', 'softmax' or 'gat')")
     if cfg["aggregate"] not in ("add", "cat"):
         raise ValueError(f"Invalid aggregate type:{cfg['aggregate']}")
     return cfg

@@ -23,6 +23,19 @@
 //   norm     dq = gs (Aq - <q,Aq>/||q||^2 q),  dk = gs (Ak - <k,Ak>/||k||^2 k)  (the norm backward; <q,Aq> from per-CTA partials
 //            that bwd_q / bwd_kv write, summed in a fixed order)
 // G is the gradient of o (per head, or one [n, d] block shared by every head: the head mean's); gs (gscale) scales every output.
+//
+// Scaled mode (SCALED, args.scaled = 1): the scaled dot-product attention of SGFormerGAT (medium/ablation/oursGAT.py:31-44),
+//   s[n,l,h] = c q[n,h].k[l,h] with a host constant c = args.scale (1/sqrt(dk)), the same softmax over the heads and the same o.
+// Nothing bounds these scores (exp overflows fp32 once c q.k > 88), so each pair's exponents are taken relative to the pair's
+// maximum over the heads.  The thread that holds a pair's score fragment holds that pair's score for every head, so the maximum
+// needs no cross-thread reduction; it is kept online while the head loop runs: E_h' = exp(c (s_h' - mx)) against the running
+// maximum mx, and when a head raises mx every term accumulated so far (E_h, den, and the backward's numerator) is rescaled by
+// exp(c (mx_old - mx_new)).  A separate max pass would recompute every head's score tile (H more 16 x 16 mma blocks per block
+// of pairs) to save one multiply per accumulated term; the online rescale costs one exp2f per head and pair, as the
+// unscaled mode does.  Every exponent is <= 0 and the own head's or the maximum's term is 1, so den lies in [1, H].
+// The backward recomputes the same maximum and the same dS_h; there is no norm backward: the sweeps write
+//   dq_h = gs c dS_h K_h (bwd_q) and dk_h = gs c dS_h^T Q_h (bwd_kv) directly in the activation dtype, no <q,Aq> partials.
+// dV is unchanged (v is always per head in this mode).  With one head P = 1 and dS = 0 exactly, as in the unscaled mode.
 // Precision: bf16 activations use one bf16 plane; fp32 activations split every operand (and P, dS in registers) into bf16 hi/lo
 // planes and accumulate hi.hi + hi.lo + lo.hi (the bf16x3 scheme of the GEMMs: fp32-accurate products).
 #include "common.cuh"
@@ -167,12 +180,40 @@ __device__ __forceinline__ void tile16(float (&s)[2][4], const T* A, int lda, in
 __device__ __forceinline__ float c_scale(const sgf_attn_softmax_args& a) {
     return (float)(1.0 / (sqrt(fixed_sum(a.sq_q, a.heads * a.m)) * sqrt(fixed_sum(a.sq_k, a.heads * a.m))));
 }
+template <bool SCALED> __device__ __forceinline__ float score_scale(const sgf_attn_softmax_args& a) {
+    return SCALED ? a.scale : c_scale(a);
+}
+
+// Scaled mode: the first head's raw score s of a pair starts its running maximum; its term is exp(0) = 1.
+__device__ __forceinline__ void max_first(float (&s)[2][4], float (&mx)[2][4], float (&eh)[2][4], float (&den)[2][4]) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) { mx[j][e] = s[j][e]; eh[j][e] = den[j][e] = 1.f; }
+}
+// Scaled mode: one more head's raw score s of a pair.  ex = exp(-c |s - mx|): below the running maximum it is the new term;
+// above it, the factor r that rescales what has been accumulated (and the new head's term is 1; else r = 1).  Returns the new
+// term.
+__device__ __forceinline__ float max_step(float s, float cl2, float& mx, float& eh, float& den, float& r) {
+    const float dd = (s - mx) * cl2;
+    const float ex = exp2f(-fabsf(dd));
+    if (dd > 0.f) {
+        r = ex;
+        eh *= ex;
+        den = fmaf(den, ex, 1.f);
+        mx = s;
+        return 1.f;
+    }
+    r = 1.f;
+    den += ex;
+    return ex;
+}
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // forward: query tile x head h x 128-column block of v_h.  Per 16-key block: E_h' = exp(c Q_h' K_h'^T) for every head,
 // P_h = E_h / sum_h' E_h', o_h += P_h V_h.
 // ---------------------------------------------------------------------------------------------------------------------------
-template <typename T, int BS>
+template <typename T, int BS, bool SCALED>
 __global__ void __launch_bounds__(kThreads, 1) fwd_kernel(const __grid_constant__ sgf_attn_softmax_args a) {
     constexpr bool SPLIT = std::is_same<T, float>::value;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -189,7 +230,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_kernel(const __grid_constant_
     const T* v = static_cast<const T*>(a.v) + (a.shared_v ? 0 : (int64_t)h * D);
     const int64_t row0 = (int64_t)blockIdx.x * kRows;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c4 = lane & 3;
-    if (threadIdx.x == 0) s_c = c_scale(a);
+    if (threadIdx.x == 0) s_c = score_scale<SCALED>(a);
 
     const int nt = (n + BS - 1) / BS;
     load_heads(Qs, slq, q, a.ldq, row0, kRows, n, H, M);
@@ -218,19 +259,30 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_kernel(const __grid_constant_
         const T* Vb = Vs + buf * BS * slv;
 #pragma unroll 1
         for (int sb = 0; sb < BS; sb += 16) {
-            float s[2][4], eh[2][4], den[2][4];
+            float s[2][4], eh[2][4], den[2][4], mx[2][4];
             tile16<SPLIT>(s, Qs, slq, r0, h * Mp, Kb, slq, sb, h * Mp, Mp, lane);
+            if (SCALED) {
+                max_first(s, mx, eh, den);
+            } else {
 #pragma unroll
-            for (int j = 0; j < 2; ++j)
+                for (int j = 0; j < 2; ++j)
 #pragma unroll
-                for (int e = 0; e < 4; ++e) den[j][e] = eh[j][e] = exp2f(s[j][e] * cl2);
+                    for (int e = 0; e < 4; ++e) den[j][e] = eh[j][e] = exp2f(s[j][e] * cl2);
+            }
             for (int hp = 0; hp < H; ++hp) {      // the other heads' terms of the softmax over heads, in head order
                 if (hp == h) continue;
                 tile16<SPLIT>(s, Qs, slq, r0, hp * Mp, Kb, slq, sb, hp * Mp, Mp, lane);
 #pragma unroll
                 for (int j = 0; j < 2; ++j)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) den[j][e] += exp2f(s[j][e] * cl2);
+                    for (int e = 0; e < 4; ++e) {
+                        if (SCALED) {
+                            float r;
+                            max_step(s[j][e], cl2, mx[j][e], eh[j][e], den[j][e], r);
+                        } else {
+                            den[j][e] += exp2f(s[j][e] * cl2);
+                        }
+                    }
             }
 #pragma unroll
             for (int j = 0; j < 2; ++j)
@@ -272,17 +324,22 @@ __device__ __forceinline__ void cta_partial(float v, float* red, float* out) {
 // dS_h of a 16 x 16 block: with E_h' = exp(c S_h') and dP_h' of every head (own head h first),
 //   dS_h = P_h (dP_h - sum_h' P_h' dP_h') = (E_h / den) * (sum_h' E_h' (dP_h - dP_h')) / den,   den = sum_h' E_h'.
 // The difference form is exactly zero when every head has the same dP (one head, or a shared v under the head mean).
-template <bool SPLIT, typename T>
+// Scaled mode: the same with E_h' relative to the pair's running maximum (num rescaled with den and E_h).
+template <bool SPLIT, bool SCALED, typename T>
 __device__ __forceinline__ void dscore16(float (&ds)[2][4], int h, int H, float cl2, const T* Qa, int lda, int r0, const T* Kb, int ldb,
                                          int b0, int Mp, const T* Ga, int ldga, const T* Vb, int ldvb, int Dp, bool shared_ga, bool shared_vb,
                                          int lane) {
-    float s[2][4], dp[2][4], dpo[2][4], eh[2][4], den[2][4], num[2][4];
+    float s[2][4], dp[2][4], dpo[2][4], eh[2][4], den[2][4], num[2][4], mx[2][4];
     tile16<SPLIT>(s, Qa, lda, r0, h * Mp, Kb, ldb, b0, h * Mp, Mp, lane);
     tile16<SPLIT>(dp, Ga, ldga, r0, shared_ga ? 0 : h * Dp, Vb, ldvb, b0, shared_vb ? 0 : h * Dp, Dp, lane);
+    if (SCALED) max_first(s, mx, eh, den);
 #pragma unroll
     for (int j = 0; j < 2; ++j)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) { den[j][e] = eh[j][e] = exp2f(s[j][e] * cl2); num[j][e] = 0.f; }
+        for (int e = 0; e < 4; ++e) {
+            if (!SCALED) den[j][e] = eh[j][e] = exp2f(s[j][e] * cl2);
+            num[j][e] = 0.f;
+        }
     for (int hp = 0; hp < H; ++hp) {
         if (hp == h) continue;
         tile16<SPLIT>(s, Qa, lda, r0, hp * Mp, Kb, ldb, b0, hp * Mp, Mp, lane);
@@ -291,9 +348,15 @@ __device__ __forceinline__ void dscore16(float (&ds)[2][4], int h, int H, float 
         for (int j = 0; j < 2; ++j)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float ex = exp2f(s[j][e] * cl2);
-                den[j][e] += ex;
-                num[j][e] += ex * (dp[j][e] - dpo[j][e]);
+                if (SCALED) {
+                    float r;
+                    const float ex = max_step(s[j][e], cl2, mx[j][e], eh[j][e], den[j][e], r);
+                    num[j][e] = fmaf(num[j][e], r, ex * (dp[j][e] - dpo[j][e]));
+                } else {
+                    const float ex = exp2f(s[j][e] * cl2);
+                    den[j][e] += ex;
+                    num[j][e] += ex * (dp[j][e] - dpo[j][e]);
+                }
             }
     }
 #pragma unroll
@@ -305,7 +368,7 @@ __device__ __forceinline__ void dscore16(float (&ds)[2][4], int h, int H, float 
 // ---------------------------------------------------------------------------------------------------------------------------
 // backward, query sweep: query tile x head h x 128-column block of q_h:  Aq_h = c dS_h K_h
 // ---------------------------------------------------------------------------------------------------------------------------
-template <typename T, int BS>
+template <typename T, int BS, bool SCALED>
 __global__ void __launch_bounds__(kThreads) bwd_q_kernel(const __grid_constant__ sgf_attn_softmax_args a) {
     constexpr bool SPLIT = std::is_same<T, float>::value;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -327,7 +390,7 @@ __global__ void __launch_bounds__(kThreads) bwd_q_kernel(const __grid_constant__
     const T* gp = static_cast<const T*>(a.g);
     const int64_t row0 = (int64_t)blockIdx.x * kRows;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c4 = lane & 3;
-    if (threadIdx.x == 0) s_c = c_scale(a);
+    if (threadIdx.x == 0) s_c = score_scale<SCALED>(a);
 
     const int nt = (n + BS - 1) / BS;
     load_heads(Qs, slq, q, a.ldq, row0, kRows, n, H, M);
@@ -358,7 +421,7 @@ __global__ void __launch_bounds__(kThreads) bwd_q_kernel(const __grid_constant__
 #pragma unroll 1
         for (int sb = 0; sb < BS; sb += 16) {
             float ds[2][4];
-            dscore16<SPLIT>(ds, h, H, cl2, Qs, slq, r0, Kb, slq, sb, Mp, Gs, slg, Vb, slv, Dp, sg, sv, lane);
+            dscore16<SPLIT, SCALED>(ds, h, H, cl2, Qs, slq, r0, Kb, slq, sb, Mp, Gs, slg, Vb, slv, Dp, sg, sv, lane);
 #pragma unroll
             for (int j = 0; j < 2; ++j)
 #pragma unroll
@@ -370,6 +433,23 @@ __global__ void __launch_bounds__(kThreads) bwd_q_kernel(const __grid_constant__
                 if (mj < nmt) mma<SPLIT>(acc[mj], da, ld_b_k(Kb, slq, sb, h * Mp + mc0 + mj * 8, lane));
         }
         __syncthreads();
+    }
+    if (SCALED) {       // dq = gs c acc
+        const float f = a.gscale * s_c;
+        T* dq = static_cast<T*>(a.dq) + (int64_t)h * M + mc0;
+#pragma unroll
+        for (int e2 = 0; e2 < 2; ++e2) {
+            const int64_t row = row0 + r0 + g + 8 * e2;
+            if (row >= n) continue;
+#pragma unroll
+            for (int mj = 0; mj < 16; ++mj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = mj * 8 + 2 * c4 + e;
+                    if (mj < nmt && col < mw) dq[row * a.lddq + col] = from_f32<T>(f * acc[mj][2 * e2 + e]);
+                }
+        }
+        return;
     }
     // Aq = c * acc; partial <q, Aq> of this CTA
     const float cs = s_c;
@@ -398,7 +478,7 @@ __global__ void __launch_bounds__(kThreads) bwd_q_kernel(const __grid_constant__
 // ---------------------------------------------------------------------------------------------------------------------------
 // backward, key sweep: key tile x head h x (128-column block of k_h: Ak_h = c dS_h^T Q_h | of v_h: dV_h = gs P_h^T G_h)
 // ---------------------------------------------------------------------------------------------------------------------------
-template <typename T, int BS>
+template <typename T, int BS, bool SCALED>
 __global__ void __launch_bounds__(kThreads) bwd_kv_kernel(const __grid_constant__ sgf_attn_softmax_args a) {
     constexpr bool SPLIT = std::is_same<T, float>::value;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -423,7 +503,7 @@ __global__ void __launch_bounds__(kThreads) bwd_kv_kernel(const __grid_constant_
     const T* gp = static_cast<const T*>(a.g);
     const int64_t row0 = (int64_t)blockIdx.x * kRows;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c4 = lane & 3;
-    if (threadIdx.x == 0) s_c = c_scale(a);
+    if (threadIdx.x == 0) s_c = score_scale<SCALED>(a);
     const int nj = (ow + 7) / 8;
     const int r0 = warp * 16;
     const int nt = (n + BS - 1) / BS;
@@ -457,21 +537,32 @@ __global__ void __launch_bounds__(kThreads) bwd_kv_kernel(const __grid_constant_
             for (int sb = 0; sb < BS; sb += 16) {
                 float w[2][4];
                 if (want_dk) {
-                    dscore16<SPLIT>(w, hd, H, cl2, Ks, slq, r0, Qb, slq, sb, Mp, Vs, slv, Gb, slg, Dp, sv, sg, lane);
+                    dscore16<SPLIT, SCALED>(w, hd, H, cl2, Ks, slq, r0, Qb, slq, sb, Mp, Vs, slv, Gb, slg, Dp, sv, sg, lane);
                 } else {       // P_h^T
-                    float s[2][4], den[2][4];
+                    float s[2][4], den[2][4], mx[2][4];
                     tile16<SPLIT>(s, Ks, slq, r0, hd * Mp, Qb, slq, sb, hd * Mp, Mp, lane);
+                    if (SCALED) {
+                        max_first(s, mx, w, den);
+                    } else {
 #pragma unroll
-                    for (int j = 0; j < 2; ++j)
+                        for (int j = 0; j < 2; ++j)
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) den[j][e] = w[j][e] = exp2f(s[j][e] * cl2);
+                            for (int e = 0; e < 4; ++e) den[j][e] = w[j][e] = exp2f(s[j][e] * cl2);
+                    }
                     for (int hp = 0; hp < H; ++hp) {
                         if (hp == hd) continue;
                         tile16<SPLIT>(s, Ks, slq, r0, hp * Mp, Qb, slq, sb, hp * Mp, Mp, lane);
 #pragma unroll
                         for (int j = 0; j < 2; ++j)
 #pragma unroll
-                            for (int e = 0; e < 4; ++e) den[j][e] += exp2f(s[j][e] * cl2);
+                            for (int e = 0; e < 4; ++e) {
+                                if (SCALED) {
+                                    float r;
+                                    max_step(s[j][e], cl2, mx[j][e], w[j][e], den[j][e], r);
+                                } else {
+                                    den[j][e] += exp2f(s[j][e] * cl2);
+                                }
+                            }
                     }
 #pragma unroll
                     for (int j = 0; j < 2; ++j)
@@ -497,7 +588,22 @@ __global__ void __launch_bounds__(kThreads) bwd_kv_kernel(const __grid_constant_
             __syncthreads();
         }
     }
-    if (want_dk) {      // Ak = c * acc; partial <k, Ak> of this CTA
+    if (SCALED && want_dk) {        // dk = gs c acc
+        const float f = a.gscale * s_c;
+        T* dk = static_cast<T*>(a.dk) + (int64_t)blockIdx.y * M + oc0;
+#pragma unroll
+        for (int e2 = 0; e2 < 2; ++e2) {
+            const int64_t row = row0 + r0 + g + 8 * e2;
+            if (row >= n) continue;
+#pragma unroll
+            for (int mj = 0; mj < 16; ++mj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = mj * 8 + 2 * c4 + e;
+                    if (mj < nj && col < ow) dk[row * a.lddk + col] = from_f32<T>(f * acc[mj][2 * e2 + e]);
+                }
+        }
+    } else if (want_dk) {      // Ak = c * acc; partial <k, Ak> of this CTA
         const float cs = s_c;
         float* ak = a.ak + (int64_t)blockIdx.y * M + oc0;
         float part = 0.f;
@@ -636,7 +742,9 @@ template <typename T> static bool aligned16(const void* p, int64_t ld) {
 // the padded head blocks of one q/k row and of one v row each take at most SGF_ATTN_SOFTMAX_MAX_ROW_BYTES
 template <typename T> static int check_common(const sgf_attn_softmax_args* a) {
     constexpr int E = 16 / sizeof(T);
-    if (!a || a->n <= 0 || a->heads <= 0 || a->m <= 0 || a->d <= 0 || !a->sq_q || !a->sq_k) return SGF_ERR_ARG;
+    if (!a || a->n <= 0 || a->heads <= 0 || a->m <= 0 || a->d <= 0) return SGF_ERR_ARG;
+    if (a->scaled != 0 && a->scaled != 1) return SGF_ERR_ARG;
+    if (a->scaled ? !(a->scale > 0.f && a->scale < INFINITY) || a->shared_v : !a->sq_q || !a->sq_k) return SGF_ERR_ARG;
     const int64_t vh = a->shared_v ? 1 : a->heads;
     if (a->m % E || a->d % E || (int64_t)a->heads * ceil16(a->m) * sizeof(T) > SGF_ATTN_SOFTMAX_MAX_ROW_BYTES ||
         vh * ceil16(a->d) * sizeof(T) > SGF_ATTN_SOFTMAX_MAX_ROW_BYTES)
@@ -656,9 +764,15 @@ template <typename K> static int launch(K kernel, dim3 grid, int threads, size_t
     do {                                                                                         \
         size_t sm = 0;                                                                           \
         const int bs = pick_bs<T>(a, kind, &sm);                                                 \
-        if (bs == 64) return launch(kern<T, 64>, grid, kThreads, sm, a, st);                     \
-        if (bs == 32) return launch(kern<T, 32>, grid, kThreads, sm, a, st);                     \
-        if (bs == 16) return launch(kern<T, 16>, grid, kThreads, sm, a, st);                     \
+        if (a->scaled) {                                                                         \
+            if (bs == 64) return launch(kern<T, 64, true>, grid, kThreads, sm, a, st);           \
+            if (bs == 32) return launch(kern<T, 32, true>, grid, kThreads, sm, a, st);           \
+            if (bs == 16) return launch(kern<T, 16, true>, grid, kThreads, sm, a, st);           \
+            return SGF_ERR_UNSUPPORTED;                                                          \
+        }                                                                                        \
+        if (bs == 64) return launch(kern<T, 64, false>, grid, kThreads, sm, a, st);              \
+        if (bs == 32) return launch(kern<T, 32, false>, grid, kThreads, sm, a, st);              \
+        if (bs == 16) return launch(kern<T, 16, false>, grid, kThreads, sm, a, st);              \
         return SGF_ERR_UNSUPPORTED;                                                              \
     } while (0)
 
@@ -675,16 +789,25 @@ static int64_t parts_q(int n, int heads, int m) { return (int64_t)((n + kRows - 
 template <typename T> static int bwd_check(const sgf_attn_softmax_args* a) {
     int rc = check_common<T>(a);
     if (rc) return rc;
-    if (!aligned16<T>(a->g, a->ldg) || (a->g_hstride != 0 && a->g_hstride != a->d) || !a->ws) return SGF_ERR_ARG;
+    if (!aligned16<T>(a->g, a->ldg) || (a->g_hstride != 0 && a->g_hstride != a->d)) return SGF_ERR_ARG;
+    if (a->scaled) return SGF_OK;       // no partial sums
+    if (!a->ws) return SGF_ERR_ARG;
     int64_t need = 0;
     sgf_attn_softmax_ws_floats(a->n, a->heads, a->m, a->d, &need);
     return a->ws_floats < need ? SGF_ERR_ARG : SGF_OK;
 }
 
+// the sweep's output: aq / ak (fp32, pitch ld_a), or in scaled mode dq / dk (dtype, pitch lddq / lddk)
+template <typename T> static bool grad_out_ok(const sgf_attn_softmax_args* a, const float* acc, const void* out, int64_t ld) {
+    const int64_t hm = (int64_t)a->heads * a->m;
+    if (!a->scaled) return acc && a->ld_a >= hm;
+    return out && (reinterpret_cast<uintptr_t>(out) % sizeof(T)) == 0 && ld >= hm;
+}
+
 template <typename T> static int bwd_q(const sgf_attn_softmax_args* a, cudaStream_t st) {
     int rc = bwd_check<T>(a);
     if (rc) return rc;
-    if (!a->aq || a->ld_a < (int64_t)a->heads * a->m) return SGF_ERR_ARG;
+    if (!grad_out_ok<T>(a, a->aq, a->dq, a->lddq)) return SGF_ERR_ARG;
     const dim3 grid((a->n + kRows - 1) / kRows, a->heads, (a->m + kOutCols - 1) / kOutCols);
     SGF_SOFT_LAUNCH(bwd_q_kernel, 1, grid);
 }
@@ -692,7 +815,7 @@ template <typename T> static int bwd_q(const sgf_attn_softmax_args* a, cudaStrea
 template <typename T> static int bwd_kv(const sgf_attn_softmax_args* a, cudaStream_t st) {
     int rc = bwd_check<T>(a);
     if (rc) return rc;
-    if (!a->ak || a->ld_a < (int64_t)a->heads * a->m || !a->dv) return SGF_ERR_ARG;
+    if (!grad_out_ok<T>(a, a->ak, a->dk, a->lddk) || !a->dv) return SGF_ERR_ARG;
     const int n_mc = (a->m + kOutCols - 1) / kOutCols, n_dc = (a->d + kOutCols - 1) / kOutCols;
     const dim3 grid((a->n + kRows - 1) / kRows, a->heads, n_mc + n_dc);
     SGF_SOFT_LAUNCH(bwd_kv_kernel, 2, grid);
@@ -700,7 +823,7 @@ template <typename T> static int bwd_kv(const sgf_attn_softmax_args* a, cudaStre
 
 template <typename T> static int bwd_norm(const sgf_attn_softmax_args* a, cudaStream_t st) {
     if (!a || a->n <= 0 || a->heads <= 0 || a->m <= 0 || !a->aq || !a->ak || !a->dq || !a->dk || !a->q || !a->k || !a->ws ||
-        !a->sq_q || !a->sq_k)
+        !a->sq_q || !a->sq_k || a->scaled)      // the scaled mode's sweeps write dq, dk themselves
         return SGF_ERR_ARG;
     const int64_t nq = parts_q(a->n, a->heads, a->m);
     const int64_t total = (int64_t)a->n * a->heads * a->m;
@@ -711,7 +834,8 @@ template <typename T> static int bwd_norm(const sgf_attn_softmax_args* a, cudaSt
 }
 
 template <typename T> static int probs(const sgf_attn_softmax_args* a, float* att, int64_t ld_att, cudaStream_t st) {
-    if (!a || a->n <= 0 || a->heads <= 0 || a->m <= 0 || !a->q || !a->k || !a->sq_q || !a->sq_k || !att || ld_att < a->n)
+    if (!a || a->n <= 0 || a->heads <= 0 || a->m <= 0 || !a->q || !a->k || !a->sq_q || !a->sq_k || !att || ld_att < a->n ||
+        a->scaled)
         return SGF_ERR_ARG;
     const int64_t total = (int64_t)a->n * a->n;
     const int blocks = (int)((total + 255) / 256 < 8 * num_sms() ? (total + 255) / 256 : 8 * num_sms());

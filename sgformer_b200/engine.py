@@ -253,6 +253,121 @@ def attention_softmax_backward(tape: Tape, g: Tensor, gscale: float, dq: Tensor,
 
 
 # =================================================================================================
+# scaled dot-product attention of SGFormerGAT (GATAttention, medium/ablation/oursGAT.py:13-44)
+# =================================================================================================
+def _gat_attn_dims(P, lp: str, heads: int, prec: Precision) -> Tuple[int, int, int]:
+    """-> (dk, padded dk, width of v per head) of layer `lp`.  The kernels read each head's q / k block at a multiple of 16 bytes,
+    so dk is padded to 4 (fp32) / 8 (bf16) columns."""
+    a = lp + "attention.attention."
+    dk = P[a + "Wq.weight"].shape[0] // heads
+    d = P[a + "Wv.weight"].shape[0] // heads
+    if dk == 0:
+        raise ValueError(f"sgformer_b200: GAT attention with {heads} heads needs hidden_channels >= num_heads (dk = hidden // heads is 0)")
+    return dk, gat_attn_pad(dk, prec), d
+
+
+def gat_attn_scale(dk: int) -> float:
+    """1/sqrt(dk) as oursGAT.py:37 takes it: the square root of an fp32 tensor holding dk."""
+    return 1.0 / float(torch.tensor(float(dk), dtype=torch.float32).sqrt())
+
+
+def gat_attn_pad(dk: int, prec: Precision) -> int:
+    """Width of a head's q / k block in the kernels' layout: dk padded to a multiple of 16 bytes."""
+    return K.ceil_to(dk, 16 // prec.act_dtype.itemsize)
+
+
+def gat_attn_pad_rows(t: Tensor, heads: int, dk: int, mp: int) -> Tensor:
+    """[heads*dk, ...] -> [heads*mp, ...]: each head's rows followed by mp - dk zero rows (differentiable)."""
+    if mp == dk:
+        return t
+    out = t.new_zeros((heads, mp) + tuple(t.shape[1:]))
+    out[:, :dk] = t.reshape((heads, dk) + tuple(t.shape[1:]))
+    return out.reshape((heads * mp,) + tuple(t.shape[1:]))
+
+
+def _gat_attn_unpad_rows(t: Tensor, heads: int, dk: int, mp: int) -> Tensor:
+    if mp == dk:
+        return t
+    return t.reshape((heads, mp) + tuple(t.shape[1:]))[:, :dk].reshape((heads * dk,) + tuple(t.shape[1:]))
+
+
+def _gat_attn_weight(P, lp: str, heads: int, dk: int, mp: int, use_weight: bool) -> (Tensor, Tensor):
+    """Packed weight / bias of the layer's first GEMM: [Wq | Wk] of GATAttention with each head's rows padded to mp, then (with
+    use_weight) TransConvLayerGAT.Wv, which gives u."""
+    a = lp + "attention.attention."
+    ws = [gat_attn_pad_rows(P[a + w + ".weight"], heads, dk, mp) for w in ("Wq", "Wk")]
+    bs = [gat_attn_pad_rows(P[a + w + ".bias"], heads, dk, mp) for w in ("Wq", "Wk")]
+    if use_weight:
+        ws.append(P[lp + "attention.Wv.weight"])
+        bs.append(P[lp + "attention.Wv.bias"])
+    return torch.cat(ws, 0), torch.cat(bs, 0)
+
+
+def _gat_attn_project(P, lp: str, x: Tensor, heads: int, use_weight: bool, prec: Precision):
+    """-> (q, k, u, v, scale, (dk, padded dk, width of the first GEMM)): one GEMM of x gives [q | k | u] (u = x without
+    use_weight), a second gives v = Wv_att u + b."""
+    dk, mp, d = _gat_attn_dims(P, lp, heads, prec)
+    if not K.attn_softmax_fits(heads, mp, d, prec.act_dtype, False):
+        raise ValueError(f"sgformer_b200: GAT attention with {heads} heads of key width {dk} and value width {d} in precision "
+                         f"'{prec.name}' is not supported: the heads' columns of one q row and of one v row, each padded to 16, "
+                         f"must take at most {K.ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+    wcat, bcat = _gat_attn_weight(P, lp, heads, dk, mp, use_weight)
+    nout = wcat.shape[0]
+    xop = K.as_operand(x, prec.planes, memo=True)
+    proj = torch.empty((x.shape[0], K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=x.device)[:, :nout]
+    K.gemm_nt([xop], [K.pack_operand(wcat, False, prec.planes)], [(0, 0, 0, 0, xop.k)], nout, proj, bias=bcat)
+    hq = heads * mp
+    q, k = proj[:, :hq], proj[:, hq:2 * hq]
+    u = proj[:, 2 * hq:] if use_weight else x
+    a = lp + "attention.attention."
+    uop = K.as_operand(u, prec.planes, memo=True)
+    v = K.alloc_act(x.shape[0], heads * d, prec.act_dtype, x.device)
+    K.gemm_nt([uop], [_w(P, a + "Wv.weight", prec)], [(0, 0, 0, 0, uop.k)], heads * d, v, bias=P[a + "Wv.bias"])
+    return q, k, u, v, gat_attn_scale(dk), (dk, mp, nout)
+
+
+def gat_attn_backward(P, lp: str, L: dict, da: Tensor, heads: int, use_weight: bool, prec: Precision, dprev: Tensor,
+                           dprev_accumulate: bool, grads: Dict[str, Tensor]):
+    """Backward of one GAT-attention layer from da = dL/d(head mean of o): the attention sweeps (dq, dk, dv), then
+    dWv_att = dv^T u, du = dv Wv_att, and one GEMM pair for [dq | dk | du] against [Wq; Wk; Wv] (the pad rows dropped from the
+    weight gradients).  Without use_weight, u = x and du adds to dprev directly.  The layer's own Wq / Wk / Wv and their biases
+    never reach the output (oursGAT.py:85-101) and get no gradient."""
+    at, x_in = L["attn"], L["x_in"]
+    dk, mp, nout = L["gat"]
+    n, dev = da.shape[0], da.device
+    a = lp + "attention.attention."
+    hq = heads * mp
+    d = at["v"].shape[1] // heads
+    dproj = torch.empty((n, K.ceil_to(nout, 8)), dtype=prec.act_dtype, device=dev)[:, :nout]
+    dv = K.alloc_act(n, heads * d, prec.act_dtype, dev)
+    K.attn_scaled_bwd(at["q"], at["k"], at["v"], heads, at["scale"], da, 1.0 / heads, dproj[:, :hq], dproj[:, hq:2 * hq], dv)
+    dv_op = K.as_operand(dv, prec.planes)
+    u = at["u"]
+    dwv = torch.empty((heads * d, u.shape[1]), dtype=torch.float32, device=dev)
+    K.gemm_tn(dv_op, K.as_operand(u, prec.planes, memo=True), dwv)
+    grads[a + "Wv.weight"] = dwv
+    grads[a + "Wv.bias"], _ = K.colstats(dv, want_sumsq=False)
+    wv_t = _w(P, a + "Wv.weight", prec, transpose=True)
+    if use_weight:
+        K.gemm_nt([dv_op], [wv_t], [(0, 0, 0, 0, heads * d)], u.shape[1], dproj[:, 2 * hq:])
+    else:
+        K.gemm_nt([dv_op], [wv_t], [(0, 0, 0, 0, heads * d)], u.shape[1], dprev, accumulate=dprev_accumulate)
+        dprev_accumulate = True
+    wcat, _ = _gat_attn_weight(P, lp, heads, dk, mp, use_weight)
+    dproj_op = K.as_operand(dproj, prec.planes)
+    K.gemm_nt([dproj_op], [K.pack_operand(wcat, True, prec.planes)], [(0, 0, 0, 0, nout)], x_in.shape[1], dprev,
+              accumulate=dprev_accumulate)
+    dw = torch.empty((nout, x_in.shape[1]), dtype=torch.float32, device=dev)
+    K.gemm_tn(dproj_op, K.as_operand(x_in, prec.planes, memo=True), dw)
+    dbias, _ = K.colstats(dproj, want_sumsq=False)
+    for j, nm in enumerate(("Wq", "Wk")):
+        grads[a + nm + ".weight"] = _gat_attn_unpad_rows(dw[j * hq:(j + 1) * hq], heads, dk, mp)
+        grads[a + nm + ".bias"] = _gat_attn_unpad_rows(dbias[j * hq:(j + 1) * hq], heads, dk, mp)
+    if use_weight:
+        grads[lp + "attention.Wv.weight"], grads[lp + "attention.Wv.bias"] = dw[2 * hq:], dbias[2 * hq:]
+
+
+# =================================================================================================
 # linear attention in Gram form (single head): projections + full_attention_conv without materialising q, k, v
 # =================================================================================================
 # With q = x Wq^T + bq, k = x Wk^T + bk, v = x Wv^T + bv every node-contracted quantity of full_attention_conv
@@ -419,12 +534,20 @@ def trans_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precisi
     ca, cb, use_res = _res_coef(cfg)
     use_weight = bool(cfg["trans_use_weight"])
     softmax = cfg["trans_attention"] == "softmax"
-    if softmax and comm.active:
-        raise NotImplementedError("sgformer_b200: row sharding of the softmax attention is not supported")
+    gat = cfg["trans_attention"] == "gat"
+    if (softmax or gat) and comm.active:
+        raise NotImplementedError(f"sgformer_b200: row sharding of the {cfg['trans_attention']} attention is not supported")
     for i in range(cfg["trans_num_layers"]):
         lp = f"{pfx}convs.{i}."
         at = Tape() if tape is not None else None
-        if softmax:
+        if gat:
+            q, k, u, v, scale, dims = _gat_attn_project(P, lp, x, H, use_weight, prec)
+            o = K.attn_scaled_fwd(q, k, v, H, scale)
+            if at is not None:
+                at.update(q=q, k=k, u=u, v=v, scale=scale)
+            a = K.head_mean(o, H, h) if H > 1 else o
+            saved = dict(gat=dims)
+        elif softmax:
             qkv, _, csq = _project_qkv(P, lp, K.as_operand(x, prec.planes, memo=True), use_weight, prec, stats=True)
             q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
             v = qkv[:, 2 * H * h:] if use_weight else x
@@ -459,6 +582,9 @@ def trans_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Prec
     tensor-core GEMM of the concatenated heads (sum over heads of per-head dot products) with 1/(H ||q|| ||k||) read from the
     device and the row normaliser as its row scale; the layer stack itself runs the un-fused attention (q, k materialised).
     Inference only (no dropout, no tape), O(N^2) memory like the reference: meant for small graphs."""
+    if cfg["trans_attention"] == "gat":
+        raise ValueError("sgformer_b200: SGFormerGAT has no attention matrices to return: the reference's TransConvLayer "
+                         "(medium/ablation/oursGAT.py:95-96) unpacks its attention output into two names and raises")
     h, H = cfg["hidden"], cfg["num_heads"]
     check_width(h, prec, "hidden_channels")
     n = xin.rows
@@ -515,6 +641,11 @@ def trans_backward(P, cfg: dict, tape: Tape, dout: Tensor, gscale: float, prec: 
                                                        seed + _SEED_LAYER + i, gs, use_res, dg, db, at["den"])
             dprev = dr if dr is not None else K.new_like(x_in)
             attention_gram_backward(P, lp, at, x_in, gnum, gden, cs, pg, sg, use_weight, prec, dprev, dr is not None, grads, comm)
+        elif L.get("gat"):
+            da, dr = K.ln_bwd(dcur, L["a"], x_in if use_res else None, ca, cb, P.get(bn + "weight"), P.get(bn + "bias"), L["st"],
+                              use_ln, bool(cfg["trans_use_act"]), p, seed + _SEED_LAYER + i, gs, use_res, dg, db)
+            dprev = dr if dr is not None else K.new_like(x_in)
+            gat_attn_backward(P, lp, L, da, H, use_weight, prec, dprev, dr is not None, grads)
         else:       # materialised q, k (and v with use_weight): several heads
             nout = L["nout"]
             da, dr = K.ln_bwd(dcur, L["a"], x_in if use_res else None, ca, cb, P.get(bn + "weight"), P.get(bn + "bias"), L["st"],

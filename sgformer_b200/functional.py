@@ -301,6 +301,40 @@ class SoftmaxAttentionFn(_TapeFunction):
                 _from_act(dv, dtv).reshape(n, vh, d), None, None)
 
 
+class ScaledAttentionFn(_TapeFunction):
+    """GATAttention's scaled dot-product attention (medium/ablation/oursGAT.py:36-43) on q, k in the kernels' layout: q, k
+    [N, H*mp], each head's dk columns followed by mp - dk zero columns (zero columns add nothing to q.k), v [N, H*D] ->
+    [N, H, D], the softmax over the heads of q.k / sqrt(dk)."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, heads, dk, prec):
+        n = q.shape[0]
+        mp, d = q.shape[1] // heads, v.shape[1] // heads
+        if k.shape != q.shape or v.shape[0] != n or mp != E.gat_attn_pad(dk, prec):
+            raise ValueError(f"GATAttention: q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} do not hold {heads} heads of "
+                             f"key width {dk} padded to {E.gat_attn_pad(dk, prec)}")
+        if not K.attn_softmax_fits(heads, mp, d, prec.act_dtype, False):
+            raise ValueError(f"sgformer_b200: GAT attention with {heads} heads of key width {dk} and value width {d} in precision "
+                             f"'{prec.name}' is not supported: the heads' columns of one q row and of one v row, each padded to 16, "
+                             f"must take at most {K.ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+        qa, ka, va = (_to_act(t, prec) for t in (q, k, v))
+        scale = E.gat_attn_scale(dk)
+        o = K.attn_scaled_fwd(qa, ka, va, heads, scale)
+        ctx.state = (qa, ka, va, scale, q.dtype, k.dtype, v.dtype, heads, prec) if _want_tape(ctx) else None
+        return _from_act(o, q.dtype).reshape(n, heads, d)
+
+    @staticmethod
+    def backward(ctx, g):
+        qa, ka, va, scale, dtq, dtk, dtv, heads, prec = ctx.state
+        n, _, d = g.shape
+        ga = _to_act(g.reshape(n, heads * d), prec)
+        dq, dk = (K.alloc_act(n, qa.shape[1], prec.act_dtype, g.device) for _ in range(2))
+        dv = K.alloc_act(n, heads * d, prec.act_dtype, g.device)
+        K.attn_scaled_bwd(qa, ka, va, heads, scale, ga, 1.0, dq, dk, dv)
+        ctx.state = None
+        return _from_act(dq, dtq), _from_act(dk, dtk), _from_act(dv, dtv), None, None, None
+
+
 class AttentionFn(_TapeFunction):
     """full_attention_conv(qs, ks, vs) -> [N, H, D]  (medium/ours.py:14-34, 100M/ours.py:12-43).  A one-head vs [N, 1, D]
     is shared by all H heads, as the reference's einsum broadcasts it; its gradient is the sum over the heads."""

@@ -1028,7 +1028,9 @@ def attn_softmax_fits(heads: int, m: int, d: int, dtype, shared_v: bool) -> bool
         (1 if shared_v else heads) * ceil_to(d, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES
 
 
-def _softmax_args(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Tensor, sq_k: Tensor, shared_v: bool) -> AttnSoftmaxArgs:
+def _softmax_args(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Optional[Tensor], sq_k: Optional[Tensor], shared_v: bool,
+                  scale: Optional[float] = None) -> AttnSoftmaxArgs:
+    """Arguments of both modes: the Frobenius-normalised scores (sq_q, sq_k), or with `scale` the scaled scores scale*q.k."""
     _use(q)
     n, hm = q.shape
     m = hm // heads
@@ -1039,7 +1041,10 @@ def _softmax_args(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Tensor, sq_
     a = AttnSoftmaxArgs()
     a.n, a.heads, a.m, a.d, a.dtype, a.shared_v = n, heads, m, d, dcode(q), int(shared_v)
     a.q, a.ldq, a.k, a.ldk, a.v, a.ldv = _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0)
-    a.sq_q, a.sq_k = _p(_f32vec(sq_q, hm, "sq_q")), _p(_f32vec(sq_k, hm, "sq_k"))
+    if scale is None:
+        a.sq_q, a.sq_k = _p(_f32vec(sq_q, hm, "sq_q")), _p(_f32vec(sq_k, hm, "sq_k"))
+    else:
+        a.scaled, a.scale = 1, float(scale)
     return a
 
 
@@ -1077,6 +1082,31 @@ def attn_softmax_bwd(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Tensor, 
     check(lib().sgf_attn_softmax_bwd_q(C.byref(a), _stream()), "sgf_attn_softmax_bwd_q")
     check(lib().sgf_attn_softmax_bwd_kv(C.byref(a), _stream()), "sgf_attn_softmax_bwd_kv")
     check(lib().sgf_attn_softmax_bwd_norm(C.byref(a), _stream()), "sgf_attn_softmax_bwd_norm")
+
+
+def attn_scaled_fwd(q: Tensor, k: Tensor, v: Tensor, heads: int, scale: float) -> Tensor:
+    """SGFormerGAT's scaled dot-product attention: P = softmax over the heads of s[n,l,:] = scale q_n.k_l per head (against
+    each pair's maximum over the heads); o_h = sum_l P[:,l,h] v_l,h.  q, k [N, H*M], v [N, H*D] -> o [N, H*D] in q's dtype."""
+    n = q.shape[0]
+    a = _softmax_args(q, k, v, heads, None, None, False, scale)
+    o = alloc_act(n, v.shape[1], q.dtype, q.device)
+    a.o, a.ldo = _p(o), o.stride(0)
+    check(lib().sgf_attn_softmax_fwd(C.byref(a), _stream()), "sgf_attn_softmax_fwd")
+    return o
+
+
+def attn_scaled_bwd(q: Tensor, k: Tensor, v: Tensor, heads: int, scale: float, g: Tensor, gscale: float, dq: Tensor, dk: Tensor,
+                    dv: Tensor, dv_accumulate: bool = False):
+    """Backward of attn_scaled_fwd for the gradient gscale*g of o (g [N, H*D], or [N, D] shared by every head): writes dq, dk
+    [N, H*M] and dv [N, H*D] (+= with dv_accumulate).  Two launches, no workspace."""
+    d = v.shape[1] // heads
+    shared_g = g.shape[1] == d and heads > 1
+    a = _softmax_args(q, k, v, heads, None, None, False, scale)
+    a.g, a.ldg, a.g_hstride, a.gscale = _p(g), g.stride(0), 0 if shared_g else d, float(gscale)
+    a.dv, a.lddv, a.dv_accumulate = _p(dv), dv.stride(0), int(dv_accumulate)
+    a.dq, a.lddq, a.dk, a.lddk = _p(dq), dq.stride(0), _p(dk), dk.stride(0)
+    check(lib().sgf_attn_softmax_bwd_q(C.byref(a), _stream()), "sgf_attn_softmax_bwd_q")
+    check(lib().sgf_attn_softmax_bwd_kv(C.byref(a), _stream()), "sgf_attn_softmax_bwd_kv")
 
 
 def attn_softmax_probs(q: Tensor, k: Tensor, heads: int, sq_q: Tensor, sq_k: Tensor) -> Tensor:

@@ -120,7 +120,7 @@ class TransConvLayerBase(_Base):
 
 class TransConvBase(_Base):
     variant = "large"
-    attention = "linear"        # engine config `trans_attention`: "softmax" for SGFormerSOFT's TransConv
+    attention = "linear"        # engine config `trans_attention`: "softmax" / "gat" for SGFormerSOFT's / SGFormerGAT's TransConv
 
     def _build(self, in_channels, hidden_channels, num_layers, num_heads, use_weight, layer_cls):
         self.convs = nn.ModuleList()
