@@ -532,7 +532,11 @@ int sgf_attn_gram_prepare_bwd_vsum(const sgf_attn_gram_args* args /* host */, vo
  * Scaled mode (scaled = 1; SGFormerGAT, medium/ablation/oursGAT.py:31-44): s[n,l,h] = scale q[n,h].k[l,h] with a host constant
  * scale > 0 (1/sqrt(dk)), the softmax over the heads taken against each pair's maximum over the heads; sq_q, sq_k, ws, aq, ak
  * are unused and v is per head (shared_v = 0).  fwd as above; bwd_q writes dq = gscale scale dS k and bwd_kv writes
- * dk = gscale scale dS^T q (dtype, pitches lddq / lddk) and dv as above.  bwd_norm and probs refuse this mode. */
+ * dk = gscale scale dS^T q (dtype, pitches lddq / lddk) and dv as above.  bwd_norm and probs refuse this mode.
+ * tile_rows (host only, no CUDA call): rows[0..2] = the height of the streamed tile (64, 32 or 16 rows) that fwd, bwd_q and bwd_kv
+ * pick for this shape in either mode, 0 where no height fits in shared memory (that launch returns SGF_ERR_UNSUPPORTED);
+ * shared_g: the backward's g is one [n, d] block for every head (g_hstride = 0), else one block per head.  SGF_ERR_UNSUPPORTED for
+ * widths the launches refuse (not multiples of 16 bytes, or past SGF_ATTN_SOFTMAX_MAX_ROW_BYTES). */
 #define SGF_ATTN_SOFTMAX_MAX_ROW_BYTES 1024
 typedef struct {
     int32_t n, heads, m, d, dtype, shared_v;
@@ -550,6 +554,7 @@ typedef struct {
     int32_t scaled; float scale;    /* 1: scaled mode (below); 0: the Frobenius-normalised scores above */
 } sgf_attn_softmax_args;
 int sgf_attn_softmax_ws_floats(int n, int heads, int m, int d, int64_t* n_floats /* host out */);
+int sgf_attn_softmax_tile_rows(int heads, int m, int d, int dtype, int shared_v, int shared_g, int32_t rows[3] /* host out */);
 int sgf_attn_softmax_fwd(const sgf_attn_softmax_args* args /* host */, void* stream);
 int sgf_attn_softmax_bwd_q(const sgf_attn_softmax_args* args /* host */, void* stream);
 int sgf_attn_softmax_bwd_kv(const sgf_attn_softmax_args* args /* host */, void* stream);

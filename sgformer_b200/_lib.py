@@ -149,6 +149,7 @@ _SIGS = {
     "sgf_attn_gram_prepare_fwd_vsum": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
     "sgf_attn_gram_prepare_bwd_vsum": (C.c_int, [C.POINTER(AttnGramArgs), _vp]),
     "sgf_attn_softmax_ws_floats": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_i64)]),
+    "sgf_attn_softmax_tile_rows": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_i32)]),
     "sgf_attn_softmax_fwd": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),
     "sgf_attn_softmax_bwd_q": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),
     "sgf_attn_softmax_bwd_kv": (C.c_int, [C.POINTER(AttnSoftmaxArgs), _vp]),

@@ -711,19 +711,18 @@ __global__ void __launch_bounds__(256) probs_kernel(const __grid_constant__ sgf_
 // ---------------------------------------------------------------------------------------------------------------------------
 constexpr int kSmemMax = 227 * 1024;
 
-struct Widths {      // shared-memory row strides (elements) of the all-head q/k rows, the v rows and the g rows
-    int slq, slv, slg;
+struct Widths {      // shared-memory row strides (elements) of the all-head q/k rows, the v rows and the g rows; d: v's width
+    int slq, slv, slg, d;
 };
-template <typename T> static Widths widths(const sgf_attn_softmax_args* a) {
+template <typename T> static Widths widths(int heads, int m, int d, bool shared_v, bool shared_g) {
     constexpr int E = 16 / sizeof(T);
-    const int gh = a->g_hstride == 0 ? 1 : a->heads, vh = a->shared_v ? 1 : a->heads;
-    return Widths{a->heads * ceil16(a->m) + E, vh * ceil16(a->d) + E, gh * ceil16(a->d) + E};
+    const int gh = shared_g ? 1 : heads, vh = shared_v ? 1 : heads;
+    return Widths{heads * ceil16(m) + E, vh * ceil16(d) + E, gh * ceil16(d) + E, d};
 }
 // largest streamed tile (64, 32 or 16 rows) whose double buffer fits next to the resident tiles; the static shared memory is
-// counted with a margin.  kind 0: fwd, 1: bwd_q, 2: bwd_kv
-template <typename T> static int pick_bs(const sgf_attn_softmax_args* a, int kind, size_t* bytes) {
-    const Widths w = widths<T>(a);
-    const int dw = a->d < kOutCols ? a->d : kOutCols;
+// counted with a margin.  kind 0: fwd, 1: bwd_q, 2: bwd_kv.  0: none fits.
+template <typename T> static int pick_bs(const Widths& w, int kind, size_t* bytes) {
+    const int dw = w.d < kOutCols ? w.d : kOutCols;
     for (int bs : {64, 32, 16}) {
         size_t e = 0;
         if (kind == 0) e = (size_t)kRows * w.slq + 2 * (size_t)bs * (w.slq + row_stride<T>(dw));
@@ -734,22 +733,38 @@ template <typename T> static int pick_bs(const sgf_attn_softmax_args* a, int kin
     }
     return 0;
 }
+template <typename T> static int pick_bs(const sgf_attn_softmax_args* a, int kind, size_t* bytes) {
+    return pick_bs<T>(widths<T>(a->heads, a->m, a->d, a->shared_v != 0, a->g_hstride == 0), kind, bytes);
+}
 
 template <typename T> static bool aligned16(const void* p, int64_t ld) {
     return p && (reinterpret_cast<uintptr_t>(p) & 15u) == 0 && (ld * (int64_t)sizeof(T)) % 16 == 0;
 }
 
-// the padded head blocks of one q/k row and of one v row each take at most SGF_ATTN_SOFTMAX_MAX_ROW_BYTES
-template <typename T> static int check_common(const sgf_attn_softmax_args* a) {
+// m and d are multiples of 16 bytes, and the padded head blocks of one q/k row and of one v row each take at most
+// SGF_ATTN_SOFTMAX_MAX_ROW_BYTES
+template <typename T> static bool shape_ok(int heads, int m, int d, bool shared_v) {
     constexpr int E = 16 / sizeof(T);
+    const int64_t vh = shared_v ? 1 : heads;
+    return m % E == 0 && d % E == 0 && (int64_t)heads * ceil16(m) * sizeof(T) <= SGF_ATTN_SOFTMAX_MAX_ROW_BYTES &&
+           vh * ceil16(d) * sizeof(T) <= SGF_ATTN_SOFTMAX_MAX_ROW_BYTES;
+}
+
+template <typename T> static int check_common(const sgf_attn_softmax_args* a) {
     if (!a || a->n <= 0 || a->heads <= 0 || a->m <= 0 || a->d <= 0) return SGF_ERR_ARG;
     if (a->scaled != 0 && a->scaled != 1) return SGF_ERR_ARG;
     if (a->scaled ? !(a->scale > 0.f && a->scale < INFINITY) || a->shared_v : !a->sq_q || !a->sq_k) return SGF_ERR_ARG;
-    const int64_t vh = a->shared_v ? 1 : a->heads;
-    if (a->m % E || a->d % E || (int64_t)a->heads * ceil16(a->m) * sizeof(T) > SGF_ATTN_SOFTMAX_MAX_ROW_BYTES ||
-        vh * ceil16(a->d) * sizeof(T) > SGF_ATTN_SOFTMAX_MAX_ROW_BYTES)
-        return SGF_ERR_UNSUPPORTED;
+    if (!shape_ok<T>(a->heads, a->m, a->d, a->shared_v != 0)) return SGF_ERR_UNSUPPORTED;
     if (!aligned16<T>(a->q, a->ldq) || !aligned16<T>(a->k, a->ldk) || !aligned16<T>(a->v, a->ldv)) return SGF_ERR_ARG;
+    return SGF_OK;
+}
+
+// host only (no CUDA call): the streamed-tile heights the fwd, bwd_q and bwd_kv launches would pick
+template <typename T> static int tile_rows(int heads, int m, int d, bool shared_v, bool shared_g, int32_t* rows) {
+    if (!shape_ok<T>(heads, m, d, shared_v)) return SGF_ERR_UNSUPPORTED;
+    const Widths w = widths<T>(heads, m, d, shared_v, shared_g);
+    size_t bytes = 0;
+    for (int kind = 0; kind < 3; ++kind) rows[kind] = pick_bs<T>(w, kind, &bytes);
     return SGF_OK;
 }
 
@@ -853,6 +868,13 @@ extern "C" int sgf_attn_softmax_ws_floats(int n, int heads, int m, int d, int64_
     if (!n_floats || n <= 0 || heads <= 0 || m <= 0 || d <= 0) return SGF_ERR_ARG;
     *n_floats = 2 * parts_q(n, heads, m);        // bwd_q's and bwd_kv's per-CTA partials (same grid extent)
     return SGF_OK;
+}
+
+extern "C" int sgf_attn_softmax_tile_rows(int heads, int m, int d, int dtype, int shared_v, int shared_g, int32_t rows[3]) {
+    if (!rows || heads <= 0 || m <= 0 || d <= 0) return SGF_ERR_ARG;
+    if (dtype == 0) return tile_rows<float>(heads, m, d, shared_v != 0, shared_g != 0, rows);
+    if (dtype == 1) return tile_rows<__nv_bfloat16>(heads, m, d, shared_v != 0, shared_g != 0, rows);
+    return SGF_ERR_ARG;
 }
 
 #define SGF_SOFT_DISPATCH(fn, ...)                                                                 \

@@ -20,6 +20,9 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import kernels as K
+# Host-only shape queries of the compiled attention kernels (no launch, no GPU needed): bound here rather than read through K,
+# which tests replace with a CPU emulation of the launches, so that the same library answers which shapes run either way.
+from .kernels import ATTN_SOFTMAX_MAX_ROW_BYTES, attn_softmax_fits, attn_softmax_tile_rows
 from ._lib import EPI_ATTN_APPLY, EPI_ATTN_GRAM
 from .dist import SINGLE, Comm
 from .graph import Graph
@@ -220,17 +223,34 @@ def attention_backward(tape: Tape, g: Tensor, gscale: float, prec: Precision, dq
 # =================================================================================================
 # softmax attention core (SGFormerSOFT's softmax_attention, medium/ablation/oursSOFT.py:14-34)
 # =================================================================================================
+def check_attn_softmax(what: str, heads: int, m: int, d: int, prec: Precision, shared_v: bool, shared_g: Optional[bool]):
+    """Refuse, before anything is launched, a shape the fused attention kernels (csrc/attn_softmax.cu) cannot run.  shared_g: the
+    gradient the backward will receive, one [N, D] block for every head (True, the head mean's) or one block per head (False);
+    None when no backward follows, so that only the forward has to fit."""
+    if attn_softmax_fits(heads, m, d, prec.act_dtype, shared_v, bool(shared_g)):
+        return
+    rows = attn_softmax_tile_rows(heads, m, d, prec.act_dtype, shared_v, bool(shared_g))
+    if rows is None:
+        raise ValueError(f"sgformer_b200: {what} in precision '{prec.name}' is not supported: each head's q and v columns must be a "
+                         f"multiple of 16 bytes, and the heads' columns of one q row and of one v row, each padded to 16, must take "
+                         f"at most {ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+    if shared_g is None and rows[0] != 0:
+        return
+    g = f"one gradient block of width {d} shared by every head" if shared_g else f"a gradient block of width {d} for each of {heads} heads"
+    raise ValueError(f"sgformer_b200: {what} in precision '{prec.name}' is not supported: its backward (bwd_q / bwd_kv) has no "
+                     f"streamed tile that fits in shared memory next to {g}")
+
+
 def attention_softmax_forward(q: Tensor, k: Tensor, v: Tensor, heads: int, prec: Precision, tape: Optional[Tape], stats=None,
-                              shared_v: bool = False) -> Tensor:
+                              shared_v: bool = False, shared_g: Optional[bool] = False) -> Tensor:
     """q, k: [N, H*M], v: [N, H*D] (or [N, D] shared by every head) -> o [N, H*D] of SGFormerSOFT's softmax_attention: one
     Frobenius norm over all heads, s[n,l,h] = q~[n,h].k~[l,h], softmax over the HEADS of s[n,l,:] (oursSOFT.py:21-22 applies
     F.softmax(dim=-1) to [N, L, H] scores), o[n,h] = sum_l P[n,l,h] v[l,h].  stats: (sums of squares of q's columns, of k's
-    columns), e.g. from the projection's epilogue.  The fused kernel never stores an N x N tile (csrc/attn_softmax.cu)."""
+    columns), e.g. from the projection's epilogue.  shared_g: the gradient attention_softmax_backward will receive (see
+    check_attn_softmax; None: no backward).  The fused kernel never stores an N x N tile (csrc/attn_softmax.cu)."""
     m = q.shape[1] // heads
     d = v.shape[1] if shared_v else v.shape[1] // heads
-    if not K.attn_softmax_fits(heads, m, d, q.dtype, shared_v):
-        raise ValueError(f"sgformer_b200: softmax attention with {heads} heads of width {m} in precision '{prec.name}' is not supported: "
-                         f"the heads' columns of one row, each padded to 16, must take at most {K.ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+    check_attn_softmax(f"softmax attention with {heads} heads of width {m} and value width {d}", heads, m, d, prec, shared_v, shared_g)
     if stats is None:
         _, sq_q = K.colstats(q, want_sum=False)
         _, sq_k = K.colstats(k, want_sum=False)
@@ -307,10 +327,7 @@ def _gat_attn_project(P, lp: str, x: Tensor, heads: int, use_weight: bool, prec:
     """-> (q, k, u, v, scale, (dk, padded dk, width of the first GEMM)): one GEMM of x gives [q | k | u] (u = x without
     use_weight), a second gives v = Wv_att u + b."""
     dk, mp, d = _gat_attn_dims(P, lp, heads, prec)
-    if not K.attn_softmax_fits(heads, mp, d, prec.act_dtype, False):
-        raise ValueError(f"sgformer_b200: GAT attention with {heads} heads of key width {dk} and value width {d} in precision "
-                         f"'{prec.name}' is not supported: the heads' columns of one q row and of one v row, each padded to 16, "
-                         f"must take at most {K.ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+    check_attn_softmax(f"GAT attention with {heads} heads of key width {dk} and value width {d}", heads, mp, d, prec, False, heads > 1)
     wcat, bcat = _gat_attn_weight(P, lp, heads, dk, mp, use_weight)
     nout = wcat.shape[0]
     xop = K.as_operand(x, prec.planes, memo=True)
@@ -551,7 +568,8 @@ def trans_forward(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Precisi
             qkv, _, csq = _project_qkv(P, lp, K.as_operand(x, prec.planes, memo=True), use_weight, prec, stats=True)
             q, k = qkv[:, :H * h], qkv[:, H * h:2 * H * h]
             v = qkv[:, 2 * H * h:] if use_weight else x
-            o = attention_softmax_forward(q, k, v, H, prec, at, stats=(csq[:H * h], csq[H * h:2 * H * h]), shared_v=not use_weight)
+            o = attention_softmax_forward(q, k, v, H, prec, at, stats=(csq[:H * h], csq[H * h:2 * H * h]), shared_v=not use_weight,
+                                          shared_g=H > 1)
             a = K.head_mean(o, H, h) if H > 1 else o
             saved = dict(nout=qkv.shape[1], softmax=True)
         elif H == 1:
@@ -601,7 +619,7 @@ def trans_attentions(P: Dict[str, Tensor], cfg: dict, xin: K.Operand, prec: Prec
         v = qkv[:, 2 * H * h:] if use_weight else x
         at = Tape()
         if cfg["trans_attention"] == "softmax":       # head mean of the softmax weights (oursSOFT.py:28-29)
-            o = attention_softmax_forward(q, k, v, H, prec, at, shared_v=not use_weight)
+            o = attention_softmax_forward(q, k, v, H, prec, at, shared_v=not use_weight, shared_g=None)
             out.append(K.attn_softmax_probs(q, k, H, at["sq_q"], at["sq_k"]))
             a = K.head_mean(o, H, h) if H > 1 else o
             x, _ = K.ln_fwd(a, x if use_res else None, ca, cb, P.get(f"{pfx}bns.{i + 1}.weight"), P.get(f"{pfx}bns.{i + 1}.bias"),

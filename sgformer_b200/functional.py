@@ -276,11 +276,13 @@ class SoftmaxAttentionFn(_TapeFunction):
         if k.shape != q.shape or v.shape[0] != n or vh not in (1, heads):
             raise ValueError(f"softmax_attention: qs {tuple(q.shape)}, ks {tuple(k.shape)}, vs {tuple(v.shape)}: ks must match qs "
                              f"and vs must have {n} rows and 1 or {heads} heads")
+        want = _want_tape(ctx)
         qa, ka, va = (_to_act(t.reshape(n, -1), prec) for t in (q, k, v))
         tape = E.Tape()
-        o = E.attention_softmax_forward(qa, ka, va, heads, prec, tape, shared_v=vh != heads)
+        # the backward passes each head its own gradient block: refuse here a shape whose backward could not run
+        o = E.attention_softmax_forward(qa, ka, va, heads, prec, tape, shared_v=vh != heads, shared_g=False if want else None)
         att = K.attn_softmax_probs(qa, ka, heads, tape["sq_q"], tape["sq_k"]) if want_attn else None
-        ctx.state = (tape, q.dtype, k.dtype, v.dtype, heads, vh, m, d, prec) if _want_tape(ctx) else None
+        ctx.state = (tape, q.dtype, k.dtype, v.dtype, heads, vh, m, d, prec) if want else None
         out = _from_act(o, q.dtype).reshape(n, heads, d)
         if att is not None:
             ctx.mark_non_differentiable(att)
@@ -313,10 +315,8 @@ class ScaledAttentionFn(_TapeFunction):
         if k.shape != q.shape or v.shape[0] != n or mp != E.gat_attn_pad(dk, prec):
             raise ValueError(f"GATAttention: q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} do not hold {heads} heads of "
                              f"key width {dk} padded to {E.gat_attn_pad(dk, prec)}")
-        if not K.attn_softmax_fits(heads, mp, d, prec.act_dtype, False):
-            raise ValueError(f"sgformer_b200: GAT attention with {heads} heads of key width {dk} and value width {d} in precision "
-                             f"'{prec.name}' is not supported: the heads' columns of one q row and of one v row, each padded to 16, "
-                             f"must take at most {K.ATTN_SOFTMAX_MAX_ROW_BYTES} bytes")
+        E.check_attn_softmax(f"GAT attention with {heads} heads of key width {dk} and value width {d}", heads, mp, d, prec, False,
+                             False if _want_tape(ctx) else None)
         qa, ka, va = (_to_act(t, prec) for t in (q, k, v))
         scale = E.gat_attn_scale(dk)
         o = K.attn_scaled_fwd(qa, ka, va, heads, scale)

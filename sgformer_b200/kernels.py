@@ -1021,11 +1021,22 @@ def _heads_fit(x: Tensor, heads: int, d: int, name: str):
 ATTN_SOFTMAX_MAX_ROW_BYTES = 1024     # SGF_ATTN_SOFTMAX_MAX_ROW_BYTES
 
 
-def attn_softmax_fits(heads: int, m: int, d: int, dtype, shared_v: bool) -> bool:
-    """Whether the heads' 16-element-padded blocks of a q row and of a v row fit the kernels' shared-memory tiles."""
-    es = 2 if dtype == torch.bfloat16 else 4
-    return heads * ceil_to(m, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES and \
-        (1 if shared_v else heads) * ceil_to(d, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES
+def attn_softmax_tile_rows(heads: int, m: int, d: int, dtype, shared_v: bool, shared_g: bool) -> Optional[Tuple[int, int, int]]:
+    """(fwd, bwd_q, bwd_kv): the height of the streamed tile each launch picks for this shape, 0 where none fits in shared
+    memory (shared_g: the backward's gradient is one [N, D] block for every head).  None for widths the kernels refuse: not
+    multiples of 16 bytes, or past ATTN_SOFTMAX_MAX_ROW_BYTES.  Host-only: needs no GPU."""
+    rows = (C.c_int32 * 3)()
+    rc = lib().sgf_attn_softmax_tile_rows(heads, m, d, 1 if dtype == torch.bfloat16 else 0, int(shared_v), int(shared_g), rows)
+    if rc == -2:        # SGF_ERR_UNSUPPORTED
+        return None
+    check(rc, "sgf_attn_softmax_tile_rows")
+    return tuple(rows)
+
+
+def attn_softmax_fits(heads: int, m: int, d: int, dtype, shared_v: bool, shared_g: bool) -> bool:
+    """Whether the forward and both backward sweeps run this shape: widths the kernels take, and a streamed tile for each."""
+    rows = attn_softmax_tile_rows(heads, m, d, dtype, shared_v, shared_g)
+    return rows is not None and 0 not in rows
 
 
 def _softmax_args(q: Tensor, k: Tensor, v: Tensor, heads: int, sq_q: Optional[Tensor], sq_k: Optional[Tensor], shared_v: bool,

@@ -2,21 +2,14 @@
 tests/kernel_emu.py, in both modes: the Frobenius-normalised scores of SGFormerSOFT (attn_softmax_*) and the scaled scores of
 SGFormerGAT (attn_scaled_*).  `module()` is kernel_emu plus these entry points, for running the TransConv schedule with
 trans_attention="softmax" / "gat" (engine.trans_forward / trans_backward) without a GPU.  The softmax runs over the heads of each
-(node, key) pair; the backward is the exact derivative of the forward (autograd in the working precision)."""
+(node, key) pair; the backward is the exact derivative of the forward (autograd in the working precision).  Which shapes the
+kernels take is not emulated: the engine asks the library's host-only query (kernels.attn_softmax_tile_rows) directly."""
 import types
 
 import torch
 
 import kernel_emu
-from kernel_emu import _f, _st, alloc_act, ceil_to
-
-ATTN_SOFTMAX_MAX_ROW_BYTES = 1024
-
-
-def attn_softmax_fits(heads, m, d, dtype, shared_v):
-    es = 2 if dtype == torch.bfloat16 else 4
-    return heads * ceil_to(m, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES and \
-        (1 if shared_v else heads) * ceil_to(d, 16) * es <= ATTN_SOFTMAX_MAX_ROW_BYTES
+from kernel_emu import _f, _st, alloc_act
 
 
 def _attend(q, k, v, heads, shared_v, scale):
@@ -76,7 +69,7 @@ def attn_scaled_bwd(q, k, v, heads, scale, g, gscale, dq, dk, dv, dv_accumulate=
 def module():
     m = types.ModuleType("kernel_emu_attn_softmax")
     m.__dict__.update(kernel_emu.__dict__)
-    for name in ("ATTN_SOFTMAX_MAX_ROW_BYTES", "attn_softmax_fits", "attn_softmax_fwd", "attn_softmax_bwd", "attn_softmax_probs",
+    for name in ("attn_softmax_fwd", "attn_softmax_bwd", "attn_softmax_probs",
                  "attn_scaled_fwd", "attn_scaled_bwd"):
         setattr(m, name, globals()[name])
     return m

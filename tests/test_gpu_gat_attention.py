@@ -36,8 +36,10 @@ def _check(name, x, ref, tol, scale, exact_zero=True):
     assert err <= tol, f"{name}: relative error {err:.3g}"
 
 
-def _kernel_case(n, heads, dk, d, prec_name, smax, seed=0):
-    """q, k in the kernels' layout (each head's dk columns padded with zeros to 16 bytes), scaled so that max |s| = smax."""
+def _kernel_case(n, heads, dk, d, prec_name, smax, seed=0, per_head_g=False, accumulate=False):
+    """q, k in the kernels' layout (each head's dk columns padded with zeros to 16 bytes), scaled so that max |s| = smax.
+    per_head_g: a gradient block per head (ScaledAttentionFn's) instead of the head mean's shared one.  accumulate: dv starts
+    from random values and the backward adds to them."""
     prec = E.precision(prec_name)
     dt = prec.act_dtype
     mp = E.gat_attn_pad(dk, prec)
@@ -51,21 +53,25 @@ def _kernel_case(n, heads, dk, d, prec_name, smax, seed=0):
     q[:, :, :dk], k[:, :, :dk] = q0.to(dt), k0.to(dt)
     q, k = q.reshape(n, heads * mp), k.reshape(n, heads * mp)
     v = torch.randn(n, heads * d, device="cuda", generator=g).to(dt)
-    gr = torch.randn(n, d, device="cuda", generator=g).to(dt)          # the head mean's gradient: one block for every head
+    gr = torch.randn(n, (heads if per_head_g else 1) * d, device="cuda", generator=g).to(dt)     # shared: the head mean's
     o = K.attn_scaled_fwd(q, k, v, heads, scale)
     dq, dkk = K.alloc_act(n, heads * mp, dt, "cuda"), K.alloc_act(n, heads * mp, dt, "cuda")
     dv = K.alloc_act(n, heads * d, dt, "cuda")
-    K.attn_scaled_bwd(q, k, v, heads, scale, gr, 1.0 / heads, dq, dkk, dv)
+    if accumulate:
+        dv.copy_(torch.randn(n, heads * d, device="cuda", generator=g) * 2)
+    dv0 = dv.double() if accumulate else 0.0
+    K.attn_scaled_bwd(q, k, v, heads, scale, gr, 1.0 if per_head_g else 1.0 / heads, dq, dkk, dv, dv_accumulate=accumulate)
     qr, kr = (t.double().reshape(n, heads, mp)[:, :, :dk].clone().requires_grad_() for t in (q, k))
     vr = v.double().reshape(n, heads, d).requires_grad_()
     ref = O.gat_attention(qr, kr, vr)
-    ref.backward(gr.double()[:, None, :].expand(n, heads, d) / heads)
+    gd = gr.double().reshape(n, -1, d).expand(n, heads, d)
+    ref.backward(gd if per_head_g else gd / heads)
     torch.cuda.synchronize()
     unpad = lambda t: t.reshape(n, heads, mp)[:, :, :dk].reshape(n, -1)      # noqa: E731
     pads = lambda t: t.reshape(n, heads, mp)[:, :, dk:]                       # noqa: E731
     assert torch.count_nonzero(pads(dq)) == 0 and torch.count_nonzero(pads(dkk)) == 0
     return {"o": (o, ref.detach().reshape(n, -1)), "dq": (unpad(dq), qr.grad.reshape(n, -1)),
-            "dk": (unpad(dkk), kr.grad.reshape(n, -1)), "dv": (dv, vr.grad.reshape(n, -1))}
+            "dk": (unpad(dkk), kr.grad.reshape(n, -1)), "dv": (dv, dv0 + vr.grad.reshape(n, -1))}
 
 
 def _check_case(res, tol, heads):

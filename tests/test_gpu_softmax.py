@@ -33,10 +33,11 @@ def _check(name, x, ref, tol, scale, exact_zero=True):
     assert err <= tol, f"{name}: relative error {err:.3g}"
 
 
-def _kernel_case(n, heads, m, shared_v, per_head_g, prec_name, seed=0):
+def _kernel_case(n, heads, m, shared_v, per_head_g, prec_name, seed=0, d=None, accumulate=False):
+    """d: v's width per head (default m).  accumulate: dv starts from random values and the backward adds to them."""
     prec = E.precision(prec_name)
     g = torch.Generator(device="cuda").manual_seed(seed)
-    d = m
+    d = m if d is None else d
     dt = prec.act_dtype
     q = (torch.randn(n, heads * m, device="cuda", generator=g) * 2 + 0.5).to(dt)
     k = (torch.randn(n, heads * m, device="cuda", generator=g) - 0.3).to(dt)
@@ -44,17 +45,20 @@ def _kernel_case(n, heads, m, shared_v, per_head_g, prec_name, seed=0):
     gr = torch.randn(n, (heads if per_head_g else 1) * d, device="cuda", generator=g).to(dt)
     gscale = 1.0 if per_head_g else 1.0 / heads
     tape = E.Tape()
-    o = E.attention_softmax_forward(q, k, v, heads, prec, tape, shared_v=shared_v)
+    o = E.attention_softmax_forward(q, k, v, heads, prec, tape, shared_v=shared_v, shared_g=not per_head_g and heads > 1)
     dq, dk = K.alloc_act(n, heads * m, dt, "cuda"), K.alloc_act(n, heads * m, dt, "cuda")
     dv = K.alloc_act(n, v.shape[1], dt, "cuda")
-    E.attention_softmax_backward(tape, gr, gscale, dq, dk, dv)
+    if accumulate:
+        dv.copy_(torch.randn(n, v.shape[1], device="cuda", generator=g) * 2)
+    dv0 = dv.double() if accumulate else 0.0
+    E.attention_softmax_backward(tape, gr, gscale, dq, dk, dv, dv_accumulate=accumulate)
     qr, kr = (t.double().reshape(n, heads, m).requires_grad_() for t in (q, k))
     vr = v.double().reshape(n, -1, d).requires_grad_()
     ref, _ = O.softmax_attention(qr, kr, vr)
     ref.backward(gr.double().reshape(n, -1, d).expand(n, heads, d) * gscale)
     torch.cuda.synchronize()
     return {"o": (o, ref.detach().reshape(n, -1)), "dq": (dq, qr.grad.reshape(n, -1)), "dk": (dk, kr.grad.reshape(n, -1)),
-            "dv": (dv, vr.grad.reshape(n, -1))}
+            "dv": (dv, dv0 + vr.grad.reshape(n, -1))}
 
 
 def _check_case(res, tol):
