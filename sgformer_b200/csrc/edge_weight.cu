@@ -9,6 +9,8 @@
 // gcn_conv normalises by the unweighted degree: no degree term (y = u = NULL).
 //
 // One warp per row; a row's operand a_c stays in registers while the warp walks the row's entries, gathering b_r like the SpMM.
+// A lane holds 2 KB / 32 of a_c: 16 fp32 or 32 bf16 values, so rows up to 512 fp32 / 1024 bf16 features (the widths the layers
+// admit, engine.check_width).
 // Every non-loop edge is one CSR entry, so `out[eid]` is written by one thread of one launch: no atomics, deterministic.  The added
 // self loop of a self_loop_mode 1 row has no edge of its own; its gradient goes to loop_grad[c], and a second pass adds it to every
 // existing self loop (c, c) of node c (autograd of PyG's `loop_attr[idx] = attr`, which scatters into all of them).
@@ -18,7 +20,8 @@
 
 namespace sgf {
 
-constexpr int kEdgeGradMaxPerLane = 16;     // h <= 512
+template <typename T>
+constexpr int kEdgeGradMaxPerLane = 2048 / 32 / (int)sizeof(T);     // h <= 512 (fp32) / 1024 (bf16)
 
 template <typename T>
 __global__ void __launch_bounds__(256) edge_weight_grad_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col,
@@ -31,17 +34,18 @@ __global__ void __launch_bounds__(256) edge_weight_grad_kernel(const int64_t* __
     const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t c = warp0; c < n_rows; c += nwarps) {
-        float ac[kEdgeGradMaxPerLane];
+        constexpr int kPerLane = kEdgeGradMaxPerLane<T>;
+        float ac[kPerLane];
         float q = 0.f;
 #pragma unroll
-        for (int k = 0; k < kEdgeGradMaxPerLane; ++k) {
+        for (int k = 0; k < kPerLane; ++k) {
             const int f = lane + 32 * k;
             ac[k] = f < h ? to_f32(a[c * lda + f]) : 0.f;
         }
         if (y) {
             float d = 0.f;
 #pragma unroll
-            for (int k = 0; k < kEdgeGradMaxPerLane; ++k) {
+            for (int k = 0; k < kPerLane; ++k) {
                 const int f = lane + 32 * k;
                 if (f < h) d += ac[k] * to_f32(y[c * ldy + f]) + to_f32(b[c * ldb + f]) * to_f32(u[c * ldu + f]);
             }
@@ -52,7 +56,7 @@ __global__ void __launch_bounds__(256) edge_weight_grad_kernel(const int64_t* __
             const T* br = b + r * ldb;
             float d = 0.f;
 #pragma unroll
-            for (int k = 0; k < kEdgeGradMaxPerLane; ++k) {
+            for (int k = 0; k < kPerLane; ++k) {
                 const int f = lane + 32 * k;
                 if (f < h) d += ac[k] * to_f32(br[f]);
             }
@@ -98,7 +102,8 @@ extern "C" int sgf_edge_weight_grad(const int64_t* rowptr, const int32_t* col, c
                                     const void* a, int64_t lda, const void* b, int64_t ldb, const void* y, int64_t ldy, const void* u,
                                     int64_t ldu, const float* dinv, const int64_t* edge_index, int64_t nnz, float* loop_grad,
                                     float* out, void* stream) {
-    if (!rowptr || n_rows < 0 || h <= 0 || h > 32 * sgf::kEdgeGradMaxPerLane || nnz < 0 || (nnz > 0 && !out)) return SGF_ERR_ARG;
+    if (!rowptr || n_rows < 0 || h <= 0 || nnz < 0 || (nnz > 0 && !out)) return SGF_ERR_ARG;
+    if (h > 32 * (dtype == 1 ? sgf::kEdgeGradMaxPerLane<__nv_bfloat16> : sgf::kEdgeGradMaxPerLane<float>)) return SGF_ERR_ARG;
     if (n_rows > 0 && (!col || !eid || !a || !b)) return SGF_ERR_ARG;
     if (y && (!u || !dinv)) return SGF_ERR_ARG;
     if (loop_grad && nnz > 0 && !edge_index) return SGF_ERR_ARG;

@@ -37,12 +37,7 @@ constexpr int kSpmmBlock = 256;
 #ifndef SGF_SPMM_MIN_BLOCKS
 #define SGF_SPMM_MIN_BLOCKS 4
 #endif
-// Tuning knobs (scripts/bench_spmm.py times the variants): rows in flight per lane group x CTAs per SM, and software-pipelining
-// the rowptr -> column-id -> feature-row chain across a warp's rows (SGF_SPMM_PIPELINE=1).  Once the gather saturates the memory
-// system extra memory-level parallelism buys nothing, so the simple loop is the default.
-#ifndef SGF_SPMM_PIPELINE
-#define SGF_SPMM_PIPELINE 0
-#endif
+// Tuning knobs (scripts/bench_spmm.py times the variants): rows in flight per lane group x CTAs per SM.
 constexpr int kUnroll = SGF_SPMM_UNROLL;
 constexpr int kMinBlocks = SGF_SPMM_MIN_BLOCKS;
 
@@ -157,9 +152,7 @@ __device__ __forceinline__ void gather_range_flagged(const int32_t* __restrict__
 }
 
 // One warp per output row, rows r = warp, warp + nwarps, ...; rows longer than max_len (> 0) are left to the segmented path
-// below.  SGF_SPMM_PIPELINE=1 software-pipelines the dependent chain rowptr -> column ids -> feature rows across the warp's work
-// items (an item = up to 32 neighbours of one row): while the gathers of item i are in flight, the column ids of item i+1 (same
-// row or the warp's next row) and the rowptr entries of the row after next are already loading (off by default, see above).
+// below.
 // Row range of a phased SpMM (row-sharded runs, dist.Comm._spmm_phased): the launch handles entries [lo[r], hi[r]) of every row r
 // (offsets relative to the row start; null = row start / row end), starts from the fp32 partial sums of the previous phases
 // (part_in, nullable) and either hands fp32 partials on (part_out) or scales and stores the finished row.
@@ -262,74 +255,6 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
         cval[c] = ch < chunks;
         coff[c] = ch * VN;
     }
-#if SGF_SPMM_PIPELINE
-    static_assert(!FLAGS && !WEIGHTED, "the flagged and weighted variants use the simple loop");
-    int64_t r = warp0;
-    if (r >= n_rows) return;
-    // current row [s, e) (a skipped hub row behaves like an empty row that is not stored), next row [sn, en)
-    int64_t s = rowptr[r], e = rowptr[r + 1];
-    bool skip = max_len > 0 && e - s > max_len;
-    if (skip) e = s;
-    int64_t rn = r + nwarps, sn = 0, en = 0;
-    if (rn < n_rows) { sn = rowptr[rn]; en = rowptr[rn + 1]; }
-    int64_t base = s;
-    int idx = (base + lane < e) ? ldg_nc_na_s32(col + base + lane) : -1;
-    float acc[CPL][VN];
-#pragma unroll
-    for (int c = 0; c < CPL; ++c)
-#pragma unroll
-        for (int i = 0; i < VN; ++i) acc[c][i] = 0.f;
-    while (true) {
-        const int cnt = (int)((e - base) < 32 ? (e - base) : 32);      // 0 for an empty row
-        const bool last = base + 32 >= e;                               // last item of this row
-        // ---- put the next item's column ids (and, at a row end, the rowptr pair of the row after next) in flight ----
-        int64_t nbase, ne;
-        bool nskip = false;
-        int64_t rnn = rn, snn = 0, enn = 0;
-        if (!last) { nbase = base + 32; ne = e; }
-        else {
-            nskip = max_len > 0 && en - sn > max_len;
-            nbase = sn; ne = nskip ? sn : en;
-            rnn = rn + nwarps;
-            if (rnn < n_rows) { snn = rowptr[rnn]; enn = rowptr[rnn + 1]; }
-        }
-        const bool have_next = !last || rn < n_rows;
-        const int nidx = (have_next && nbase + lane < ne) ? ldg_nc_na_s32(col + nbase + lane) : -1;
-        // ---- this item ----
-        gather_item<T, CPL>(idx, cnt, x, ldx, groups, grp, coff, cval, acc);
-        if (last) {
-            if (!skip) {
-                for (int o = lpr; o < 32; o <<= 1) {
-#pragma unroll
-                    for (int c = 0; c < CPL; ++c)
-#pragma unroll
-                        for (int i = 0; i < VN; ++i) acc[c][i] += __shfl_xor_sync(0xffffffffu, acc[c][i], o);
-                }
-                const float rs = (SCALED && row_scale) ? row_scale[r] : 1.0f;
-                if (grp == 0) {
-                    T* dst = y + r * ldy;
-#pragma unroll
-                    for (int c = 0; c < CPL; ++c) {
-                        if (!cval[c]) continue;
-                        float f[VN];
-#pragma unroll
-                        for (int i = 0; i < VN; ++i) f[i] = SCALED ? acc[c][i] * rs : acc[c][i];
-                        stg_na(dst + coff[c], Vec16<T>::pack(f));
-                    }
-                }
-            }
-            if (rn >= n_rows) break;
-            r = rn; s = sn; e = ne; skip = nskip;
-            rn = rnn; sn = snn; en = enn;
-#pragma unroll
-            for (int c = 0; c < CPL; ++c)
-#pragma unroll
-                for (int i = 0; i < VN; ++i) acc[c][i] = 0.f;
-        }
-        base = nbase;
-        idx = nidx;
-    }
-#else
     for (int64_t r = warp0; r < n_rows; r += nwarps) {
         const int64_t s = rowptr[r];
         const int64_t e = rowptr[r + 1];
@@ -360,7 +285,6 @@ spmm_rows_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__
             }
         }
     }
-#endif
 }
 
 // hub rows (power-law graphs): a row longer than the threshold is cut into segments, one warp per segment writes an fp32
@@ -519,6 +443,7 @@ static int launch_heavy(const int32_t* col, const float* row_scale, const void* 
                         const float* val = nullptr) {
     constexpr int VN = Vec16<T>::N;
     if (h % VN != 0 || ldx % VN != 0) return SGF_ERR_ARG;
+    if (reinterpret_cast<uintptr_t>(x) & 15) return SGF_ERR_ARG;        // the segment kernel gathers x in 16-byte loads
     const int chunks = h / VN;
     int lpr_log2 = 0;
     while ((1 << lpr_log2) < chunks && lpr_log2 < 5) ++lpr_log2;
