@@ -140,6 +140,16 @@ int sgf_csr_subset_ws_bytes(int64_t n_sub, int64_t max_out_nnz, size_t* bytes);
 int sgf_csr_subset(const int64_t* rowptr, const int32_t* col, int64_t n, const int64_t* subset, int64_t n_sub,
                    int32_t* node_map, int64_t* out_rowptr /* [n_sub+1] */, int32_t* out_col, int64_t out_col_capacity,
                    float* dinv /* [n_sub] or NULL */, int64_t* out_needed, void* ws, size_t ws_bytes, void* stream);
+/* sgf_csr_subset of a directed graph: the subset of the forward CSR (rowptr, col; rows = edge targets) as above, and the subset of
+ * its transpose (rowptr_t, col_t of sgf_csr_build by_source = 1; rows = edge sources) into out_rowptr_t / out_col_t, both with
+ * the local ids of one fill of node_map.  The transposed half equals sgf_csr_build(by_source = 1) of the subset's edge list and
+ * has no dinv.  Each half has out_col_capacity entries, is clamped on its own and reports its own induced nnz (out_needed,
+ * out_needed_t; nullable).  ws sized by sgf_csr_subset_ws_bytes(n_sub, out_col_capacity), reused by the two halves in turn. */
+int sgf_csr_subset_pair(const int64_t* rowptr, const int32_t* col, const int64_t* rowptr_t, const int32_t* col_t, int64_t n,
+                        const int64_t* subset, int64_t n_sub, int32_t* node_map, int64_t* out_rowptr /* [n_sub+1] */,
+                        int32_t* out_col, int64_t* out_rowptr_t /* [n_sub+1] */, int32_t* out_col_t, int64_t out_col_capacity,
+                        float* dinv /* [n_sub] or NULL */, int64_t* out_needed, int64_t* out_needed_t, void* ws, size_t ws_bytes,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K6 / K7 — CSR SpMM (replaces torch_sparse.matmul(adj, x), large/ours.py:34, 100M/ours.py:80, and its

@@ -174,6 +174,8 @@ _SIGS = {
     "sgf_pack_operand": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, _vp, _i64, C.c_int, _i64, _vp, _vp, _vp, _sz, _vp]),
     "sgf_csr_subset_ws_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
     "sgf_csr_subset": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "sgf_csr_subset_pair": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz,
+                                      _vp]),
     "sgf_eval_acc": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, C.c_int, _vp, _vp, _vp]),
     "sgf_softmax_nll": (C.c_int, [_vp, _i64, _vp, _vp, _i64, C.c_int, _f32, _vp, _vp, _i64, _vp, _sz, _vp]),
     "sgf_head_mean": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, C.c_int, _vp, _i64, _vp]),

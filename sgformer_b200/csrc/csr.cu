@@ -908,23 +908,12 @@ extern "C" int sgf_csr_subset_ws_bytes(int64_t n_sub, int64_t max_out_nnz, size_
     return SGF_OK;
 }
 
-extern "C" int sgf_csr_subset(const int64_t* rowptr, const int32_t* col, int64_t n, const int64_t* subset, int64_t n_sub,
-                              int32_t* node_map, int64_t* out_rowptr, int32_t* out_col, int64_t out_col_capacity, float* dinv,
-                              int64_t* out_needed, void* ws, size_t ws_bytes, void* stream) {
-    if (!rowptr || n < 0 || n_sub < 0 || !node_map || !out_rowptr || !ws || (n_sub > 0 && !subset) || out_col_capacity < 0)
-        return SGF_ERR_ARG;
-    CsrWs w = carve_ws(ws, out_col_capacity, n_sub);
-    if (ws_bytes < w.bytes) return SGF_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n_sub == 0) {
-        SGF_CUDA_TRY(cudaMemsetAsync(out_rowptr, 0, 8, st));
-        if (out_needed) SGF_CUDA_TRY(cudaMemsetAsync(out_needed, 0, 8, st));
-        return SGF_OK;
-    }
+// One orientation of the subset: rows of (rowptr, col) at `subset`, columns through the already-filled node_map.  The halves of
+// sgf_csr_subset_pair run one after the other on the stream and share the workspace.
+static int subset_half(const int64_t* rowptr, const int32_t* col, int64_t n, const int64_t* subset, int64_t n_sub,
+                       const int32_t* node_map, int64_t* out_rowptr, int32_t* out_col, int64_t out_col_capacity, float* dinv,
+                       int64_t* out_needed, const CsrWs& w, cudaStream_t st) {
     SGF_CUDA_TRY(cudaMemsetAsync(w.total, 0, 64, st));
-    // node_map holds -1 everywhere on entry (maintained by the caller across batches) and is restored on exit
-    subgraph_map_kernel<<<grid_for(n_sub, 256), 256, 0, st>>>(subset, n_sub, n, node_map);
-    SGF_LAUNCH_CHECK(); count_launch();
     subset_count_kernel<<<grid_for(n_sub * 32, 256), 256, 0, st>>>(rowptr, col, subset, n_sub, n, node_map, w.counts);
     SGF_LAUNCH_CHECK(); count_launch();
     int rc = launch_scan(w.counts, n_sub, 0, out_rowptr, w.block_sums, w.total, w.cursor, st);
@@ -933,21 +922,62 @@ extern "C" int sgf_csr_subset(const int64_t* rowptr, const int32_t* col, int64_t
     SGF_LAUNCH_CHECK(); count_launch();
     subset_fill_kernel<<<grid_for(n_sub * 32, 256), 256, 0, st>>>(rowptr, col, subset, n_sub, n, node_map, out_rowptr, out_col);
     SGF_LAUNCH_CHECK(); count_launch();
-    subset_unmap_kernel<<<grid_for(n_sub, 256), 256, 0, st>>>(subset, n_sub, n, node_map);
-    SGF_LAUNCH_CHECK(); count_launch();
     // local ids are a permutation of the global ones: restore sorted rows (canonical CSR)
-    csr_sort_rows_warp_kernel<<<grid_for(n_sub * 32, 256), 256, 0, st>>>(out_rowptr, n_sub, out_col, w.long_rows, w.n_long);
-    SGF_LAUNCH_CHECK(); count_launch();
-    int64_t share = w.scratch_elems / kHubBlocks;
-    csr_sort_rows_block_kernel<<<num_sms() * 4, 256, 0, st>>>(out_rowptr, out_col, w.long_rows, w.n_long, w.scratch, 0, 0, kSortSmemMax);
-    SGF_LAUNCH_CHECK(); count_launch();
-    csr_sort_rows_block_kernel<<<kHubBlocks, 1024, 0, st>>>(out_rowptr, out_col, w.long_rows, w.n_long, w.scratch, share, kSortSmemMax, share);
-    SGF_LAUNCH_CHECK(); count_launch();
+    rc = sort_rows(out_rowptr, out_col, n_sub, w, st);
+    if (rc) return rc;
     if (dinv) {
         csr_dinv_kernel<<<grid_for(n_sub, 256), 256, 0, st>>>(out_rowptr, n_sub, dinv);
         SGF_LAUNCH_CHECK(); count_launch();
     }
     return SGF_OK;
+}
+
+// node_map holds -1 everywhere on entry (maintained by the caller across batches), is filled once for both halves and is
+// restored on exit.  rowptr_t == NULL: the forward half only.
+static int csr_subset(const int64_t* rowptr, const int32_t* col, const int64_t* rowptr_t, const int32_t* col_t, int64_t n,
+                      const int64_t* subset, int64_t n_sub, int32_t* node_map, int64_t* out_rowptr, int32_t* out_col,
+                      int64_t* out_rowptr_t, int32_t* out_col_t, int64_t out_col_capacity, float* dinv, int64_t* out_needed,
+                      int64_t* out_needed_t, void* ws, size_t ws_bytes, void* stream) {
+    if (!rowptr || n < 0 || n_sub < 0 || !node_map || !out_rowptr || !ws || (n_sub > 0 && !subset) || out_col_capacity < 0)
+        return SGF_ERR_ARG;
+    if (rowptr_t && !out_rowptr_t) return SGF_ERR_ARG;
+    CsrWs w = carve_ws(ws, out_col_capacity, n_sub);
+    if (ws_bytes < w.bytes) return SGF_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_sub == 0) {
+        SGF_CUDA_TRY(cudaMemsetAsync(out_rowptr, 0, 8, st));
+        if (out_needed) SGF_CUDA_TRY(cudaMemsetAsync(out_needed, 0, 8, st));
+        if (rowptr_t) SGF_CUDA_TRY(cudaMemsetAsync(out_rowptr_t, 0, 8, st));
+        if (rowptr_t && out_needed_t) SGF_CUDA_TRY(cudaMemsetAsync(out_needed_t, 0, 8, st));
+        return SGF_OK;
+    }
+    subgraph_map_kernel<<<grid_for(n_sub, 256), 256, 0, st>>>(subset, n_sub, n, node_map);
+    SGF_LAUNCH_CHECK(); count_launch();
+    int rc = subset_half(rowptr, col, n, subset, n_sub, node_map, out_rowptr, out_col, out_col_capacity, dinv, out_needed, w, st);
+    if (!rc && rowptr_t)
+        rc = subset_half(rowptr_t, col_t, n, subset, n_sub, node_map, out_rowptr_t, out_col_t, out_col_capacity, nullptr,
+                         out_needed_t, w, st);
+    if (rc) return rc;
+    subset_unmap_kernel<<<grid_for(n_sub, 256), 256, 0, st>>>(subset, n_sub, n, node_map);
+    SGF_LAUNCH_CHECK(); count_launch();
+    return SGF_OK;
+}
+
+extern "C" int sgf_csr_subset(const int64_t* rowptr, const int32_t* col, int64_t n, const int64_t* subset, int64_t n_sub,
+                              int32_t* node_map, int64_t* out_rowptr, int32_t* out_col, int64_t out_col_capacity, float* dinv,
+                              int64_t* out_needed, void* ws, size_t ws_bytes, void* stream) {
+    return csr_subset(rowptr, col, nullptr, nullptr, n, subset, n_sub, node_map, out_rowptr, out_col, nullptr, nullptr,
+                      out_col_capacity, dinv, out_needed, nullptr, ws, ws_bytes, stream);
+}
+
+extern "C" int sgf_csr_subset_pair(const int64_t* rowptr, const int32_t* col, const int64_t* rowptr_t, const int32_t* col_t,
+                                   int64_t n, const int64_t* subset, int64_t n_sub, int32_t* node_map, int64_t* out_rowptr,
+                                   int32_t* out_col, int64_t* out_rowptr_t, int32_t* out_col_t, int64_t out_col_capacity,
+                                   float* dinv, int64_t* out_needed, int64_t* out_needed_t, void* ws, size_t ws_bytes,
+                                   void* stream) {
+    if (!rowptr_t) return SGF_ERR_ARG;
+    return csr_subset(rowptr, col, rowptr_t, col_t, n, subset, n_sub, node_map, out_rowptr, out_col, out_rowptr_t, out_col_t,
+                      out_col_capacity, dinv, out_needed, out_needed_t, ws, ws_bytes, stream);
 }
 
 // ---- K10 host side ---------------------------------------------------------------------------------------------------------

@@ -70,7 +70,9 @@ class Graph:
     def subset(self, idx: Tensor, capacity: Optional[int] = None) -> "Graph":
         """Induced subgraph of the nodes `idx` (int64, local id = position in idx), built from this CSR in
         O(sum of the selected rows' lengths) — the mini-batch structure of large/main-batch.py:136-139 without the per-batch
-        O(E) PyG `subgraph` mask and without a CSR rebuild.  Requires a symmetric edge set for the backward (checked once)."""
+        O(E) PyG `subgraph` mask and without a CSR rebuild.  On a symmetric edge set (checked once per graph) the subset's
+        transpose shares its storage; on a directed one the subset of the transposed CSR is built beside it on the same local
+        ids (`nnz_needed_t` is its induced nnz)."""
         if self.rows is not None:
             raise ValueError("subset() needs the full (unsharded) graph")
         if self.val is not None:
@@ -78,10 +80,15 @@ class Graph:
         if not hasattr(self, "_node_map"):
             self._node_map = torch.full((max(self.n, 1),), -1, dtype=torch.int32, device=self.rowptr.device)
             self._symmetric = self.transpose()[0] is self.rowptr
-            if not self._symmetric:
-                raise NotImplementedError("Graph.subset: directed graphs need the transposed subset as well")
-        rp, cl, dv, needed = K.csr_subset(self.rowptr, self.col, self.n, idx, self._node_map, capacity)
-        g = Graph._from_parts(idx.numel(), rp, cl, dv, True)
+        if self._symmetric:
+            rp, cl, dv, needed = K.csr_subset(self.rowptr, self.col, self.n, idx, self._node_map, capacity)
+            g = Graph._from_parts(idx.numel(), rp, cl, dv, True)
+            g.nnz_needed_t = needed
+        else:
+            rp, cl, dv, needed, rp_t, cl_t, needed_t = K.csr_subset(self.rowptr, self.col, self.n, idx, self._node_map, capacity,
+                                                                    transposed=self._t)
+            g = Graph._from_parts(idx.numel(), rp, cl, dv, False)
+            g._t, g.nnz_needed_t = (rp_t, cl_t), needed_t
         g.nnz_needed, g.capacity = needed, capacity      # device int64 [1]: > capacity means the batch structure was truncated
         return g
 

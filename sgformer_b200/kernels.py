@@ -273,18 +273,27 @@ def add_self_loops(edge_index: Tensor, n: int) -> Tensor:
 spmm_events = None
 
 
-def csr_subset(rowptr: Tensor, col: Tensor, n: int, subset: Tensor, node_map: Tensor, capacity: Optional[int] = None):
+def csr_subset(rowptr: Tensor, col: Tensor, n: int, subset: Tensor, node_map: Tensor, capacity: Optional[int] = None,
+               transposed: Optional[Tuple[Tensor, Tensor]] = None):
     """Induced-subgraph CSR of `subset` from the full CSR.  -> (rowptr int64 [b+1], col int32 [nnz_b], dinv fp32 [b], needed).
     `capacity` bounds the output nnz (default: a device sync to read the exact sum of the subset rows' lengths); the kernels
     never write past it, and `needed` (device int64 [1]) holds the nnz the untruncated result requires: needed > capacity
-    means the batch was truncated (checked without a per-batch sync by RandomPartitionSampler.check)."""
+    means the batch was truncated (checked without a per-batch sync by RandomPartitionSampler.check).
+    `transposed=(rowptr_t, col_t)`, the transposed CSR of a directed graph: its subset as well, on the same node map and local
+    ids (sgf_csr_subset_pair); -> (rowptr, col, dinv, needed, rowptr_t, col_t, needed_t), each half bounded by `capacity`."""
     _use(rowptr)
     subset = subset.contiguous().to(torch.int64)
     b = subset.numel()
     dev = rowptr.device
+    rowptr_t, col_t = transposed if transposed is not None else (None, None)
     trim = capacity is None
     if capacity is None:
-        capacity = int((rowptr[subset + 1] - rowptr[subset]).sum().item()) if b else 0
+        capacity = 0
+        if b:
+            bound = (rowptr[subset + 1] - rowptr[subset]).sum()
+            if rowptr_t is not None:    # both halves hold the same induced edges, so either row-length sum bounds both
+                bound = torch.minimum(bound, (rowptr_t[subset + 1] - rowptr_t[subset]).sum())
+            capacity = int(bound.item())
     out_rowptr = torch.empty(b + 1, dtype=torch.int64, device=dev)
     out_col = torch.empty(max(capacity, 1), dtype=torch.int32, device=dev)
     dinv = torch.empty(max(b, 1), dtype=torch.float32, device=dev)
@@ -292,11 +301,22 @@ def csr_subset(rowptr: Tensor, col: Tensor, n: int, subset: Tensor, node_map: Te
     nbytes = C.c_size_t(0)
     check(lib().sgf_csr_subset_ws_bytes(b, capacity, C.byref(nbytes)), "sgf_csr_subset_ws_bytes")
     ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
-    check(lib().sgf_csr_subset(_p(rowptr), _p(col), n, _p(subset), b, _p(node_map), _p(out_rowptr), _p(out_col), capacity,
-                               _p(dinv), _p(needed), _p(ws), nbytes.value, _stream()), "sgf_csr_subset")
-    if trim:    # exact-size result (one more device sync); with a caller-provided capacity the tail of `col` is unused
-        out_col = out_col[:int(out_rowptr[b].item())]
-    return out_rowptr, out_col, dinv[:b], needed
+    if rowptr_t is None:
+        check(lib().sgf_csr_subset(_p(rowptr), _p(col), n, _p(subset), b, _p(node_map), _p(out_rowptr), _p(out_col), capacity,
+                                   _p(dinv), _p(needed), _p(ws), nbytes.value, _stream()), "sgf_csr_subset")
+        if trim:    # exact-size result (one more device sync); with a caller-provided capacity the tail of `col` is unused
+            out_col = out_col[:int(out_rowptr[b].item())]
+        return out_rowptr, out_col, dinv[:b], needed
+    out_rowptr_t = torch.empty(b + 1, dtype=torch.int64, device=dev)
+    out_col_t = torch.empty(max(capacity, 1), dtype=torch.int32, device=dev)
+    needed_t = torch.empty(1, dtype=torch.int64, device=dev)
+    check(lib().sgf_csr_subset_pair(_p(rowptr), _p(col), _p(rowptr_t), _p(col_t), n, _p(subset), b, _p(node_map), _p(out_rowptr),
+                                    _p(out_col), _p(out_rowptr_t), _p(out_col_t), capacity, _p(dinv), _p(needed), _p(needed_t),
+                                    _p(ws), nbytes.value, _stream()), "sgf_csr_subset_pair")
+    if trim:
+        nnz, nnz_t = torch.stack([out_rowptr[b], out_rowptr_t[b]]).tolist()
+        out_col, out_col_t = out_col[:nnz], out_col_t[:nnz_t]
+    return out_rowptr, out_col, dinv[:b], needed, out_rowptr_t, out_col_t, needed_t
 
 
 HEAVY_ROW = 1024      # rows longer than this are processed in segments of HEAVY_ROW entries (hub rows of power-law graphs)

@@ -41,7 +41,9 @@ class RandomPartitionSampler:
     def batch(self, idx: Tensor) -> MiniBatch:
         g = self.graph.subset(idx, self.capacity)
         if self.capacity is not None:
-            self._max_needed = g.nnz_needed.clone() if self._max_needed is None else torch.maximum(self._max_needed, g.nnz_needed)
+            # a directed graph's batch has a transposed half with its own induced nnz; a symmetric one shares it
+            needed = g.nnz_needed if g.nnz_needed_t is g.nnz_needed else torch.maximum(g.nnz_needed, g.nnz_needed_t)
+            self._max_needed = needed.clone() if self._max_needed is None else torch.maximum(self._max_needed, needed)
         return MiniBatch(idx, self.x.index_select(0, idx), g, None if self.y is None else self.y.index_select(0, idx))
 
     def __iter__(self) -> Iterator[MiniBatch]:
