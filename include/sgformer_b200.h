@@ -135,7 +135,9 @@ int sgf_edge_weight_grad(const int64_t* rowptr, const int32_t* col, const int64_
  * node_map: int32 [n] scratch that must hold -1 everywhere on entry and is restored to -1 on exit (kept across batches).
  * out_col_capacity >= sum of the subset rows' lengths is always enough.  A smaller capacity never overruns out_col: the row
  * pointers are clamped to it (the tail rows come out truncated / empty) and *out_needed (device int64, nullable) receives the
- * induced nnz the full result needs, so the caller can detect out_needed > out_col_capacity without a sync per batch. */
+ * induced nnz the full result needs, so the caller can detect out_needed > out_col_capacity without a sync per batch.
+ * Either self-loop mode: the subset of a self_loop_mode 1 CSR equals sgf_csr_build(self_loop_mode = 1) of the subset's edge list
+ * (one self loop per row, dinv of its row lengths), as the subset of a mode 0 CSR equals the mode 0 build (csr.cu, subset_half). */
 int sgf_csr_subset_ws_bytes(int64_t n_sub, int64_t max_out_nnz, size_t* bytes);
 int sgf_csr_subset(const int64_t* rowptr, const int32_t* col, int64_t n, const int64_t* subset, int64_t n_sub,
                    int32_t* node_map, int64_t* out_rowptr /* [n_sub+1] */, int32_t* out_col, int64_t out_col_capacity,
@@ -438,6 +440,18 @@ int sgf_softmax_nll(const float* logits, int64_t ld, const int64_t* labels, cons
  * (large/eval.py:28-31) for single-column int64 labels.  correct: device int64, nll_sum: device fp64 or NULL. */
 int sgf_eval_acc(const float* logits, int64_t ld, const int64_t* labels, const int64_t* idx, int64_t m, int64_t rows, int32_t c,
                  int64_t* correct, double* nll_sum, void* stream);
+/* K11 over one batch of a mini-batch evaluation (replaces the three eval_acc calls per batch of large/eval.py:67-118
+ * evaluate_batch and their three host syncs).  Row i < m of logits [m, c] (pitch ld) is node r = idx[i] (r = i when idx is
+ * NULL; then m <= rows); labels int64 [rows] and split uint8 [rows] are read at r.  split[r] holds one bit per split (1 train,
+ * 2 valid, 4 test; overlapping splits set several) and for every bit k set:  counts[2k] += 1,  counts[2k+1] += (argmax_j
+ * logits[i, j] == labels[r]), with the argmax of sgf_eval_acc: the first maximum on ties, as torch.max(dim=1), checked against
+ * the reference's eval_acc with planted ties in tests/test_gpu_kernels.py (test_eval_acc_matches_reference_semantics) for
+ * sgf_eval_acc and tests/test_gpu_eval_batch.py (test_eval_acc_splits_counts_exactly) for this entry point.  Both differ
+ * from torch.max on non-finite rows: a NaN entry never wins (torch.max returns the NaN's index), and a row of -inf only
+ * has no argmax (torch.max returns 0), so neither counts as a hit.  counts: device int64 [6], ADDED into (the caller zeroes it
+ * once per epoch).  Integer sums only: deterministic.  No allocation, no sync. */
+int sgf_eval_acc_splits(const float* logits, int64_t ld, int64_t m, int32_t c, const int64_t* labels, const uint8_t* split,
+                        const int64_t* idx, int64_t rows, int64_t* counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Linear attention glue (full_attention_conv, medium/ours.py:14-34; backward per SURVEY.md Appendix A.1)

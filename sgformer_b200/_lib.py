@@ -177,6 +177,7 @@ _SIGS = {
     "sgf_csr_subset_pair": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz,
                                       _vp]),
     "sgf_eval_acc": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, C.c_int, _vp, _vp, _vp]),
+    "sgf_eval_acc_splits": (C.c_int, [_vp, _i64, _i64, C.c_int, _vp, _vp, _vp, _i64, _vp, _vp]),
     "sgf_softmax_nll": (C.c_int, [_vp, _i64, _vp, _vp, _i64, C.c_int, _f32, _vp, _vp, _i64, _vp, _sz, _vp]),
     "sgf_head_mean": (C.c_int, [_vp, _i64, _i64, C.c_int, C.c_int, C.c_int, _vp, _i64, _vp]),
     "sgf_attn_prepare_fwd": (C.c_int, [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _i64, _vp, _i64,

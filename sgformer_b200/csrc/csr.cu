@@ -910,6 +910,15 @@ extern "C" int sgf_csr_subset_ws_bytes(int64_t n_sub, int64_t max_out_nnz, size_
 
 // One orientation of the subset: rows of (rowptr, col) at `subset`, columns through the already-filled node_map.  The halves of
 // sgf_csr_subset_pair run one after the other on the stream and share the workspace.
+//
+// The same kernels serve parents of either self-loop mode.  A self_loop_mode 1 build (either orientation) drops every self loop
+// of the edge list in the count and fill passes (duplicated loops included) and csr_add_loops_kernel then adds exactly one
+// entry (i, i) to every row; non-loop entries are kept with their duplicates.  So a mode-1 parent row v holds its non-loop
+// entries plus one v.  Its induced row, for distinct subset ids (a permutation slice), keeps the non-loop entries whose column
+// is in the subset, duplicates included, plus exactly one node_map[v] = local id of v: that is the mode-1 build of the
+// batch's `subgraph` edge list, whose loops (any number, or none) are dropped and replaced by one per row.  Missing or
+// duplicated loops in the parent's edge list therefore need no rule here; the sort restores the build's row order.  The
+// mode-1 dinv of an unweighted build is csr_dinv_kernel over the row lengths, loop included, which is the dinv computed below.
 static int subset_half(const int64_t* rowptr, const int32_t* col, int64_t n, const int64_t* subset, int64_t n_sub,
                        const int32_t* node_map, int64_t* out_rowptr, int32_t* out_col, int64_t out_col_capacity, float* dinv,
                        int64_t* out_needed, const CsrWs& w, cudaStream_t st) {

@@ -1257,6 +1257,23 @@ __global__ void __launch_bounds__(kRowBlock) softmax_nll_kernel(const float* __r
     grid_reduce_add(s_acc, 1, 1, 0, loss, red);
 }
 
+// Row argmax of xr[0..c) by one warp, the same in every lane: the first maximum on ties, as numpy/torch argmax (lane order,
+// then the lowest column among equal maxima).  Shared by the K11 kernels so that they resolve ties alike.
+__device__ __forceinline__ int warp_row_argmax(const float* __restrict__ xr, int c, int lane, float& best) {
+    best = -INFINITY;
+    int arg = c;
+    for (int j = lane; j < c; j += 32) {
+        const float v = xr[j];
+        if (v > best) { best = v; arg = j; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
+        if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+    }
+    return arg;
+}
+
 // K11 - evaluation on the device: accuracy (argmax == label) and summed NLL of log_softmax over the rows idx[0..m) (all rows if
 // idx is NULL).  Replaces eval_acc (reference large/data_utils.py:210-220: argmax -> D2H -> numpy loop) and the valid_loss of
 // evaluate() (large/eval.py:28-31) for single-column integer labels.  Ties: first maximum, as numpy/torch argmax.
@@ -1272,17 +1289,8 @@ __global__ void __launch_bounds__(kRowBlock) eval_acc_kernel(const float* __rest
         const int64_t r = idx ? idx[i] : i;
         if (r < 0 || r >= rows) continue;
         const float* xr = x + r * ldx;
-        float best = -INFINITY;
-        int arg = c;
-        for (int j = lane; j < c; j += 32) {
-            const float v = xr[j];
-            if (v > best) { best = v; arg = j; }
-        }
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
-            if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
-        }
+        float best;
+        const int arg = warp_row_argmax(xr, c, lane, best);
         const int64_t lab = y[r];
         if (lane == 0 && lab == arg) ++hit;
         if (nll_sum) {
@@ -1296,6 +1304,41 @@ __global__ void __launch_bounds__(kRowBlock) eval_acc_kernel(const float* __rest
         if (hit) atomicAdd(correct, hit);
         if (nll_sum && acc != 0.0) atomicAdd(nll_sum, acc);
     }
+}
+
+// K11 over the batches of a mini-batch evaluation epoch (large/eval.py:67-118 evaluate_batch): batch row i (logits row i) is node
+// r = idx[i] (i when idx is NULL); its split bits split[r] (1 train, 2 valid, 4 test) select the counters it adds to:
+// counts[2k] += 1 (rows of split k) and counts[2k + 1] += (argmax == labels[r]).  Integer sums only: per-warp registers, a
+// shared-memory sum per block, one atomicAdd per block and counter - the totals do not depend on the order of the adds.
+__global__ void __launch_bounds__(kRowBlock) eval_acc_splits_kernel(const float* __restrict__ x, int64_t ldx, int64_t m, int c,
+                                                                     const int64_t* __restrict__ y, const uint8_t* __restrict__ split,
+                                                                     const int64_t* __restrict__ idx, int64_t rows,
+                                                                     unsigned long long* __restrict__ counts) {
+    __shared__ unsigned long long s_cnt[6];
+    if (threadIdx.x < 6) s_cnt[threadIdx.x] = 0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    unsigned long long cnt[6] = {0, 0, 0, 0, 0, 0};
+    for (int64_t i = warp; i < m; i += nwarps) {
+        const int64_t r = idx ? idx[i] : i;
+        if (r < 0 || r >= rows) continue;
+        const unsigned bits = split[r];
+        if (!(bits & 7u)) continue;
+        float best;
+        const int arg = warp_row_argmax(x + i * ldx, c, lane, best);
+        const unsigned hit = y[r] == arg;
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+            if (bits & (1u << k)) { cnt[2 * k] += 1; cnt[2 * k + 1] += hit; }
+    }
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+            if (cnt[k]) atomicAdd(&s_cnt[k], cnt[k]);
+    __syncthreads();
+    if (threadIdx.x < 6 && s_cnt[threadIdx.x]) atomicAdd(&counts[threadIdx.x], s_cnt[threadIdx.x]);
 }
 
 }  // namespace sgf
@@ -1810,6 +1853,20 @@ extern "C" int sgf_eval_acc(const float* logits, int64_t ld, const int64_t* labe
     if (blocks > cap) blocks = cap;
     eval_acc_kernel<<<(unsigned)blocks, kRowBlock, 0, st>>>(logits, ld, labels, idx, m, rows, c,
                                                             reinterpret_cast<unsigned long long*>(correct), nll_sum);
+    SGF_LAUNCH_CHECK(); count_launch();
+    return SGF_OK;
+}
+
+extern "C" int sgf_eval_acc_splits(const float* logits, int64_t ld, int64_t m, int c, const int64_t* labels, const uint8_t* split,
+                                   const int64_t* idx, int64_t rows, int64_t* counts, void* stream) {
+    if (m < 0 || rows < 0 || c <= 0 || !counts || (m > 0 && (!logits || !labels || !split)) || ld < c || (!idx && m > rows))
+        return SGF_ERR_ARG;
+    if (m == 0) return SGF_OK;
+    int64_t blocks = (m * 32 + kRowBlock - 1) / kRowBlock;
+    int64_t cap = (int64_t)num_sms() * 8;
+    if (blocks > cap) blocks = cap;
+    eval_acc_splits_kernel<<<(unsigned)blocks, kRowBlock, 0, (cudaStream_t)stream>>>(
+        logits, ld, m, c, labels, split, idx, rows, reinterpret_cast<unsigned long long*>(counts));
     SGF_LAUNCH_CHECK(); count_launch();
     return SGF_OK;
 }

@@ -58,9 +58,9 @@ class Graph:
         return int(self.rowptr[-1].item())
 
     @classmethod
-    def _from_parts(cls, n, rowptr, col, dinv, transpose_same: bool):
+    def _from_parts(cls, n, rowptr, col, dinv, transpose_same: bool, self_loop_mode: int = 0):
         g = cls.__new__(cls)
-        g.n, g.rows, g.self_loop_mode, g.edge_index, g.col_rot = int(n), None, 0, None, None
+        g.n, g.rows, g.self_loop_mode, g.edge_index, g.col_rot = int(n), None, self_loop_mode, None, None
         g.edge_weight = g.val = g.eid = g.val_t = g.eid_t = None
         g.rowptr, g.col, g.dinv = rowptr, col, dinv
         g.heavy = g.heavy_t = None       # batch subgraphs: no per-batch sync for a hub plan
@@ -72,7 +72,8 @@ class Graph:
         O(sum of the selected rows' lengths) — the mini-batch structure of large/main-batch.py:136-139 without the per-batch
         O(E) PyG `subgraph` mask and without a CSR rebuild.  On a symmetric edge set (checked once per graph) the subset's
         transpose shares its storage; on a directed one the subset of the transposed CSR is built beside it on the same local
-        ids (`nnz_needed_t` is its induced nnz)."""
+        ids (`nnz_needed_t` is its induced nnz).  The subset keeps this graph's self_loop_mode: in mode 1 it equals
+        Graph(subgraph(edge_index, idx), b, self_loop_mode=1), one self loop per row (see csr.cu, subset_half)."""
         if self.rows is not None:
             raise ValueError("subset() needs the full (unsharded) graph")
         if self.val is not None:
@@ -82,12 +83,12 @@ class Graph:
             self._symmetric = self.transpose()[0] is self.rowptr
         if self._symmetric:
             rp, cl, dv, needed = K.csr_subset(self.rowptr, self.col, self.n, idx, self._node_map, capacity)
-            g = Graph._from_parts(idx.numel(), rp, cl, dv, True)
+            g = Graph._from_parts(idx.numel(), rp, cl, dv, True, self.self_loop_mode)
             g.nnz_needed_t = needed
         else:
             rp, cl, dv, needed, rp_t, cl_t, needed_t = K.csr_subset(self.rowptr, self.col, self.n, idx, self._node_map, capacity,
                                                                     transposed=self._t)
-            g = Graph._from_parts(idx.numel(), rp, cl, dv, False)
+            g = Graph._from_parts(idx.numel(), rp, cl, dv, False, self.self_loop_mode)
             g._t, g.nnz_needed_t = (rp_t, cl_t), needed_t
         g.nnz_needed, g.capacity = needed, capacity      # device int64 [1]: > capacity means the batch structure was truncated
         return g

@@ -1455,5 +1455,35 @@ def eval_acc(logits: Tensor, labels: Tensor, idx: Optional[Tensor] = None, want_
     return acc, (float(nll.item()) / m if want_loss and m else None)
 
 
+SPLIT_TRAIN, SPLIT_VALID, SPLIT_TEST = 1, 2, 4      # bits of the split codes of eval_acc_splits
+
+
+def eval_acc_splits(logits: Tensor, labels: Tensor, split: Tensor, idx: Optional[Tensor], counts: Tensor) -> Tensor:
+    """K11 over one mini-batch: adds into `counts` (device int64 [6], zeroed by the caller once per epoch) the rows of each split
+    and their argmax hits, [train rows, train hits, valid rows, valid hits, test rows, test hits].  Logits row i is node idx[i]
+    (row i if idx is None); `labels` (int64) and `split` (uint8 bit codes SPLIT_*) have one entry per node.  No sync."""
+    _use(logits)
+    if logits.dtype != torch.float32:
+        raise TypeError("eval_acc_splits expects fp32 logits")
+    m, c, ld = _mat(logits, "logits")
+    for name, t in (("labels", labels), ("split", split), ("idx", idx), ("counts", counts)):
+        if t is not None and t.device != logits.device:
+            raise ValueError(f"eval_acc_splits: {name} must be on the logits' device {logits.device}, not {t.device}")
+    labels = labels.reshape(-1)
+    if labels.dtype != torch.int64 or split.dtype != torch.uint8 or split.dim() != 1 or labels.numel() != split.numel():
+        raise ValueError("eval_acc_splits: labels must be int64 and split uint8, one entry per node")
+    if not (labels.is_contiguous() and split.is_contiguous()):
+        raise ValueError("eval_acc_splits: labels and split must be contiguous")
+    if counts.dtype != torch.int64 or counts.numel() != 6 or not counts.is_contiguous():
+        raise ValueError("eval_acc_splits: counts must be a contiguous int64 [6]")
+    if idx is not None:
+        idx = idx.reshape(-1)
+        if idx.dtype != torch.int64 or not idx.is_contiguous() or idx.numel() != m:
+            raise ValueError("eval_acc_splits: idx must be a contiguous int64 with one entry per logits row")
+    check(lib().sgf_eval_acc_splits(_p(logits), ld, m, c, _p(labels), _p(split), _p(idx), labels.numel(), _p(counts), _stream()),
+          "sgf_eval_acc_splits")
+    return counts
+
+
 def launch_count() -> int:
     return int(lib().sgf_launch_count())

@@ -11,7 +11,7 @@ from . import engine as E
 from . import functional as Fn
 from .config import make_config
 from .dist import SINGLE
-from .graph import get_graph
+from .graph import Graph, get_graph
 from .modules import SGFormerBase, TransConvBase, TransConvLayerBase, _Base, full_attention_conv
 
 # GAT / GATConv / GCNJK stay out of __all__: the medium drop-in star-imports this module after the reference's `models`, and a star
@@ -243,11 +243,12 @@ class GAT(_Base):
         return self._run(x, edge_index)
 
     def _run(self, x, edge_index, names=None, tensors=None):
-        """The stack on CUDA x / edge_index; (names, tensors) default to this module's own (large_gnns.GAT passes device copies)."""
+        """The stack on CUDA x / edge_index (or a prebuilt self_loop_mode 1 Graph, from large_gnns.GAT); (names, tensors) default
+        to this module's own (large_gnns.GAT passes device copies)."""
         if names is None:
             names, tensors = _gat_flat(self, "")
         cfg = make_config("medium", x.shape[1], self.convs[0].lin_src.weight.shape[0], self.convs[-1].out_channels, **self._cfg_kw())
-        graph = get_graph(edge_index, x.shape[0], 1)
+        graph = edge_index if isinstance(edge_index, Graph) else get_graph(edge_index, x.shape[0], 1)
         return Fn.GraphBranchFn.apply(x, graph, cfg, E.precision(self.precision), self.training, "gat", "", names, *tensors)
 
 
