@@ -58,6 +58,9 @@ int sgf_set_device(int device);
  * dinv (nullable, by_source = 0 only): dinv[i] = sqrt(1/len(row i)) or 0 for empty rows
  * (== (1/d).sqrt() with nan_to_num -> 0, large/ours.py:29-32).
  * col must hold nnz (+ n when self_loop_mode = 1) entries; the true count is rowptr[n].
+ * Every node id of edge_index must lie in [0, n) (n_cols for the row shard below): an id outside it is the caller's error.
+ * The kernels skip such an edge, so rowptr[n] falls short of nnz and col's tail is left unwritten; kernels.csr_build,
+ * csr_build_weighted and to_undirected refuse such an edge list with a ValueError before they launch.
  * ------------------------------------------------------------------------------------------------ */
 int sgf_csr_build_ws_bytes(int64_t nnz, int64_t n, size_t* bytes /* host out */);
 int sgf_csr_build(const int64_t* edge_index /* [2,nnz] */, int64_t nnz, int64_t n, int by_source,

@@ -97,6 +97,16 @@ def new_like(x: Tensor) -> Tensor:
 # ------------------------------------------------------------------------------------------------
 # graph structure
 # ------------------------------------------------------------------------------------------------
+def _check_node_ids(ei: Tensor, n: int):
+    """Refuse node ids outside [0, n): the build kernels would skip such an edge and build a different graph (one aminmax, one
+    device sync; graph-build time)."""
+    if ei.shape[1] == 0:
+        return
+    lo, hi = torch.stack(torch.aminmax(ei)).tolist()
+    if lo < 0 or hi >= n:
+        raise ValueError(f"edge_index holds node ids in [{lo}, {hi}], outside [0, n={n})")
+
+
 def csr_build(edge_index: Tensor, n: int, by_source: bool = False, self_loop_mode: int = 0, want_dinv: bool = True,
               rows: Optional[Tuple[int, int]] = None, col_rot: Optional[Tuple[int, int]] = None):
     """-> (rowptr int64 [n_rows+1], col int32 [nnz'], dinv fp32 [n_rows] | None).  See sgf_csr_build(_rect).
@@ -106,6 +116,7 @@ def csr_build(edge_index: Tensor, n: int, by_source: bool = False, self_loop_mod
     if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
         raise ValueError("edge_index must be int64 [2, nnz]")
     ei = edge_index.contiguous()
+    _check_node_ids(ei, n)
     nnz = ei.shape[1]
     dev = ei.device
     r0, r1 = rows if rows is not None else (0, n)
@@ -146,6 +157,7 @@ def csr_build_weighted(edge_index: Tensor, edge_weight: Tensor, n: int, by_sourc
     if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
         raise ValueError("edge_index must be int64 [2, nnz]")
     ei = edge_index.contiguous()
+    _check_node_ids(ei, n)
     nnz = ei.shape[1]
     w = edge_weight_vec(edge_weight, nnz)
     dev = ei.device
@@ -237,6 +249,7 @@ def edge_symmetry(edge_index: Tensor, n: int) -> bool:
 def to_undirected(edge_index: Tensor, n: int) -> Tensor:
     """K10: PyG to_undirected = every edge in both directions, sorted by (row, col), duplicates removed (bit-exact)."""
     ei = _edge_index(edge_index)
+    _check_node_ids(ei, n)
     nnz, dev = ei.shape[1], ei.device
     out = torch.empty((2, max(2 * nnz, 1)), dtype=torch.int64, device=dev)
     count = torch.zeros(1, dtype=torch.int64, device=dev)
