@@ -156,6 +156,38 @@ int sgf_csr_subset_pair(const int64_t* rowptr, const int32_t* col, const int64_t
                         float* dinv /* [n_sub] or NULL */, int64_t* out_needed, int64_t* out_needed_t, void* ws, size_t ws_bytes,
                         void* stream);
 
+/* K11 — neighbour sampling (replaces PyG NeighborLoader(num_neighbors=[15, 10, 5], batch_size=1000) of 100M/nb-sample.py:125-150
+ * with replace=False, disjoint=False; DESIGN.md §4.15).  Rows of the parent CSR (sgf_csr_build by_source = 0: rows = edge targets,
+ * entries = sources) are sampled hop by hop; the batch's nodes get local ids in order of first appearance ordered by (hop, position
+ * of the target in the frontier, slot), seeds first.  Buffers are sized by static bounds (batch_cap = B, hop t's frontier capacity
+ * F_0 = B, F_{t+1} = F_t * width_t, width_t = k_t or, for k_t = -1, the caller's row capacity; max_nodes = B + sum F_t width_t,
+ * max_edges = sum F_t width_t), so no launcher reads a size back.  bounds: device int64 [hops + 2], bounds[t] = first local id
+ * of hop t's frontier (bounds[hops + 1] = node count).  node_map: int32 [n] that holds -1 everywhere between batches.
+ * sgf_neighbor_begin: idx[0:b] = seeds (distinct ids in [0, n)), node_map[seeds[i]] = i, bounds[0..1] = (0, b), rowlen = 0.
+ * sgf_neighbor_sample_hop: hop `hop` (bounds points at bounds[hop]): frontier row i (node v = idx[bounds[0] + i]) draws
+ *   min(k, deg v) distinct entry positions of its row (Floyd's algorithm on draws fmix64(fmix64(seed ^ v*phi) ^ (hop<<32 | d)*c),
+ *   see sample.cu), or takes its first min(deg, width) entries when k = -1 (deg > width: *need = max(*need, deg), nullable), and
+ *   writes their source ids in ascending entry position to cand[i*width ..] and the count to rowlen[bounds[0] + i].
+ * sgf_neighbor_relabel: the new nodes of the hop (bounds at bounds[hop]) take local ids from bounds[1] on in key order
+ *   (key = key_base + slot, key_base = B + the slots of the earlier hops; key_base + slots < 2^31), idx[local] = global id,
+ *   bounds[2] = bounds[1] + their count, and cand is rewritten to local ids.
+ * sgf_neighbor_edges: edge_index [2, max_edges] (pitch max_edges) gets one edge (source local, target local) per drawn slot of all
+ *   `hops` (cand = every hop's slots back to back, widths host [hops]), ordered by (target, slot), then the padding edges
+ *   (max_nodes + p, max_nodes + p) up to max_edges, so that sgf_csr_build(n = max_nodes + max_edges) of the whole list equals
+ *   the build of the real edges on their first max_nodes rows; node_map is reset to -1; counts[0..1] = (nodes, edges).
+ * ws: sgf_neighbor_sample_ws_bytes(largest hop's F_t * width_t, max_nodes) bytes, shared by relabel and edges in stream order. */
+int sgf_neighbor_sample_ws_bytes(int64_t max_slots, int64_t max_nodes, size_t* bytes /* host out */);
+int sgf_neighbor_begin(const int64_t* seeds, int64_t b, int32_t* node_map, int64_t* idx /* [max_nodes] */, int64_t* bounds,
+                       int32_t* rowlen /* [max_nodes] */, int64_t max_nodes, void* stream);
+int sgf_neighbor_sample_hop(const int64_t* rowptr, const int32_t* col, const int64_t* idx, const int64_t* bounds, int64_t frontier_cap,
+                            int k, int width, int hop, uint64_t seed, int32_t* cand /* [frontier_cap * width] */, int32_t* rowlen,
+                            int64_t* need, void* stream);
+int sgf_neighbor_relabel(int32_t* cand, const int32_t* rowlen, int64_t* bounds, int64_t frontier_cap, int width, int64_t key_base,
+                         int64_t max_nodes, int32_t* node_map, int64_t* idx, void* ws, size_t ws_bytes, void* stream);
+int sgf_neighbor_edges(const int32_t* cand, const int32_t* widths /* host [hops] */, int hops, int64_t batch_cap, const int64_t* bounds,
+                       const int32_t* rowlen, int64_t max_nodes, int32_t* node_map, const int64_t* idx, int64_t* edge_index,
+                       int64_t max_edges, int64_t* counts /* [2] */, void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * K6 / K7 — CSR SpMM (replaces torch_sparse.matmul(adj, x), large/ours.py:34, 100M/ours.py:80, and its
  * autograd transpose):  y[r,:] = row_scale[r] * sum_{j in row r} x[col[j], :]   (row_scale nullable).

@@ -176,6 +176,11 @@ _SIGS = {
     "sgf_csr_subset": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "sgf_csr_subset_pair": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz,
                                       _vp]),
+    "sgf_neighbor_sample_ws_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
+    "sgf_neighbor_begin": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "sgf_neighbor_sample_hop": (C.c_int, [_vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int, _u64, _vp, _vp, _vp, _vp]),
+    "sgf_neighbor_relabel": (C.c_int, [_vp, _vp, _vp, _i64, C.c_int, _i64, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "sgf_neighbor_edges": (C.c_int, [_vp, C.POINTER(_i32), C.c_int, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _sz, _vp]),
     "sgf_eval_acc": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, C.c_int, _vp, _vp, _vp]),
     "sgf_eval_acc_splits": (C.c_int, [_vp, _i64, _i64, C.c_int, _vp, _vp, _vp, _i64, _vp, _vp]),
     "sgf_softmax_nll": (C.c_int, [_vp, _i64, _vp, _vp, _i64, C.c_int, _f32, _vp, _vp, _i64, _vp, _sz, _vp]),

@@ -332,6 +332,124 @@ def csr_subset(rowptr: Tensor, col: Tensor, n: int, subset: Tensor, node_map: Te
     return out_rowptr, out_col, dinv[:b], needed, out_rowptr_t, out_col_t, needed_t
 
 
+@dataclass(frozen=True)
+class NeighborPlan:
+    """Static buffer bounds of one neighbour-sampled batch (see neighbor_sample_plan)."""
+    batch_cap: int
+    ks: Tuple[int, ...]               # fan-out per hop (-1: every entry)
+    widths: Tuple[int, ...]           # slots per frontier row per hop: k, or the row capacity for k = -1
+    frontier_caps: Tuple[int, ...]    # F_0 = batch_cap, F_{t+1} = F_t * width_t
+    max_nodes: int                    # batch_cap + sum F_t width_t
+    max_edges: int                    # sum F_t width_t
+
+    @property
+    def slot_offsets(self) -> Tuple[int, ...]:
+        out, o = [], 0
+        for f, w in zip(self.frontier_caps, self.widths):
+            out.append(o)
+            o += f * w
+        return tuple(out)
+
+
+def neighbor_sample_plan(batch_size: int, num_neighbors: Sequence[int], capacity: Optional[int] = None) -> NeighborPlan:
+    """The static bounds B(1 + k_0 + k_0 k_1 + ...) nodes and B(k_0 + k_0 k_1 + ...) edges of a batch of `batch_size` seeds; a hop
+    with k = -1 takes at most `capacity` entries per row (required then)."""
+    ks = tuple(int(k) for k in num_neighbors)
+    if any(k < -1 for k in ks):
+        raise ValueError(f"num_neighbors must hold fan-outs >= 0 or -1, got {list(ks)}")
+    if -1 in ks and (capacity is None or int(capacity) < 1):
+        raise ValueError("num_neighbors holds -1 (every neighbour): pass capacity = the largest row length a batch may take")
+    widths = tuple(k if k >= 0 else int(capacity) for k in ks)
+    caps, f = [], int(batch_size)
+    for w in widths:
+        caps.append(f)
+        f *= w
+    max_edges = sum(c * w for c, w in zip(caps, widths))
+    max_nodes = int(batch_size) + max_edges
+    if max_nodes >= 2 ** 31:
+        raise ValueError(f"a batch of {batch_size} seeds at fan-outs {list(ks)} may hold {max_nodes} nodes: the sampler's int32 "
+                         "keys need fewer than 2^31; lower batch_size, the fan-outs or capacity")
+    return NeighborPlan(int(batch_size), ks, widths, tuple(caps), max_nodes, max_edges)
+
+
+def _ns_ws(plan: NeighborPlan, dev) -> Tuple[Tensor, int]:
+    nbytes = C.c_size_t(0)
+    max_slots = max([f * w for f, w in zip(plan.frontier_caps, plan.widths)] + [0])
+    check(lib().sgf_neighbor_sample_ws_bytes(max_slots, plan.max_nodes, C.byref(nbytes)), "sgf_neighbor_sample_ws_bytes")
+    return torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev), nbytes.value
+
+
+def neighbor_sample_hop(rowptr: Tensor, col: Tensor, idx: Tensor, bounds: Tensor, plan: NeighborPlan, hop: int, seed: int,
+                        cand: Tensor, rowlen: Tensor, need: Optional[Tensor] = None):
+    """Hop `hop`'s draws into `cand` (the hop's [F_t * width_t] int32 slots, global source ids) and rowlen (sgf_neighbor_sample_hop)."""
+    check(lib().sgf_neighbor_sample_hop(_p(rowptr), _p(col), _p(idx), _p(bounds[hop:]), plan.frontier_caps[hop], plan.ks[hop],
+                                        plan.widths[hop], hop, seed, _p(cand), _p(rowlen), _p(need), _stream()),
+          "sgf_neighbor_sample_hop")
+
+
+def neighbor_sample_relabel(cand: Tensor, rowlen: Tensor, bounds: Tensor, plan: NeighborPlan, hop: int, node_map: Tensor, idx: Tensor,
+                            ws: Tensor, ws_bytes: int):
+    """Local ids for hop `hop`'s new nodes, in key order; `cand` rewritten to local ids (sgf_neighbor_relabel)."""
+    key_base = plan.batch_cap + plan.slot_offsets[hop]
+    check(lib().sgf_neighbor_relabel(_p(cand), _p(rowlen), _p(bounds[hop:]), plan.frontier_caps[hop], plan.widths[hop], key_base,
+                                     plan.max_nodes, _p(node_map), _p(idx), _p(ws), ws_bytes, _stream()), "sgf_neighbor_relabel")
+
+
+def neighbor_sample_edges(cand: Tensor, plan: NeighborPlan, bounds: Tensor, rowlen: Tensor, node_map: Tensor, idx: Tensor,
+                          edge_index: Tensor, counts: Tensor, ws: Tensor, ws_bytes: int):
+    """The batch's padded edge list, the node map reset, counts = (nodes, edges) (sgf_neighbor_edges)."""
+    hops = len(plan.widths)
+    widths = (C.c_int32 * max(hops, 1))(*plan.widths)
+    check(lib().sgf_neighbor_edges(_p(cand), widths, hops, plan.batch_cap, _p(bounds), _p(rowlen), plan.max_nodes, _p(node_map),
+                                   _p(idx), _p(edge_index), plan.max_edges, _p(counts), _p(ws), ws_bytes, _stream()),
+          "sgf_neighbor_edges")
+
+
+def neighbor_sample(rowptr: Tensor, col: Tensor, node_map: Tensor, seeds: Tensor, plan: NeighborPlan, seed: int,
+                    need: Optional[Tensor] = None):
+    """One neighbour-sampled batch of `seeds` from the parent CSR (rowptr, col; rows = edge targets), without a host sync.
+    -> (idx int64 [max_nodes], edge_index int64 [2, max_edges], counts int64 [2] = (nodes b, edges e), rowptr, col, dinv,
+    rowptr_t, col_t): all device tensors at the plan's static sizes.  The first b entries of idx are the global ids in local order,
+    the first e columns of edge_index the edges (source local, target local); rowptr[:b+1], col[:e], dinv[:b] and
+    rowptr_t[:b+1], col_t[:e] equal Graph(edge_index[:, :e], b, 0) and its transpose (sgf_csr_build of the padded list)."""
+    _use(rowptr)
+    dev = rowptr.device
+    seeds = seeds.contiguous().to(torch.int64)
+    b = seeds.numel()
+    if b > plan.batch_cap:
+        raise ValueError(f"neighbor_sample: {b} seeds exceed the plan's batch_cap {plan.batch_cap}")
+    hops = len(plan.widths)
+    idx = torch.empty(max(plan.max_nodes, 1), dtype=torch.int64, device=dev)
+    rowlen = torch.empty(max(plan.max_nodes, 1), dtype=torch.int32, device=dev)
+    bounds = torch.empty(hops + 2, dtype=torch.int64, device=dev)
+    cand = torch.empty(max(plan.max_edges, 1), dtype=torch.int32, device=dev)
+    ei = torch.empty((2, max(plan.max_edges, 1)), dtype=torch.int64, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    ws, ws_bytes = _ns_ws(plan, dev)
+    check(lib().sgf_neighbor_begin(_p(seeds), b, _p(node_map), _p(idx), _p(bounds), _p(rowlen), plan.max_nodes, _stream()),
+          "sgf_neighbor_begin")
+    offs = plan.slot_offsets
+    for t in range(hops):
+        c = cand[offs[t]:]
+        neighbor_sample_hop(rowptr, col, idx, bounds, plan, t, seed, c, rowlen, need)
+        neighbor_sample_relabel(c, rowlen, bounds, plan, t, node_map, idx, ws, ws_bytes)
+    neighbor_sample_edges(cand, plan, bounds, rowlen, node_map, idx, ei, counts, ws, ws_bytes)
+    # both orientations by sgf_csr_build on the padded list: the padding edges are self loops on rows past max_nodes
+    n_build = plan.max_nodes + plan.max_edges
+    nbytes = C.c_size_t(0)
+    check(lib().sgf_csr_build_ws_bytes(plan.max_edges, n_build, C.byref(nbytes)), "sgf_csr_build_ws_bytes")
+    cws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+    out = []
+    for by_source in (0, 1):
+        rp = torch.empty(n_build + 1, dtype=torch.int64, device=dev)
+        cl = torch.empty(max(plan.max_edges, 1), dtype=torch.int32, device=dev)
+        dv = torch.empty(max(n_build, 1), dtype=torch.float32, device=dev) if by_source == 0 else None
+        check(lib().sgf_csr_build(_p(ei), plan.max_edges, n_build, by_source, 0, _p(rp), _p(cl), _p(dv), _p(cws), nbytes.value,
+                                  _stream()), "sgf_csr_build")
+        out += [rp, cl, dv]
+    return idx, ei, counts, out[0], out[1], out[2], out[3], out[4]
+
+
 HEAVY_ROW = 1024      # rows longer than this are processed in segments of HEAVY_ROW entries (hub rows of power-law graphs)
 
 
